@@ -18,7 +18,7 @@ sum_j w_j * noise_j, negate/clamp, Adam, post-update rollout.  Prints ONE JSON l
   extra                the other BASELINE.json configs through the same public API (short runs)
 
 `--impl reference` runs only the reference's CPU path (rank 0): the UNMODIFIED reference package from
-baseline/_ref (installed by __graft_entry__.build()) when present, else the CPU port of its cost
+oracle/_ref (installed by __graft_entry__.build()) when present, else the CPU port of its cost
 structure (oracle/reference_port.py); same metric/config.
 """
 import argparse
@@ -84,7 +84,8 @@ def load_peaks():
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], tensor_burst=p["bf16_tflops"], tensor=p["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16/FP16 TFLOP/s
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor=989.0, source="H100 SXM data sheet (not measured here)")
 
 
 class ClockSampler:
@@ -136,7 +137,7 @@ def _host_threads():
 def cpu_reference(wl, steps, warmup, budget_s=20.0):
     """Time the reference's CPU path for the workload on a bounded population sample and scale
     linearly in P (sample, cat, rollouts, mm are all O(P*n); SURVEY 8d).  Uses the unmodified
-    reference (baseline/_ref) when it is installed, else the CPU port of its cost structure."""
+    reference (oracle/_ref) when it is installed, else the CPU port of its cost structure."""
     from oracle.ref_shim import import_reference
     from oracle.reference_port import time_reference
     from estorch_b200.agents import DeviceAgent
@@ -178,7 +179,7 @@ def run_reference_arm(args, wl, rank, world):
     if rank != 0:
         return
     r = cpu_reference(wl, args.steps, min(args.warmup, 1), budget_s=60.0)
-    what = ("the UNMODIFIED reference package (baseline/_ref, estorch.ES.train(n_proc=1) through a one-rank mpi4py shim)"
+    what = ("the UNMODIFIED reference package (oracle/_ref, estorch.ES.train(n_proc=1) through a one-rank mpi4py shim)"
             if r["kind"] == "reference" else "CPU port of the reference's cost structure (oracle/reference_port.py)")
     cb = {"value": r["value"], "unit": "generations/s", "cores": r["cores"], "kind": r["kind"],
           "sample_P": r["sample_P"], "extrapolation_factor": r["extrapolation_factor"],
@@ -338,6 +339,9 @@ def run_ours(args, wl, rank, world, local_rank):
     sampler = ClockSampler(local_rank) if rank == 0 else None   # nvidia-smi needs ~1 s to start streaming
     ms, _, clocks, launches = timed_region(es, args.steps, args.warmup, world, dev, sampler)
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(es, args.dump_outputs)
+
     # ---- e2e: host buffers in, log() + host results out, every generation
     es.agent.stream_from_host, es.read_back, es._log_interval = True, True, 1
     _, e2e_s, _, _ = timed_region(es, args.steps, args.warmup, world, dev)
@@ -355,7 +359,7 @@ def run_ours(args, wl, rank, world, local_rank):
 
     extras = None
     # (single-GPU runs only: the scaling runs stay lean; the other configs at their named GPU counts are
-    #  recorded with `--workload NAME` under torchrun, see profiles/)
+    #  can be run with `--workload NAME` under torchrun)
     names = ()
     if args.extras:                       # explicit list: also under torchrun (the configs named for N GPUs)
         names = tuple(x for x in args.extras.split(",") if x)
@@ -372,7 +376,7 @@ def run_ours(args, wl, rank, world, local_rank):
             "unit": "generations/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None,
-            "dtype": {"f16": "f32 (fp32-equivalent: evaluate GEMMs on tcgen05 with fp16 operands = 11-bit significand, "
+            "dtype": {"f16": "f32 (fp32-equivalent: evaluate GEMMs on wgmma with fp16 operands = 11-bit significand, "
                              "TF32 class, each weight formed in fp32 from fp32 theta + the exactly-16-bit noise value and "
                              "rounded once, f32 accumulate, f32 bias/loss; f32 ranks, reduction, Adam)",
                       "bf16": "bf16 operands / f32 accumulate (evaluate GEMMs); f32 noise, ranks, reduction, Adam",
@@ -391,12 +395,25 @@ def run_ours(args, wl, rank, world, local_rank):
         line["cpu_baseline"] = {
             "value": r["value"], "unit": "generations/s", "cores": r["cores"], "kind": r["kind"],
             "sample_P": r["sample_P"], "extrapolation_factor": r["extrapolation_factor"],
-            "sample": f"1 generation of {'the unmodified reference (baseline/_ref)' if r['kind'] == 'reference' else 'the CPU port'} "
+            "sample": f"1 generation of {'the unmodified reference (oracle/_ref)' if r['kind'] == 'reference' else 'the CPU port'} "
                       f"at population_size={r['sample_P']} of {P}, scaled linearly in P; {r['cores']} torch threads of "
                       f"{os.cpu_count()} cpus; {r['seconds_per_generation_sample']:.2f} s/sample-generation"}
     if extras is not None:
         line["extra"] = extras
     emit(line)
+
+
+def dump_outputs(es, out_dir):
+    """What the timed path's last generation handed to its caller, as float32 .npy files: the returns of
+    every member (population_returns), the policy parameters after the update and the episode reward of
+    the post-update rollout.  The inputs are seeded, so two builds can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {"population_returns": np.asarray(es.population_returns, dtype=np.float32),
+              "theta": es._slots[0].theta.detach().float().cpu().numpy(),
+              "episode_reward": np.asarray([es.episode_reward], dtype=np.float32)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def kernel_rooflines(es, wl, args, world, rank, peaks):
@@ -448,24 +465,13 @@ def kernel_rooflines(es, wl, args, world, rank, peaks):
     bytes_grad = tbytes * n * pl + 28 * n + 8 * P
     bytes_eval = tbytes * n * pl + 4 * n + 4 * B * (dims[0] + dims[-1]) + 4 * P
     flops_eval = 2.0 * n * B * 2 * pl
-    # DRAM traffic per launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed
-    # `ncu --set full` capture of exactly these kernels / shapes on one GPU (profiles/ncu_traffic.json)
-    traffic = {}
-    if args.workload == "north_star" and world == 1:
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        except (OSError, ValueError):
-            traffic = {}
     kname_g = ("rank_grad_adam" if world == 1 else "rank_grad_xr_adam" if es.__dict__.get("_peer_ptrs") else
                "rank_grad") + ("_h" if tbytes == 2 else "")
-    tr_g = traffic.get(kname_g)
     k_grad = {"kernel": kname_g, "bound": "l2",
               "achieved": bytes_grad / t_grad / 1e6, "peak": peaks["hbm"], "unit": "GB/s",
               "frac": bytes_grad / t_grad / 1e6 / peaks["hbm"],
               "frac_algorithmic_vs_hbm": bytes_grad / t_grad / 1e6 / peaks["hbm"],
-              "frac_dram_vs_hbm": (tr_g / t_grad / 1e6 / peaks["hbm"]) if tr_g else None,
-              "ms": t_grad, "traffic": tr_g,
-              "traffic_source": "committed ncu capture (profiles/ncu_traffic.json)" if tr_g else None,
+              "ms": t_grad,
               "algorithmic_bytes": bytes_grad,
               "note": "algorithmic/HBM > 1 is L2 reuse: the rows of one generation overlap in the table and every CTA "
                       "walks the pairs in offset-sorted order, so the table is fetched from HBM about once per launch "
@@ -476,12 +482,11 @@ def kernel_rooflines(es, wl, args, world, rank, peaks):
               "peak": peaks["tensor_burst"], "peak_kind": "burst (the kernel is timed alone)", "unit": "TFLOP/s",
               "frac": flops_eval / t_eval / 1e9 / peaks["tensor_burst"],
               "frac_of_sustained_peak": flops_eval / t_eval / 1e9 / peaks["tensor"],
-              "ms": t_eval, "traffic": traffic.get(kname_e),
-              "traffic_source": "committed ncu capture (profiles/ncu_traffic.json)" if traffic.get(kname_e) else None,
+              "ms": t_eval,
               "algorithmic_bytes": bytes_eval, "flops": flops_eval,
               "hbm_frac_of_noise_stream": bytes_eval / t_eval / 1e6 / peaks["hbm"]}
     dominant = k_eval if t_eval >= t_grad else k_grad
-    roofline = {k: dominant.get(k) for k in ("bound", "achieved", "peak", "unit", "frac", "traffic")}
+    roofline = {k: dominant.get(k) for k in ("bound", "achieved", "peak", "unit", "frac")}
     roofline["kernel"] = dominant["kernel"]
     roofline["peak_source"] = peaks["source"] + (", bf16 burst" if dominant is k_eval else "")
     return {"roofline": roofline, "kernels": [k_grad, k_eval]}
@@ -511,6 +516,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the short runs of the other BASELINE configs")
     ap.add_argument("--extras", default="", help="comma list of other workloads to run in the same process (any N)")
     ap.add_argument("--eval-precision", default="auto", choices=["auto", "fp32", "f16", "bf16", "bf16s"])
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last generation's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     # >= 5 warm-up generations on our arm: a generation configuration is captured into a CUDA graph at its third
     # sighting, so the capture (tens of ms) happens in the warm-up, never inside the timed region

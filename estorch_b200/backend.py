@@ -66,7 +66,7 @@ class CudaBackend:
 
     def __init__(self, device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("estorch_b200 needs a CUDA device (B200, sm_100a); "
+            raise RuntimeError("estorch_b200 needs a CUDA device (H100, sm_90a); "
                                "torch.cuda.is_available() is False and there is no CPU fallback")
         self.lib = _capi.load()
         if device is None:

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Build libestk.so in-tree for sm_100a (B200).  nvcc cross-compiles without a GPU.
+# Build libestk.so in-tree for sm_90a (H100).  nvcc cross-compiles without a GPU.
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 ROOT="$(cd "$HERE/../.." && pwd)"
@@ -11,7 +11,7 @@ OBJDIR="$OUT${VARIANT:+/obj_$VARIANT}"
 LIBNAME="libestk${VARIANT:+_$VARIANT}.so"
 mkdir -p "$OUT" "$OBJDIR"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -I"$ROOT/include"
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -I"$ROOT/include"
        -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --cudart static)
 OBJS=()
 for src in "$HERE"/*.cu; do
@@ -21,5 +21,5 @@ for src in "$HERE"/*.cu; do
   fi
   OBJS+=("$obj")
 done
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -shared --cudart static -o "$OUT/$LIBNAME" "${OBJS[@]}"
+"$NVCC" -gencode arch=compute_90a,code=sm_90a -shared --cudart static -o "$OUT/$LIBNAME" "${OBJS[@]}"
 echo "built $OUT/$LIBNAME"

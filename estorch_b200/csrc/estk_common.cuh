@@ -1,4 +1,4 @@
-// estk_common.cuh -- shared host/device helpers for libestk (sm_100a only).
+// estk_common.cuh -- shared host/device helpers for libestk (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 #include <stdarg.h>
 #include "estk.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libestk is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libestk is written for sm_90a (H100) only"
 #endif
 
 // ---------------------------------------------------------------- errors
@@ -41,14 +41,11 @@ struct estk_ctx {
   int max_grid;            // sm_count * 8: upper bound on any persistent grid
   float* cvals;            // [ESTK_MAX_POPULATION] blended centred ranks (fp32)
   float* partial;          // [max_grid * 1024] split-over-pairs partial sums
-  float* eval_partial;     // [ESTK_MAX_POPULATION * kEvalMaxChunks] loss partials
+  float* eval_partial;     // [ESTK_MAX_POPULATION * 2 * kEvalMaxChunks] loss partials
   unsigned int* counters;  // [ESTK_MAX_POPULATION + 8] self-resetting arrival counters (+ kernel tickets)
   double* scalars;         // [8] small fp64 scratch (||archive||_F, ...)
-  void* obs_image;         // [kObsImageBytes] fp16 hi/lo image of the observation batch, laid out as the
-                           // evaluate kernel's layer-0 shared-memory operand (estk_eval_mlp_f16.cu)
 };
-static const int kEvalMaxChunks = 64;
-static const size_t kObsImageBytes = (size_t)kEvalMaxChunks * 8 * 16384;   // 128-row blocks x 8 k-blocks x 16 KB
+static const int kEvalMaxChunks = 64;   // the tensor-core evaluate writes up to 2 * kEvalMaxChunks partials per member
 
 // ---------------------------------------------------------------- hashing
 // splitmix64 finaliser; must stay in lock-step with oracle/es_oracle.py:mix64
@@ -81,16 +78,9 @@ __device__ __forceinline__ uint4 ld_noise4h(const uint4* p) {
                : "l"(p));
   return v;
 }
-// two fp32 FMAs in one instruction (sm_100 FFMA2): d = a * b + c, element-wise
+// d = a * b + c, element-wise (two IEEE fp32 fmas)
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1,%2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1,%2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1,%2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0,%1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 __device__ __forceinline__ float ld_noise1(const float* p) {
   float v;

@@ -24,8 +24,8 @@ extern "C" int estk_ctx_create(int device, estk_ctx** out) {
   ESTK_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   ESTK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    estk_set_error("libestk is built for sm_100a (B200); device %d is sm_%d%d", device, prop.major,
+  if (prop.major != 9) {
+    estk_set_error("libestk is built for sm_90a (H100); device %d is sm_%d%d", device, prop.major,
                    prop.minor);
     return ESTK_ERR_UNSUPPORTED;
   }
@@ -41,10 +41,9 @@ extern "C" int estk_ctx_create(int device, estk_ctx** out) {
   if (e == cudaSuccess) e = cudaMalloc(&c->cvals, sizeof(float) * ESTK_MAX_POPULATION);
   if (e == cudaSuccess) e = cudaMalloc(&c->partial, sizeof(float) * (size_t)c->max_grid * 1024);
   if (e == cudaSuccess)
-    e = cudaMalloc(&c->eval_partial, sizeof(float) * (size_t)ESTK_MAX_POPULATION * kEvalMaxChunks);
+    e = cudaMalloc(&c->eval_partial, sizeof(float) * (size_t)ESTK_MAX_POPULATION * 2 * kEvalMaxChunks);
   if (e == cudaSuccess) e = cudaMalloc(&c->counters, sizeof(unsigned int) * (ESTK_MAX_POPULATION + 8));
   if (e == cudaSuccess) e = cudaMalloc(&c->scalars, sizeof(double) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&c->obs_image, kObsImageBytes);
   if (e == cudaSuccess) e = cudaMemset(c->counters, 0, sizeof(unsigned int) * (ESTK_MAX_POPULATION + 8));
   if (e != cudaSuccess) {
     estk_set_error("estk_ctx_create: workspace allocation failed: %s", cudaGetErrorString(e));
@@ -62,7 +61,6 @@ extern "C" int estk_ctx_destroy(estk_ctx* c) {
   cudaFree(c->eval_partial);
   cudaFree(c->counters);
   cudaFree(c->scalars);
-  cudaFree(c->obs_image);
   delete c;
   return ESTK_OK;
 }

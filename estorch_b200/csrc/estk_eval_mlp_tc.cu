@@ -1,111 +1,71 @@
-// estk_eval_mlp_tc.cu -- kernel 1 of the ES generation on the 5th-gen tensor
-// cores (tcgen05 + TMEM), bf16 operands / fp32 accumulation.
+// estk_eval_mlp_tc.cu -- kernel 1 of the ES generation (population evaluate) on the Hopper
+// tensor cores: warpgroup MMA (wgmma), 16-bit operands / fp32 accumulation.
 //
 // Same contract as estk_eval_mlp (estk_eval_mlp.cu; reference estorch.py:187-202 +
 // Policy.forward examples/cartpole_es.py:14-20 + synthetic agent of SURVEY 8d),
 // for policies whose dense layers are worth a GEMM.
 //
-// Work unit ("task") = (antithetic pair j, sign s, chunk of 128*CG observations),
-// executed by a cluster of CG CTAs (CG = 2: one tcgen05.mma.cta_group::2 pair,
-// UMMA M = 256).  Per layer  D[obs, out] = H[obs, in] * W_s[out, in]^T :
-//   A operand  activations H, 128 observation rows per CTA, bf16, K-major,
-//              128B-swizzled, RESIDENT in shared memory across layers (in place);
-//   B operand  W_s = theta + s*sigma*eps, formed ON THE FLY into a ring of
-//              [N/CG x 64] tiles -- the perturbed weights never exist in global
-//              memory; each CTA of the pair forms its half of N.
-//              bf16 shadow sources ("bf16s"): the TMA engine drops the theta tile
-//              into the free ring slot already in the swizzled operand layout
-//              (cuTensorMapEncodeTiled, SWIZZLE_128B); a producer group streams the
-//              pair's noise row with 128-bit loads and turns the slot into
-//              theta + s*sigma*eps in place (ld.shared, fma.rn.bf16x2, st.shared).
-//              fp32 sources ("bf16"): theta and noise both through registers,
-//              one FMA, cvt.rn.bf16x2, 16-byte swizzled st.shared;
-//   D          the WHOLE layer output [128 x <=512] fp32 lives in TMEM (512
-//              columns) as two N tiles.  Tile 0 is drained while tile 1's MMAs
-//              still run: bias, ReLU, bf16, parked as packed pairs in the TMEM
-//              columns its own drain has freed (the activations in smem are still
-//              being read).  When the layer is accumulated the parked half moves
-//              to smem (k-blocks 0..3, first hand-over), then tile 1 is drained
-//              straight into k-blocks 4..7 (second hand-over) under the next
-//              layer's first MMAs.  The last layer is fused with the squared-error
-//              reduction instead.
-// Warp roles per CTA: w0 MMA issuer (leader CTA only), w1 TMEM allocator + theta-tile
-// TMA thread, w2-5 epilogue (TMEM lane quarter = warp % 4), w6-13 weight producers
-// (bf16s: 4 groups of 2 warps; fp32 sources: 2 groups of 4).
-// Pipelines: full/empty (+ tma) mbarriers on the B ring, acc0 / acc (first tile / layer
-// accumulated), h_ready (next layer's activations in place).  Persistent: clusters
-// loop over tasks; the two signs of a pair run on neighbouring clusters at the same
-// time, so the second read of the noise row is an L2 hit.
-//
-// Roofline: 2*n*B*2*pairs flops per launch on the tensor pipe; the noise stream
-// 4*n*pairs bytes (2*n*pairs from the bf16 shadow) is read once from HBM (second sign
-// from L2).  Measured and rejected (profiles/README.md): L2 bulk-prefetch warp, 2-k-block
-// ring stages, register-pipelined producer refill, 8 epilogue + 6 producer warps,
-// 16-column double-buffered TMEM drains, bias fetched a layer ahead / by a 15th warp.
+// Work unit ("task") = (antithetic pair j, sign s, chunk of 64 observations), one CTA.  Per layer
+//   D[obs, out] = H[obs, in] * W_s[out, in]^T       (wgmma m64n128k16, N tiles of 128)
+//   A  activations H, 64 rows, 16-bit, K-major, 128B-swizzled, resident in shared memory:
+//      two buffers (64 KB each) swapped per layer, so a layer's output never overwrites its input;
+//   B  W_s = theta + s*sigma*eps, formed ON THE FLY by producer warps into a ring of
+//      [128 x 64] stages (16 KB) -- the perturbed weights never exist in global memory;
+//   D  64 x 128 fp32 in the registers of the consumer warpgroup; the epilogue adds the bias,
+//      applies ReLU and rounds to 16 bits straight into the other activation buffer.  The last
+//      layer is fused with the squared-error reduction (and the behaviour characterisation).
+// Operand modes (template MODE):
+//   kModeBF16   bf16 operands formed from fp32 theta + fp32 table (one FMA in fp32, one rounding)
+//   kModeBF16S  bf16 operands formed from bf16 shadows of theta and table (fma.rn.bf16x2)
+//   kModeF16    fp16 operands (11-bit significand, the TF32 class) from fp32 theta and the EXACT
+//               16-bit copy of the noise table: W16 = rn_f16(theta + s*sigma*eps), sum in fp32; the
+//               observations enter layer 0 as x_hi + x_lo (two fp16 k-block sets, same B tile)
+// Warp roles: warpgroup 0 = consumer (MMA issue + epilogue), warps 4..11 = weight producers in
+// two groups of four, each group forming every other stage of the flattened
+// (task, layer, N tile, k-block) sequence.  full / empty mbarriers per ring stage.  Persistent:
+// CTAs loop over tasks; the two signs of a pair run on neighbouring CTAs at the same time, so
+// the second read of the noise row is an L2 hit.
 #include "estk_tc.cuh"
-#include <stdlib.h>
-#include <string.h>
-
-// Triage instrumentation (role cycle counters, ESTK_TC_DEBUG switches) exists only in builds made with
-// -DESTK_TC_PROFILE (ESTK_VARIANT=prof); the product library has no debug globals and reads no environment.
-#ifdef ESTK_TC_PROFILE
-__device__ unsigned long long g_tc_prof[32];   // ESTK_TC_DEBUG bit 8: per-role cycle counters of cluster 0 / CTA 0
-#define TC_PROF_ATOMIC(i, v) atomicAdd(&g_tc_prof[i], (unsigned long long)(v))
-#define TC_PROF_ENABLED 1
-#else
-#define TC_PROF_ATOMIC(i, v) ((void)(v))
-#define TC_PROF_ENABLED 0
-#endif
+#include <type_traits>
 
 namespace {
 
-constexpr int kStageBytes = kKBlockBytes;          // B ring stage = one k-block: [<=128 rows x 64] at CG=2
-                                                   // (two k-blocks per stage were measured: no gain, less ring depth)
-constexpr int kNumEpiWarps = 4, kNumProdWarps = 8;
-// the producer warps form groups that work on different ring stages concurrently:
-// fp32 sources: 2 groups of 4 warps (theta and noise both through registers);
-// bf16 shadows: 4 groups of 2 warps (theta tile by TMA, only the noise through registers)
-__host__ __device__ constexpr int prod_groups(int mode) { return mode == 1 ? 4 : 2; }
-// operand / source modes of the kernel template:
-//   kModeBF16   bf16 operands formed from fp32 theta + fp32 table (through registers)
-//   kModeBF16S  bf16 operands formed from bf16 shadows (theta tile by TMA, in place)
-//   kModeF16    fp16 operands (11-bit significand = TF32 class) formed from fp32 theta and the EXACT
-//               16-bit copy of the noise table (estk_shadow_f16: table values are fp16-representable),
-//               one rounding per weight: W16 = rn_f16(theta + s*sigma*eps) with the sum in fp32;
-//               layer-0 input split x = x_hi + x_lo (two fp16 k-block sets, same B tile)
+constexpr int kRows = 64;                          // observation rows per CTA (wgmma M)
+constexpr int kTileN = 128;                        // wgmma N
+constexpr int kHBlockBytes = kRows * kBlockK * 2;  // one [64 x 64] 16-bit k-block of activations = 8 KB
+constexpr int kHBytes = (kMaxW / kBlockK) * kHBlockBytes;   // 64 KB per activation buffer
+constexpr int kStageBytes = kTileN * kBlockK * 2;  // one [128 x 64] 16-bit B stage = 16 KB
+constexpr int kStages = 5;
+constexpr int kProdWarps = 8, kProdGroups = 2, kProdGroupWarps = kProdWarps / kProdGroups;
+constexpr int kPT = 32 * kProdGroupWarps;          // threads per producer group
+constexpr int kThreadsTC = 128 + 32 * kProdWarps;  // 384
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
-constexpr int kThreadsTC = 32 * (2 + kNumEpiWarps + kNumProdWarps);   // 448
-
-// TMA descriptors of the bf16 theta shadow, one per (layer, N tile): [N x K] row-major,
-// box [rows of the tile per CTA x 64], SWIZZLE_128B == the UMMA B-operand layout
-struct TcMaps { CUtensorMap m[ESTK_MAX_LAYERS][2]; };
 
 struct EvalTCParams {
   estk_mlp_desc desc;
   const float* theta;
   const float* table;
-  const uint16_t* theta16;  // optional bf16 shadows of theta / table (both or neither):
-  const uint16_t* table16;  // producer sources at half the bytes (precision mode "bf16s")
-  const int64_t* offsets;  // null => centre evaluation
+  const uint16_t* theta16;  // bf16 shadows of theta / table (kModeBF16S)
+  const uint16_t* table16;  // bf16 shadow (kModeBF16S) or exact fp16 copy (kModeF16) of the table
+  const int64_t* offsets;   // null => centre evaluation
   const int32_t* order;
   int pairs;
   float sigma;
   const float* obs;
   const float* target;
-  int B, chunks;           // chunks of 128*CG observations
+  int B, chunks;            // chunks of kRows observations
   float* ret_plus;
   float* ret_minus;
   float* bc_plus;
   float* bc_minus;
   int bc_obs, bc_dim;
-  float* partial;          // [pairs*2][chunks*CG]
-  unsigned int* counters;  // [pairs*2]
-  float* centre_out;       // optional: also evaluate theta itself (sigma = 0) into centre_out[0]
-  int n_centre;            // number of leading centre tasks (0 or chunks)
-  int n_tasks;             // n_centre + pairs * n_signs * chunks
-  int n_signs;             // 2, or 1 for the centre evaluation
-  int mode;                // kModeBF16 / kModeBF16S / kModeF16
-  int dbg;                 // ESTK_TC_DEBUG bit mask (perf triage only): 1 no producer loads, 4 no MMA, 8 role counters, 16 TMEM read only
+  float* partial;           // [pairs*2 + 1][chunks]
+  unsigned int* counters;   // [pairs*2 + 1]
+  float* centre_out;        // optional: also evaluate theta itself (sigma = 0) into centre_out[0]
+  int n_centre;             // number of leading centre tasks (0 or chunks)
+  int n_tasks;              // n_centre + pairs * n_signs * chunks
+  int n_signs;              // 2, or 1 for the centre evaluation
+  int mode;
 };
 
 struct Layer { int K, N; int64_t wbase, bbase; };
@@ -122,61 +82,28 @@ __device__ __forceinline__ TaskId decode_task(const EvalTCParams& p, int task, b
   t.centre = all_centre;
   return t;
 }
-#define PROF_ON (prof)
-#define PROF_T() (PROF_ON ? clock64() : 0ll)
-#define PROF_ADD(i, t0) do { if (PROF_ON) TC_PROF_ATOMIC(i, clock64() - (t0)); } while (0)
 
-// 448 threads at 128 registers: the register file is allocated per 4 warps, so a 14-warp
-// block is charged as 16 warps and 144 registers per thread do not launch (measured)
-template <int CG, int MODE, int RING>
-__global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTCParams p,
-                                                                     const __grid_constant__ TcMaps maps) {
-  constexpr int kStages = RING;
+template <int MODE>
+__global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTCParams p) {
   constexpr bool S16 = (MODE == kModeBF16S), F16 = (MODE == kModeF16);
-  constexpr int kProdGroups = prod_groups(MODE), kProdGroupWarps = kNumProdWarps / kProdGroups;
-  constexpr int kStageB = (CG == 2) ? kStageBytes : 2 * kStageBytes;   // up to 256 rows at CG=1
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sH = smem;                                    // 8 k-blocks x 16 KB
-  uint8_t* sB = sH + (kMaxW / kBlockK) * kKBlockBytes;   // ring
-  float* sBias = reinterpret_cast<float*>(sB + kStages * kStageB);   // [2][512]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + 2 * kMaxW);
-  uint64_t* bar_full = bars;                 // [kStages]  (leader's are used)
-  uint64_t* bar_empty = bars + kStages;      // [kStages]  (local)
-  uint64_t* bar_acc = bars + 2 * kStages;    // layer accumulated (local)
-  uint64_t* bar_h = bars + 2 * kStages + 1;  // activations in place (leader's is used)
-  uint64_t* bar_acc0 = bars + 2 * kStages + 2;   // first N-tile of a two-tile layer accumulated (local)
-  uint64_t* bar_tma = bars + 2 * kStages + 3;    // [kStages] theta tile landed in the ring slot (local, bf16s only)
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 3);
-  float* s_loss = reinterpret_cast<float*>(s_tmem + 2);  // [kNumEpiWarps]
+  uint8_t* sH = smem;                                  // 2 activation buffers x 8 k-blocks x 8 KB
+  uint8_t* sB = sH + 2 * kHBytes;                      // ring
+  float* sBias = reinterpret_cast<float*>(sB + kStages * kStageBytes);   // [512], one layer at a time
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(sBias + kMaxW);      // [kStages] stage formed
+  uint64_t* bar_empty = bar_full + kStages;                             // [kStages] stage consumed
+  float* s_loss = reinterpret_cast<float*>(bar_empty + kStages);        // [4]
+  __shared__ Layer lay[ESTK_MAX_LAYERS];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int cluster_id = blockIdx.x / CG, n_clusters = gridDim.x / CG;
   const int L = p.desc.n_layers;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(smem_u32(bar_full + s), CG * kProdGroupWarps);
-      mbar_init(smem_u32(bar_empty + s), 1);
-      mbar_init(smem_u32(bar_tma + s), 1);
-    }
-    mbar_init(smem_u32(bar_acc), 1);
-    mbar_init(smem_u32(bar_acc0), 1);
-    mbar_init(smem_u32(bar_h), CG * kNumEpiWarps);
-    fence_barrier_init();
-  }
-  if (CG == 2) cluster_sync_all();
-  if (warp == 1) tmem_alloc<CG>(smem_u32(s_tmem), 512);
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(s_tmem);
-
-  // per-layer geometry, in shared memory (a local-memory array would miss the L1
-  // that the weight stream keeps evicting)
-  __shared__ Layer lay[ESTK_MAX_LAYERS];
   if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(smem_u32(bar_full + s), kProdGroupWarps);
+      mbar_init(smem_u32(bar_empty + s), 4);
+    }
+    fence_barrier_init();
     int64_t pb = 0;
     for (int l = 0; l < L; ++l) {
       lay[l].K = p.desc.dims[l];
@@ -188,288 +115,126 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   }
   __syncthreads();
   const bool centre = (p.offsets == nullptr);
-  const bool prof = TC_PROF_ENABLED && (p.dbg & 8) && blockIdx.x == 0 && lane == 0;
 
-  if (warp == 0) {
-    // =================================================================== MMA issuer
-    if (cta_rank == 0) {
-      uint32_t stage = 0, ring_phase = 0, h_phase = 0;
-      const long long tm0 = PROF_T();
-      for (int task = cluster_id; task < p.n_tasks; task += n_clusters) {
-        for (int l = 0; l < L; ++l) {
-          const long long th0 = PROF_T();
-          mbar_wait(smem_u32(bar_h), h_phase);     // k-blocks 0..3 of this layer's input are in place
-          PROF_ADD(1, th0);
-          h_phase ^= 1;
-          tc_fence_after();
-          const int K = lay[l].K, N = lay[l].N;
-          bool second_half_ready = (K <= 256) || (l == 0);   // hidden inputs wider than 256 arrive in two halves
-          for (int n0 = 0; n0 < N; n0 += 256) {
-            const int Ng = min(256, N - n0);
-            const uint32_t idesc = make_idesc(128 * CG, Ng, F16);
-            const uint32_t tmem_d = tmem_base + (uint32_t)n0;
-            // fp16 mode: the layer-0 input is x_hi + x_lo; the lo half lives K/64 k-blocks further
-            const int lo_kb = (F16 && l == 0) ? K / kBlockK : 0;
-            for (int kb = 0; kb < K / kBlockK; ++kb) {
-              if (kb >= 4 && !second_half_ready) {   // k-blocks 4..7 (and TMEM columns >= 256 drained)
-                const long long th1 = PROF_T();
-                mbar_wait(smem_u32(bar_h), h_phase);
-                PROF_ADD(1, th1);
-                h_phase ^= 1;
-                tc_fence_after();
-                second_half_ready = true;
-              }
-              const long long tf0 = PROF_T();
-              mbar_wait(smem_u32(bar_full + stage), ring_phase);
-              PROF_ADD(2, tf0);
-              const long long ti0 = PROF_T();
-              tc_fence_after();
-              if (elect_one()) {
-                const uint32_t a_addr = smem_u32(sH + kb * kKBlockBytes);
-                const uint32_t b_addr = smem_u32(sB + stage * kStageB);
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16 && !(p.dbg & 4); ++k) {
-                  const uint64_t da = make_sw128_desc(a_addr + k * 32);
-                  const uint64_t db = make_sw128_desc(b_addr + k * 32);
-                  umma_bf16<CG>(tmem_d, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-                }
-                if (lo_kb) {
-                  const uint32_t a_lo = smem_u32(sH + (kb + lo_kb) * kKBlockBytes);
-#pragma unroll
-                  for (int k = 0; k < kBlockK / 16 && !(p.dbg & 4); ++k)
-                    umma_bf16<CG>(tmem_d, make_sw128_desc(a_lo + k * 32), make_sw128_desc(b_addr + k * 32), idesc, 1u);
-                }
-                umma_commit<CG>(smem_u32(bar_empty + stage));          // frees the ring slot (both CTAs)
-                if (kb + 1 == K / kBlockK) {
-                  if (n0 + 256 >= N) umma_commit<CG>(smem_u32(bar_acc));     // layer accumulated
-                  else umma_commit<CG>(smem_u32(bar_acc0));                  // tile 0 of 2: its drain overlaps tile 1's MMAs
-                }
-              }
-              __syncwarp();
-              PROF_ADD(3, ti0);
-              if (++stage == kStages) { stage = 0; ring_phase ^= 1; }
-            }
-          }
-        }
-      }
-      PROF_ADD(0, tm0);
-    }
-  } else if (warp == 1) {
-    // =================================================================== theta-tile TMA (bf16 shadow sources)
-    // One thread walks the same (task, layer, n-tile, k-block) stage sequence as the
-    // producers and, as soon as a ring slot is free, has the TMA engine drop this CTA's
-    // [rows x 64] tile of the bf16 theta shadow into it -- already in the swizzled
-    // B-operand layout.  The producers then only stream the noise through registers and
-    // turn the slot into theta + s*sigma*eps in place.
-    if constexpr (S16) {
-      if (lane == 0) {
-        uint32_t cnt = 0;
-        for (int task = cluster_id; task < p.n_tasks; task += n_clusters) {
-          for (int l = 0; l < L; ++l) {
-            const int K = lay[l].K, N = lay[l].N;
-            for (int n0 = 0; n0 < N; n0 += 256) {
-              const int rows = min(256, N - n0) / CG;
-              const CUtensorMap* map = &maps.m[l][n0 ? 1 : 0];
-              for (int kb = 0; kb < K / kBlockK; ++kb, ++cnt) {
-                const uint32_t stage = cnt % kStages, ring_phase = (cnt / kStages) & 1u;
-                mbar_wait(smem_u32(bar_empty + stage), ring_phase ^ 1);
-                if (!(p.dbg & 2)) {
-                  mbar_arrive_expect_tx(smem_u32(bar_tma + stage), (uint32_t)rows * 128u);
-                  tma_load_2d(smem_u32(sB + stage * kStageB), map, kb * kBlockK, n0 + (int)cta_rank * rows,
-                              smem_u32(bar_tma + stage));
-                } else {
-                  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar_tma + stage)) : "memory");
-                }
-              }
-            }
-          }
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 2 && warp < 2 + kNumEpiWarps) {
-    // =================================================================== epilogue warps
-    const int q = warp & 3;                    // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;             // observation row inside the CTA's 128
-    const int etid = (warp - 2) * 32 + lane;   // 0..127
-    uint32_t acc_phase = 0, acc0_phase = 0;
-    const bool eprof = prof && warp == 2;
-    const long long te0 = eprof ? clock64() : 0ll;
-    for (int task = cluster_id; task < p.n_tasks; task += n_clusters) {
-      const long long to0 = eprof ? clock64() : 0ll;
+  if (warp < 4) {
+    // =================================================================== consumer warpgroup
+    const int tid = threadIdx.x;                     // 0..127
+    const int r0 = warp * 16 + (lane >> 2);          // accumulator rows r0 and r0 + 8
+    const int cq = (lane & 3) * 2;                   // accumulator columns 8j + cq, +1
+    uint32_t kst = 0;                                // global stage index
+    for (int task = blockIdx.x; task < p.n_tasks; task += gridDim.x) {
       const TaskId tk = decode_task(p, task, centre);
       const int chunk = tk.chunk, sgn = tk.sgn, slot = tk.slot;
       const int j = (!tk.centre && p.order) ? p.order[slot] : slot;
       const float* trow = tk.centre ? p.theta : p.table + p.offsets[j];
       const float ssig = tk.centre ? 0.f : (sgn ? -p.sigma : p.sigma);
-      const int b = (chunk * CG + (int)cta_rank) * 128 + row;      // global observation index
-      // ---- stage this CTA's observations as the layer-0 A operand
+      float* bc = (tk.centre && !centre) ? nullptr : (sgn ? p.bc_minus : p.bc_plus);
+      // ---- this CTA's observations as the layer-0 A operand (buffer 0)
       {
-        const int K0 = lay[0].K;
-        const float* orow = p.obs + (size_t)b * K0;
-        for (int c0 = 0; c0 < K0 / 8; c0 += 8) {            // 16 independent 128-bit loads per batch
-          float4 x[8][2];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            x[u][0] = __ldg(reinterpret_cast<const float4*>(orow + (c0 + u) * 8));
-            x[u][1] = __ldg(reinterpret_cast<const float4*>(orow + (c0 + u) * 8 + 4));
-          }
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const int c = c0 + u;
-            const uint32_t addr = smem_u32(sH + (c >> 3) * kKBlockBytes) + sw128_offset(row, c & 7);
-            const uint32_t h0 = pack16<F16>(x[u][0].x, x[u][0].y), h1 = pack16<F16>(x[u][0].z, x[u][0].w);
-            const uint32_t h2 = pack16<F16>(x[u][1].x, x[u][1].y), h3 = pack16<F16>(x[u][1].z, x[u][1].w);
-            st_shared_v4(addr, h0, h1, h2, h3);
-            if constexpr (F16) {
-              // x_lo = rn_f16(x - x_hi): the observation enters layer 0 with ~22 significant bits
-              const float2 f0 = unpack_f16(h0), f1 = unpack_f16(h1), f2 = unpack_f16(h2), f3 = unpack_f16(h3);
-              const uint32_t alo = smem_u32(sH + ((c >> 3) + K0 / kBlockK) * kKBlockBytes) + sw128_offset(row, c & 7);
-              st_shared_v4(alo, pack_f16(x[u][0].x - f0.x, x[u][0].y - f0.y), pack_f16(x[u][0].z - f1.x, x[u][0].w - f1.y),
-                           pack_f16(x[u][1].x - f2.x, x[u][1].y - f2.y), pack_f16(x[u][1].z - f3.x, x[u][1].w - f3.y));
-            }
+        const int K0 = lay[0].K, per_row = K0 / 8;
+        for (int it = tid; it < kRows * per_row; it += 128) {
+          const int r = it / per_row, c = it % per_row;
+          const float* src = p.obs + (size_t)(chunk * kRows + r) * K0 + c * 8;
+          const float4 x0 = __ldg(reinterpret_cast<const float4*>(src));
+          const float4 x1 = __ldg(reinterpret_cast<const float4*>(src + 4));
+          const uint32_t addr = smem_u32(sH + (c >> 3) * kHBlockBytes) + sw128_offset(r, c & 7);
+          const uint32_t h0 = pack16<F16>(x0.x, x0.y), h1 = pack16<F16>(x0.z, x0.w);
+          const uint32_t h2 = pack16<F16>(x1.x, x1.y), h3 = pack16<F16>(x1.z, x1.w);
+          st_shared_v4(addr, h0, h1, h2, h3);
+          if constexpr (F16) {
+            // x_lo = rn_f16(x - x_hi): the observation enters layer 0 with ~22 significant bits
+            const float2 f0 = unpack_f16(h0), f1 = unpack_f16(h1), f2 = unpack_f16(h2), f3 = unpack_f16(h3);
+            st_shared_v4(addr + (K0 / kBlockK) * kHBlockBytes, pack_f16(x0.x - f0.x, x0.y - f0.y),
+                         pack_f16(x0.z - f1.x, x0.w - f1.y), pack_f16(x1.x - f2.x, x1.y - f2.y),
+                         pack_f16(x1.z - f3.x, x1.w - f3.y));
           }
         }
       }
-      if (eprof) TC_PROF_ATOMIC(11, clock64() - to0);
       float loss = 0.f;
-      const uint32_t trow_addr = tmem_base + ((uint32_t)(q * 32) << 16);
       for (int l = 0; l < L; ++l) {
-        const long long tb0 = eprof ? clock64() : 0ll;
-        const int N = lay[l].N;
-        float* bias = sBias + (l & 1) * kMaxW;
-        // this layer's output is the next layer's input: it is handed over in halves
-        // (k-blocks 0..3, then 4..7) so the next layer's first MMAs overlap the rest of
-        // this epilogue
-        auto hand_over = [&]() {
-          fence_proxy_async();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_on<CG>(smem_u32(bar_h), 0);
-        };
-        // the staged observations are this task's layer-0 input (the previous task's TMEM
-        // reads are long done): release the MMA warp before anything else
-        if (l == 0) hand_over();
-        for (int o = etid; o < N; o += 32 * kNumEpiWarps)
-          bias[o] = fmaf(ssig, ld_noise1(trow + lay[l].bbase + o), __ldg(p.theta + lay[l].bbase + o));
-        named_bar_sync(1, 32 * kNumEpiWarps);   // publishes bias[] among the epilogue warps
-        if (eprof) TC_PROF_ATOMIC(12, clock64() - tb0);
+        const int K = lay[l].K, N = lay[l].N;
         const bool last = (l == L - 1);
-        const bool two = N > 256;               // two N tiles: columns [0,256) and [256,N)
-        // bias + ReLU + round to bf16: 32 accumulator columns -> 16 packed words
-        auto pack = [&](const uint32_t (&v)[32], int c0, uint32_t (&pk)[16]) {
-          const uint32_t baddr = smem_u32(bias + c0);
+        const uint32_t h_in = smem_u32(sH + (l & 1) * kHBytes);
+        const uint32_t h_out = smem_u32(sH + ((l + 1) & 1) * kHBytes);
+        named_bar_sync(1, 128);          // previous layer's epilogue (bias reads) done
+        for (int o = tid; o < N; o += 128)
+          sBias[o] = fmaf(ssig, ld_noise1(trow + lay[l].bbase + o), __ldg(p.theta + lay[l].bbase + o));
+        fence_proxy_async();             // this layer's input (generic-proxy stores) -> wgmma
+        named_bar_sync(1, 128);          // ... by every thread; bias[] published
+        const int lo_kb = (F16 && l == 0) ? K / kBlockK : 0;   // layer 0 in fp16: x_lo k-blocks
+        for (int n0 = 0; n0 < N; n0 += kTileN) {
+          const int width = min(kTileN, N - n0);
+          float d[64];                     // the first MMA of the tile overwrites (scale-d = 0)
+          uint32_t prev = 0;
+          // NP = 2: layer 0 in fp16, x_lo on the same B tile (a separate instantiation, so that no
+          // wgmma sits under a branch)
+          auto k_loop = [&](auto np_tag) {
+            constexpr int NP = decltype(np_tag)::value;
+            for (int kb = 0; kb < K / kBlockK; ++kb, ++kst) {
+              const uint32_t stage = kst % kStages, phase = (kst / kStages) & 1u;
+              mbar_wait(smem_u32(bar_full + stage), phase);
+              const uint32_t a_addr = h_in + kb * kHBlockBytes, b_addr = smem_u32(sB + stage * kStageBytes);
+              wgmma_fence();
 #pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const float4 t = ld_shared_v4(baddr + g * 16);
-            pk[g * 2 + 0] = pack16_relu<F16>(__uint_as_float(v[g * 4 + 0]) + t.x, __uint_as_float(v[g * 4 + 1]) + t.y);
-            pk[g * 2 + 1] = pack16_relu<F16>(__uint_as_float(v[g * 4 + 2]) + t.z, __uint_as_float(v[g * 4 + 3]) + t.w);
-          }
-        };
-        // W packed words (2*W output features starting at feature f0) -> activations in smem
-        auto store_h = [&](const uint32_t* pk, int f0, int words) {
+              for (int pass = 0; pass < NP; ++pass) {
+                const uint32_t a = a_addr + pass * lo_kb * kHBlockBytes;
 #pragma unroll
-          for (int g = 0; g < 8; ++g) {          // chunks of 8 output features = 16 bytes of bf16
-            if (g * 4 < words) {
-              const int col = f0 + g * 8;
-              const uint32_t addr = smem_u32(sH + (col >> 6) * kKBlockBytes) + sw128_offset(row, (col & 63) >> 3);
-              st_shared_v4(addr, pk[g * 4 + 0], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
+                for (int k = 0; k < kBlockK / 16; ++k)
+                  wgmma_m64n128k16<F16>(d, make_sw128_desc(a + k * 32), make_sw128_desc(b_addr + k * 32),
+                                        (kb | k | pass) != 0 ? 1u : 0u);
+              }
+              wgmma_commit();
+              wgmma_wait<1>();             // the previous stage's MMAs are done: release its slot
+              if (kb > 0 && lane == 0) mbar_arrive(smem_u32(bar_empty + prev));
+              prev = stage;
             }
-          }
-        };
-        // last layer: fused squared error (and the behaviour characterisation)
-        auto loss_chunk = [&](const uint32_t (&v)[32], int c0) {
-          const uint32_t baddr = smem_u32(bias + c0);
-          const float* trg = p.target + (size_t)b * N + c0;
-          float* bc = (tk.centre && !centre) ? nullptr : (sgn ? p.bc_minus : p.bc_plus);
+          };
+          if (F16 && lo_kb) k_loop(std::integral_constant<int, 2>{});
+          else k_loop(std::integral_constant<int, 1>{});
+          wgmma_wait<0>();
+          fence_acc(d);
+          if (lane == 0) mbar_arrive(smem_u32(bar_empty + prev));
+          // ---- epilogue of the tile
 #pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const float4 t4 = __ldg(reinterpret_cast<const float4*>(trg + g * 4));
-            const float4 b4 = ld_shared_v4(baddr + g * 16);
-            const float tv[4] = {t4.x, t4.y, t4.z, t4.w};
-            const float bv[4] = {b4.x, b4.y, b4.z, b4.w};
+          for (int jb = 0; jb < kTileN / 8; ++jb) {
+            if (jb * 8 < width) {
+              const int col = n0 + jb * 8 + cq;
+              const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int o = c0 + g * 4 + e;
-              const float y = __uint_as_float(v[g * 4 + e]) + bv[e];
-              const float d = y - tv[e];
-              loss = fmaf(d, d, loss);
-              if (bc) {
-                const int64_t idx = (int64_t)b * N + o;
-                if (b < p.bc_obs && idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y;
+              for (int h = 0; h < 2; ++h) {
+                const int r = r0 + 8 * h;
+                const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                if (last) {
+                  const int b = chunk * kRows + r;
+                  const float2 t = __ldg(reinterpret_cast<const float2*>(p.target + (size_t)b * N + col));
+                  const float e0 = y0 - t.x, e1 = y1 - t.y;
+                  loss = fmaf(e0, e0, loss);
+                  loss = fmaf(e1, e1, loss);
+                  if (bc && b < p.bc_obs) {
+                    const int64_t idx = (int64_t)b * N + col;
+                    if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
+                    if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
+                  }
+                } else {
+                  st_shared_u32(h_out + (col >> 6) * kHBlockBytes + sw128_offset(r, (col & 63) >> 3) + (col & 7) * 2,
+                                pack16_relu<F16>(y0, y1));
+                }
               }
             }
           }
-        };
-        if (two) {
-          // ---- tile 0 is accumulated while tile 1's MMAs still run (they read the
-          // activations in smem, so those cannot be overwritten yet): drain tile 0 now.
-          // Hidden layers park the result as packed bf16 pairs in TMEM columns the drain
-          // has already freed (columns [c0,c0+32) -> [c0/2,c0/2+16), in place).
-          const long long ta0 = eprof ? clock64() : 0ll;
-          mbar_wait(smem_u32(bar_acc0), acc0_phase);
-          acc0_phase ^= 1;
-          tc_fence_after();
-          if (eprof) TC_PROF_ATOMIC(13, clock64() - ta0);
-          const long long tx0 = eprof ? clock64() : 0ll;
-          for (int c0 = 0; c0 < 256; c0 += 32) {
-            uint32_t va[32];
-            tmem_ld32(trow_addr + (uint32_t)c0, va);
-            tmem_ld_wait();
-            if (last) {
-              loss_chunk(va, c0);
-            } else {
-              uint32_t pk[16];
-              pack(va, c0, pk);
-              tmem_st16(trow_addr + (uint32_t)(c0 >> 1), pk);
-            }
-          }
-          if (!last) tmem_st_wait();
-          if (eprof) TC_PROF_ATOMIC(15, clock64() - tx0);
         }
-        // ---- wait for the whole layer: every MMA that reads the activations has completed
-        const long long ta1 = eprof ? clock64() : 0ll;
-        mbar_wait(smem_u32(bar_acc), acc_phase);
-        acc_phase ^= 1;
-        tc_fence_after();
-        if (eprof) TC_PROF_ATOMIC(13, clock64() - ta1);
-        const long long tx1 = eprof ? clock64() : 0ll;
-        if (!last && two) {
-          // parked half -> activation k-blocks 0..3, first hand-over
-          for (int s0 = 0; s0 < 128; s0 += 32) {
-            uint32_t pk[32];
-            tmem_ld32(trow_addr + (uint32_t)s0, pk);
-            tmem_ld_wait();
-            store_h(pk, 2 * s0, 32);
-          }
-          hand_over();
-        }
-        for (int c0 = two ? 256 : 0; c0 < N; c0 += 32) {
-          uint32_t va[32];
-          tmem_ld32(trow_addr + (uint32_t)c0, va);
-          tmem_ld_wait();
-          if (last) {
-            loss_chunk(va, c0);
-          } else {
-            uint32_t pk[16];
-            pack(va, c0, pk);
-            store_h(pk, c0, 16);
-          }
-        }
-        if (!last) hand_over();                  // second half (or the only one when N <= 256)
-        if (eprof) TC_PROF_ATOMIC(14, clock64() - tx1);
       }
       // ---- squared-error partial of this CTA; the last arriver combines them in fixed order
       loss = warp_sum_f(loss);
-      if (lane == 0) s_loss[warp - 2] = loss;
-      named_bar_sync(2, 32 * kNumEpiWarps);
-      if (etid == 0) {
+      if (lane == 0) s_loss[warp] = loss;
+      named_bar_sync(1, 128);
+      if (tid == 0) {
         const float tot = (s_loss[0] + s_loss[1]) + (s_loss[2] + s_loss[3]);
-        const int parts = p.chunks * CG;
+        const int parts = p.chunks;
         const bool folded = tk.centre && !centre;                 // centre task riding in a population launch
         const int cell = folded ? p.pairs * 2 : slot * 2 + sgn;
         float* part = p.partial + (size_t)cell * parts;
-        part[chunk * CG + (int)cta_rank] = tot;
+        part[chunk] = tot;
         __threadfence();
         const unsigned int arrived = atomicAdd(p.counters + cell, 1u);
         if (arrived == (unsigned int)parts - 1) {
@@ -483,282 +248,134 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           p.counters[cell] = 0u;
         }
       }
-      named_bar_sync(2, 32 * kNumEpiWarps);   // s_loss reusable
     }
-    if (eprof) TC_PROF_ATOMIC(10, clock64() - te0);
-  } else if (warp >= 2 + kNumEpiWarps) {
+  } else {
     // =================================================================== weight producers
-    // The producer warps form kProdGroups groups; group g builds stages g, g+G, g+2G, ... of
-    // the flattened (task, layer, n-tile, k-block) stage sequence, so G stages' loads are in
-    // flight per SM and the groups' load / form / fence phases interleave.
-    const int pwarp = warp - 2 - kNumEpiWarps;
+    // Group g forms stages g, g+G, g+2G, ... of the flattened (task, layer, N tile, k-block)
+    // sequence.  Item `it` of a stage = tile row it/8, 16-byte output chunk it%8 (8 weights).
+    const int pwarp = warp - 4;
     const int pgroup = pwarp / kProdGroupWarps;
-    const int ptid = (pwarp % kProdGroupWarps) * 32 + lane;   // thread index inside the group
-    constexpr int kPT = 32 * kProdGroupWarps;
-    struct StageDesc { const float* th; const float* ep; const uint16_t* th16; const uint16_t* ep16; int K; int n_items; float ssig; };
-    constexpr bool src16 = S16;
+    const int ptid = (pwarp % kProdGroupWarps) * 32 + lane;
+    constexpr int kBatch = (MODE == kModeBF16) ? 4 : 8;    // items whose loads are in flight together
     int cached_task = -1;
-    const float* cached_trow = p.theta;
-    const uint16_t* cached_trow16 = p.theta16;
-    float cached_ssig = 0.f;
-    auto setup = [&](int task, int l, int n0, int kb, StageDesc& d) {
-      if (task != cached_task) {            // two dependent global loads: once per task, not per stage
-        cached_task = task;
-        const TaskId tk = decode_task(p, task, centre);
-        const int j = (!tk.centre && p.order) ? p.order[tk.slot] : tk.slot;
-        const int64_t off_j = tk.centre ? 0 : p.offsets[j];
-        cached_trow = tk.centre ? p.theta : p.table + off_j;
-        cached_trow16 = tk.centre ? (F16 ? nullptr : p.theta16) : p.table16 + off_j;
-        cached_ssig = tk.centre ? 0.f : (tk.sgn ? -p.sigma : p.sigma);
-      }
-      const int K = lay[l].K;
-      const int rows = min(256, lay[l].N - n0) / CG;          // this CTA's share of the B tile
-      const int64_t rbase = lay[l].wbase + (int64_t)(n0 + (int)cta_rank * rows) * K + kb * kBlockK;
-      d.th = p.theta + rbase;
-      d.ep = cached_trow + rbase;
-      d.th16 = p.theta16 + rbase;
-      d.ep16 = cached_trow16 ? cached_trow16 + rbase : nullptr;
-      d.K = K;
-      d.n_items = rows * 8;                                    // 16-byte output chunks of the stage
-      d.ssig = cached_ssig;
-    };
-    auto advance = [&](int& task, int& l, int& n0, int& kb) -> bool {
+    const float* trow = p.theta;
+    const uint16_t* trow16 = nullptr;
+    float ssig = 0.f;
+    int task = blockIdx.x, l = 0, n0 = 0, kb = 0;
+    auto advance = [&]() -> bool {
       if (++kb >= lay[l].K / kBlockK) {
         kb = 0;
-        n0 += 256;
+        n0 += kTileN;
         if (n0 >= lay[l].N) {
           n0 = 0;
-          if (++l == L) { l = 0; task += n_clusters; }
+          if (++l == L) { l = 0; task += gridDim.x; }
         }
       }
       return task < p.n_tasks;
     };
-    float4 th[4][2], ep[4][2];
-    int task = cluster_id, l = 0, n0 = 0, kb = 0;
-    bool has_cur = task < p.n_tasks;
-    for (int sk = 0; sk < pgroup && has_cur; ++sk) has_cur = advance(task, l, n0, kb);
-    StageDesc cur = {};
-    uint32_t counter = pgroup;                                // global stage index of `cur`
-    const bool pprof = prof && pwarp == 0;
-    const long long tp0 = pprof ? clock64() : 0ll;
-    while (has_cur) {
-      const uint32_t stage = counter % kStages, ring_phase = (counter / kStages) & 1u;
-      const long long ts0 = pprof ? clock64() : 0ll;
-      setup(task, l, n0, kb, cur);
-      if (pprof) TC_PROF_ATOMIC(5, clock64() - ts0);
-      const uint32_t sbase = smem_u32(sB + stage * kStageB);
+    bool has = task < p.n_tasks;
+    for (int sk = 0; sk < pgroup && has; ++sk) has = advance();
+    uint32_t kst = pgroup;
+    while (has) {
+      if (task != cached_task) {            // two dependent global loads: once per task, not per stage
+        cached_task = task;
+        const TaskId tk = decode_task(p, task, centre);
+        const int jj = (!tk.centre && p.order) ? p.order[tk.slot] : tk.slot;
+        trow = tk.centre ? p.theta : p.table + p.offsets[jj];
+        trow16 = tk.centre ? (S16 ? p.theta16 : nullptr) : p.table16 + p.offsets[jj];
+        ssig = tk.centre ? 0.f : (tk.sgn ? -p.sigma : p.sigma);
+      }
+      const uint32_t stage = kst % kStages, phase = (kst / kStages) & 1u;
+      const uint32_t sbase = smem_u32(sB + stage * kStageBytes);
+      const int K = lay[l].K;
+      const int n_items = min(kTileN, lay[l].N - n0) * 8;
+      const int64_t rbase = lay[l].wbase + (int64_t)n0 * K + kb * kBlockK;
       bool waited = false;
-      if constexpr (src16) {
-        // bf16 shadow sources.  The theta tile arrives by TMA (see warp 1); a group of 64
-        // threads streams the noise: 16 items (128-bit loads, 8 elements each) per thread
-        // cover the whole [128 x 64] stage, issued before the slot is even free.
-        // item u of a thread = tile row u*8 + r0, 16-byte chunk c0 of the 128-byte row
-        static_assert(kPT == 64, "bf16s producer: 64-thread groups");
-        const int r0 = ptid >> 3, c0 = ptid & 7;
-        const int rows = cur.n_items >> 3;
-        const uint16_t* eptr = cur.ep16 + (size_t)r0 * cur.K + c0 * 8;
-        uint4 e16[16];
+      for (int it0 = 0; it0 < n_items; it0 += kBatch * kPT) {
+        float4 th[kBatch][2], ep[kBatch][2];
+        uint4 t16[kBatch], e16[kBatch];
+        // every load of the batch is issued up front ...
 #pragma unroll
-        for (int u = 0; u < 16; ++u)
-          if (u * 8 + r0 < rows && !(p.dbg & 1))
-            e16[u] = ld_noise4u(reinterpret_cast<const uint4*>(eptr + (size_t)(u * 8) * cur.K));
-        const long long tw0 = pprof ? clock64() : 0ll;
-        mbar_wait(smem_u32(bar_tma + stage), ring_phase);          // theta tile landed (so the slot was free)
-        if (pprof) TC_PROF_ATOMIC(7, clock64() - tw0);
-        const long long tc0 = pprof ? clock64() : 0ll;
-        // W = theta16 + (s*sigma)_bf16 * eps16, one packed fma per two elements, in place
-        // (exact product-sum, one rounding to bf16; sigma itself is rounded to bf16)
-        const uint32_t sg2 = pack_bf16(cur.ssig, cur.ssig);
-        const uint32_t taddr = sbase + (uint32_t)(r0 * 128 + ((c0 ^ r0) << 4));   // sw128_offset(u*8 + r0, c0) - u*1024
-#pragma unroll
-        for (int u = 0; u < 16; ++u) {
-          if (u * 8 + r0 < rows) {
-            const uint4 t = ld_shared_v4u(taddr + u * 1024);
-            const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
-            const uint32_t ew[4] = {e16[u].x, e16[u].y, e16[u].z, e16[u].w};
-            uint32_t w[4];
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-              asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(w[c]) : "r"(sg2), "r"(ew[c]), "r"(tw[c]));
-            st_shared_v4(taddr + u * 1024, w[0], w[1], w[2], w[3]);
-          }
-        }
-        if (pprof) TC_PROF_ATOMIC(8, clock64() - tc0);
-      } else if constexpr (F16) {
-        // fp32 theta + the exact fp16 copy of the noise row, both through registers:
-        // W = rn_f16(theta + s*sigma*eps), the sum formed in fp32 (one rounding per weight)
-        for (int it0 = 0; it0 < cur.n_items; it0 += 4 * kPT) {
-          uint4 e16[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int it = it0 + u * kPT + ptid;
-            e16[u] = make_uint4(0u, 0u, 0u, 0u);
-            if (it < cur.n_items && !(p.dbg & 1)) {
-              const int64_t off = (int64_t)(it >> 3) * cur.K + (it & 7) * 8;
-              th[u][0] = ld_noise4(reinterpret_cast<const float4*>(cur.th + off));
-              th[u][1] = ld_noise4(reinterpret_cast<const float4*>(cur.th + off + 4));
-              if (cur.ep16) e16[u] = ld_noise4u(reinterpret_cast<const uint4*>(cur.ep16 + off));
+        for (int u = 0; u < kBatch; ++u) {
+          const int it = it0 + u * kPT + ptid;
+          if (it < n_items) {
+            const int64_t off = rbase + (int64_t)(it >> 3) * K + (it & 7) * 8;
+            if constexpr (S16) {
+              t16[u] = ld_noise4u(reinterpret_cast<const uint4*>(p.theta16 + off));
+              e16[u] = ld_noise4u(reinterpret_cast<const uint4*>(trow16 + off));
+            } else if constexpr (F16) {
+              th[u][0] = ld_noise4(reinterpret_cast<const float4*>(p.theta + off));
+              th[u][1] = ld_noise4(reinterpret_cast<const float4*>(p.theta + off + 4));
+              e16[u] = trow16 ? ld_noise4u(reinterpret_cast<const uint4*>(trow16 + off)) : make_uint4(0u, 0u, 0u, 0u);
+            } else {
+              th[u][0] = ld_noise4(reinterpret_cast<const float4*>(p.theta + off));
+              th[u][1] = ld_noise4(reinterpret_cast<const float4*>(p.theta + off + 4));
+              ep[u][0] = ld_noise4(reinterpret_cast<const float4*>(trow + off));
+              ep[u][1] = ld_noise4(reinterpret_cast<const float4*>(trow + off + 4));
             }
           }
-          if (!waited) {
-            const long long tw0 = pprof ? clock64() : 0ll;
-            mbar_wait(smem_u32(bar_empty + stage), ring_phase ^ 1);
-            waited = true;
-            if (pprof) TC_PROF_ATOMIC(7, clock64() - tw0);
-          }
-          const long long tc0 = pprof ? clock64() : 0ll;
+        }
+        // ... then wait for the ring slot
+        if (!waited) {
+          mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
+          waited = true;
+        }
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int it = it0 + u * kPT + ptid;
-            if (it < cur.n_items) {
-              const float sg = cur.ssig;
+        for (int u = 0; u < kBatch; ++u) {
+          const int it = it0 + u * kPT + ptid;
+          if (it < n_items) {
+            const float sg = ssig;
+            uint32_t w[4];
+            if constexpr (S16) {
+              // W = theta16 + (s*sigma)_bf16 * eps16: exact product-sum, one rounding to bf16
+              const uint32_t sg2 = pack_bf16(sg, sg);
+              const uint32_t tw[4] = {t16[u].x, t16[u].y, t16[u].z, t16[u].w};
+              const uint32_t ew[4] = {e16[u].x, e16[u].y, e16[u].z, e16[u].w};
+#pragma unroll
+              for (int c = 0; c < 4; ++c) asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(w[c]) : "r"(sg2), "r"(ew[c]), "r"(tw[c]));
+            } else if constexpr (F16) {
               const float2 e0 = unpack_f16(e16[u].x), e1 = unpack_f16(e16[u].y);
               const float2 e2 = unpack_f16(e16[u].z), e3 = unpack_f16(e16[u].w);
-              const uint32_t w0 = pack_f16(fmaf(sg, e0.x, th[u][0].x), fmaf(sg, e0.y, th[u][0].y));
-              const uint32_t w1 = pack_f16(fmaf(sg, e1.x, th[u][0].z), fmaf(sg, e1.y, th[u][0].w));
-              const uint32_t w2 = pack_f16(fmaf(sg, e2.x, th[u][1].x), fmaf(sg, e2.y, th[u][1].y));
-              const uint32_t w3 = pack_f16(fmaf(sg, e3.x, th[u][1].z), fmaf(sg, e3.y, th[u][1].w));
-              st_shared_v4(sbase + sw128_offset(it >> 3, it & 7), w0, w1, w2, w3);
+              w[0] = pack_f16(fmaf(sg, e0.x, th[u][0].x), fmaf(sg, e0.y, th[u][0].y));
+              w[1] = pack_f16(fmaf(sg, e1.x, th[u][0].z), fmaf(sg, e1.y, th[u][0].w));
+              w[2] = pack_f16(fmaf(sg, e2.x, th[u][1].x), fmaf(sg, e2.y, th[u][1].y));
+              w[3] = pack_f16(fmaf(sg, e3.x, th[u][1].z), fmaf(sg, e3.y, th[u][1].w));
+            } else {
+              w[0] = pack_bf16(fmaf(sg, ep[u][0].x, th[u][0].x), fmaf(sg, ep[u][0].y, th[u][0].y));
+              w[1] = pack_bf16(fmaf(sg, ep[u][0].z, th[u][0].z), fmaf(sg, ep[u][0].w, th[u][0].w));
+              w[2] = pack_bf16(fmaf(sg, ep[u][1].x, th[u][1].x), fmaf(sg, ep[u][1].y, th[u][1].y));
+              w[3] = pack_bf16(fmaf(sg, ep[u][1].z, th[u][1].z), fmaf(sg, ep[u][1].w, th[u][1].w));
             }
+            st_shared_v4(sbase + sw128_offset(it >> 3, it & 7), w[0], w[1], w[2], w[3]);
           }
-          if (pprof) TC_PROF_ATOMIC(8, clock64() - tc0);
-        }
-      } else {
-      for (int it0 = 0; it0 < cur.n_items; it0 += 4 * kPT) {
-          // every 128-bit load of the batch is issued up front (16 in flight per thread) ...
-  #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int it = it0 + u * kPT + ptid;
-            if (it < cur.n_items && !(p.dbg & 1)) {
-              const int64_t off = (int64_t)(it >> 3) * cur.K + (it & 7) * 8;
-              th[u][0] = ld_noise4(reinterpret_cast<const float4*>(cur.th + off));
-              th[u][1] = ld_noise4(reinterpret_cast<const float4*>(cur.th + off + 4));
-              ep[u][0] = ld_noise4(reinterpret_cast<const float4*>(cur.ep + off));
-              ep[u][1] = ld_noise4(reinterpret_cast<const float4*>(cur.ep + off + 4));
-            }
-          }
-          // ... then wait for the ring slot (almost always free already)
-          if (!waited) {
-            const long long tw0 = pprof ? clock64() : 0ll;
-            mbar_wait(smem_u32(bar_empty + stage), ring_phase ^ 1);
-            waited = true;
-            if (pprof) TC_PROF_ATOMIC(7, clock64() - tw0);
-          }
-          const long long tc0 = pprof ? clock64() : 0ll;
-  #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int it = it0 + u * kPT + ptid;
-            if (it < cur.n_items) {
-              const float sg = cur.ssig;
-              const uint32_t w0 = pack_bf16(fmaf(sg, ep[u][0].x, th[u][0].x), fmaf(sg, ep[u][0].y, th[u][0].y));
-              const uint32_t w1 = pack_bf16(fmaf(sg, ep[u][0].z, th[u][0].z), fmaf(sg, ep[u][0].w, th[u][0].w));
-              const uint32_t w2 = pack_bf16(fmaf(sg, ep[u][1].x, th[u][1].x), fmaf(sg, ep[u][1].y, th[u][1].y));
-              const uint32_t w3 = pack_bf16(fmaf(sg, ep[u][1].z, th[u][1].z), fmaf(sg, ep[u][1].w, th[u][1].w));
-              st_shared_v4(sbase + sw128_offset(it >> 3, it & 7), w0, w1, w2, w3);
-            }
-          }
-          if (pprof) TC_PROF_ATOMIC(8, clock64() - tc0);
         }
       }
-      const long long tf0 = pprof ? clock64() : 0ll;
+      if (!waited) mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
       fence_proxy_async();
       __syncwarp();
-      if (lane == 0) mbar_arrive_on<CG>(smem_u32(bar_full + stage), 0);
-      if (pprof) TC_PROF_ATOMIC(9, clock64() - tf0);
-      for (int sk = 0; sk < kProdGroups && has_cur; ++sk) has_cur = advance(task, l, n0, kb);
-      counter += kProdGroups;
-      if (pprof) TC_PROF_ATOMIC(6, 1ull);
+      if (lane == 0) mbar_arrive(smem_u32(bar_full + stage));
+      for (int sk = 0; sk < kProdGroups && has; ++sk) has = advance();
+      kst += kProdGroups;
     }
-    if (pprof) TC_PROF_ATOMIC(4, clock64() - tp0);
   }
-
-  // ---- teardown
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) tmem_dealloc<CG>(tmem_base, 512);
 }
 
-template <int CG>
-size_t tc_smem_bytes(int stages) {
-  const int stage_b = (CG == 2) ? kStageBytes : 2 * kStageBytes;
-  return 1024 + (size_t)(kMaxW / kBlockK) * kKBlockBytes + (size_t)stages * stage_b + 2 * kMaxW * sizeof(float) +
-         (3 * stages + 3) * sizeof(uint64_t) + 128;
+size_t tc_smem_bytes() {
+  return 1024 + 2 * (size_t)kHBytes + (size_t)kStages * kStageBytes + kMaxW * sizeof(float) +
+         2 * kStages * sizeof(uint64_t) + 4 * sizeof(float);
 }
 
-template <int CG, int MODE, int RING>
-int launch_tc(estk_ctx* ctx, EvalTCParams& p, const TcMaps* maps, cudaStream_t stream) {
-  const size_t smem = tc_smem_bytes<CG>(RING);
-  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<CG, MODE, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int clusters = ctx->sm_count / CG;
-  if (clusters > p.n_tasks) clusters = p.n_tasks;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(clusters * CG);
-  cfg.blockDim = dim3(kThreadsTC);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  ESTK_CUDA(cudaLaunchKernelEx(&cfg, eval_mlp_tc_kernel<CG, MODE, RING>, p, *maps));
+template <int MODE>
+int launch_tc(estk_ctx* ctx, const EvalTCParams& p, cudaStream_t stream) {
+  const size_t smem = tc_smem_bytes();
+  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = ctx->sm_count < p.n_tasks ? ctx->sm_count : p.n_tasks;
+  eval_mlp_tc_kernel<MODE><<<grid, kThreadsTC, smem, stream>>>(p);
+  ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
 }
 
-// ---- TMA descriptors of the theta shadow (host side)
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int build_theta_maps(const estk_mlp_desc& d, const uint16_t* theta16, int cg, TcMaps* out) {
-  static EncodeTiledFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    ESTK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    if (!fn || qres != cudaDriverEntryPointSuccess) {
-      estk_set_error("cuTensorMapEncodeTiled is not available from this driver");
-      return ESTK_ERR_CUDA;
-    }
-    encode = (EncodeTiledFn)fn;
-  }
-  // single-entry cache: the descriptors only depend on the shadow's address and the layer shapes
-  static thread_local struct { const uint16_t* ptr; estk_mlp_desc desc; int device; bool valid; TcMaps maps; } cache = {};
-  int dev = -1;
-  ESTK_CUDA(cudaGetDevice(&dev));
-  if (cache.valid && cache.ptr == theta16 && cache.device == dev && memcmp(&cache.desc, &d, sizeof(d)) == 0) {
-    *out = cache.maps;
-    return ESTK_OK;
-  }
-  memset(out, 0, sizeof(*out));
-  int64_t pb = 0;
-  for (int l = 0; l < d.n_layers; ++l) {
-    const int K = d.dims[l], N = d.dims[l + 1];
-    for (int t = 0; t < 2; ++t) {
-      const int n0 = t * 256;
-      const int Nt = (n0 < N) ? (N - n0 < 256 ? N - n0 : 256) : (N < 256 ? N : 256);   // tile 1 of a one-tile layer: unused copy
-      const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)N};
-      const cuuint64_t gstride[1] = {(cuuint64_t)K * 2};
-      const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)(Nt / cg)};
-      const cuuint32_t estride[2] = {1, 1};
-      const CUresult r = encode(&out->m[l][t], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)(theta16 + pb), gdim, gstride,
-                                box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        estk_set_error("cuTensorMapEncodeTiled failed (%d) for layer %d tile %d [N=%d K=%d box %dx%d]", (int)r, l, t, N, K,
-                       Nt / cg, kBlockK);
-        return ESTK_ERR_CUDA;
-      }
-    }
-    pb += (int64_t)K * N + N;
-  }
-  cache.ptr = theta16; cache.desc = d; cache.device = dev; cache.maps = *out; cache.valid = true;
-  return ESTK_OK;
-}
-
-int tc_supported(const estk_mlp_desc& d, int B, int cg, const char** why, int mode = kModeBF16) {
+int tc_supported(const estk_mlp_desc& d, int B, const char** why, int mode) {
   if (mode == kModeF16 && d.n_layers >= 1 && 2 * d.dims[0] > kMaxW) {
     *why = "fp16 mode splits the observations into hi + lo halves: input width <= 256"; return 0;
   }
@@ -769,44 +386,27 @@ int tc_supported(const estk_mlp_desc& d, int B, int cg, const char** why, int mo
     const int N = d.dims[l + 1];
     if (N % 32 || N > kMaxW || N < 32) { *why = "layer output width must be a multiple of 32 in [32,512]"; return 0; }
   }
-  if (B % (128 * cg)) { *why = "batch must be a multiple of 256"; return 0; }
+  if (B % 256) { *why = "batch must be a multiple of 256"; return 0; }
   return 1;
 }
 
 int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who) {
   const char* why = "";
-  const int cg = 2;
-  if (!tc_supported(p.desc, p.B, cg, &why, p.mode)) {
-    estk_set_error("%s: shape not supported by the tcgen05 path (%s)", who, why);
+  if (!tc_supported(p.desc, p.B, &why, p.mode)) {
+    estk_set_error("%s: shape not supported by the tensor-core path (%s)", who, why);
     return ESTK_ERR_UNSUPPORTED;
   }
   ESTK_CHECK_ARG(p.pairs >= 1 && p.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, p.pairs);
-  p.chunks = p.B / (128 * cg);
-  ESTK_CHECK_ARG(p.chunks * cg <= kEvalMaxChunks, "%s: batch too large", who);
+  p.chunks = p.B / kRows;
+  ESTK_CHECK_ARG(p.chunks <= 2 * kEvalMaxChunks, "%s: batch too large", who);
   p.n_centre = p.centre_out ? p.chunks : 0;
   ESTK_CHECK_ARG(!p.centre_out || p.pairs * 2 < ESTK_MAX_POPULATION, "%s: population too large to fold the centre task", who);
   p.n_tasks = p.n_centre + p.pairs * p.n_signs * p.chunks;
-#ifdef ESTK_TC_PROFILE
-  { const char* e = getenv("ESTK_TC_DEBUG"); p.dbg = e ? atoi(e) : 0; }
-#endif
   p.partial = ctx->eval_partial;
   p.counters = ctx->counters;
-  // B ring depth: bf16s runs 4 producer groups and wants the 5 stages that fit beside the
-  // 128 KB of activations (ESTK_TC_RING=4|5 overrides; perf triage only)
-#ifdef ESTK_TC_PROFILE
-  static const int ring_env = [] { const char* e = getenv("ESTK_TC_RING"); return e ? atoi(e) : 0; }();
-#else
-  constexpr int ring_env = 0;
-#endif
-  static thread_local TcMaps maps;
-  if (p.mode == kModeF16)
-    return ring_env == 4 ? launch_tc<2, kModeF16, 4>(ctx, p, &maps, stream) : launch_tc<2, kModeF16, 5>(ctx, p, &maps, stream);
-  if (p.theta16) {
-    const int rc = build_theta_maps(p.desc, p.theta16, cg, &maps);
-    if (rc != ESTK_OK) return rc;
-    return ring_env == 4 ? launch_tc<2, kModeBF16S, 4>(ctx, p, &maps, stream) : launch_tc<2, kModeBF16S, 5>(ctx, p, &maps, stream);
-  }
-  return ring_env == 5 ? launch_tc<2, kModeBF16, 5>(ctx, p, &maps, stream) : launch_tc<2, kModeBF16, 4>(ctx, p, &maps, stream);
+  if (p.mode == kModeF16) return launch_tc<kModeF16>(ctx, p, stream);
+  if (p.mode == kModeBF16S) return launch_tc<kModeBF16S>(ctx, p, stream);
+  return launch_tc<kModeBF16>(ctx, p, stream);
 }
 
 }  // namespace
@@ -827,7 +427,7 @@ extern "C" int estk_eval_mlp_bf16(estk_ctx* ctx, const estk_mlp_desc* desc, cons
   p.pairs = pairs; p.sigma = sigma; p.obs = obs; p.target = target; p.B = B;
   p.ret_plus = returns_plus; p.ret_minus = returns_minus;
   p.bc_plus = bc_plus; p.bc_minus = bc_minus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 2; p.centre_out = centre_return_out;
+  p.n_signs = 2; p.centre_out = centre_return_out; p.mode = kModeBF16;
   return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_bf16");
 }
 
@@ -841,7 +441,7 @@ extern "C" int estk_eval_mlp_center_bf16(estk_ctx* ctx, const estk_mlp_desc* des
   p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
   p.ret_plus = return_out; p.ret_minus = nullptr;
   p.bc_plus = bc_out; p.bc_minus = nullptr; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 1;
+  p.n_signs = 1; p.mode = kModeBF16;
   return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center_bf16");
 }
 
@@ -905,22 +505,6 @@ extern "C" int estk_eval_mlp_center_bf16s(estk_ctx* ctx, const estk_mlp_desc* de
 }
 
 // ---- fp16 operands from fp32 theta + the exact 16-bit noise table (the default tensor-core mode).
-// The product kernel is the warpgroup-specialised one in estk_eval_mlp_f16.cu; the kModeF16
-// instantiation of the kernel above is kept as an A/B reference (ESTK_F16_V1=1, triage only).
-int estk_f16v2_supported(const estk_mlp_desc* desc, int B);
-int estk_f16v2_eval(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta, const float* table,
-                    const uint16_t* table16, const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
-                    const float* obs, const float* target, int32_t B, float* returns_plus, float* returns_minus,
-                    float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim, float* centre_return_out,
-                    int n_signs, cudaStream_t stream, const char* who);
-static bool f16_use_v1() {
-#ifdef ESTK_TC_PROFILE
-  static const bool v1 = [] { const char* e = getenv("ESTK_F16_V1"); return e && atoi(e) != 0; }();
-  return v1;
-#else
-  return false;
-#endif
-}
 __global__ void __launch_bounds__(256) shadow_f16_kernel(const float4* __restrict__ src, uint2* __restrict__ dst, int64_t n4,
                                                          unsigned long long* __restrict__ inexact) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -961,10 +545,6 @@ extern "C" int estk_eval_mlp_f16(estk_ctx* ctx, const estk_mlp_desc* desc, const
   ESTK_CHECK_ARG((bc_plus == nullptr) == (bc_minus == nullptr), "estk_eval_mlp_f16: bc_plus/bc_minus must both be set or both null");
   ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(table) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target) &&
                  ESTK_ALIGNED16(table16), "estk_eval_mlp_f16: buffers must be 16-byte aligned");
-  if (!f16_use_v1())
-    return estk_f16v2_eval(ctx, desc, theta, table, table16, offsets, order, pairs, sigma, obs, target, B, returns_plus,
-                           returns_minus, bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, 2, (cudaStream_t)stream,
-                           "estk_eval_mlp_f16");
   EvalTCParams p = {};
   p.desc = *desc; p.theta = theta; p.table = table; p.table16 = table16;
   p.offsets = offsets; p.order = order;
@@ -981,9 +561,6 @@ extern "C" int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc
   ESTK_CHECK_ARG(ctx && desc && theta && obs && target && return_out, "estk_eval_mlp_center_f16: null argument");
   ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target),
                  "estk_eval_mlp_center_f16: buffers must be 16-byte aligned");
-  if (!f16_use_v1())
-    return estk_f16v2_eval(ctx, desc, theta, theta, nullptr, nullptr, nullptr, 1, 0.f, obs, target, B, return_out, nullptr,
-                           bc_out, nullptr, bc_obs, bc_dim, nullptr, 1, (cudaStream_t)stream, "estk_eval_mlp_center_f16");
   EvalTCParams p = {};
   p.desc = *desc; p.theta = theta; p.table = theta; p.offsets = nullptr; p.order = nullptr;
   p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
@@ -995,22 +572,10 @@ extern "C" int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc
 
 extern "C" int estk_eval_mlp_f16_supported(const estk_mlp_desc* desc, int32_t B) {
   const char* why = "";
-  if (desc && !f16_use_v1()) return estk_f16v2_supported(desc, B);
-  return desc ? tc_supported(*desc, B, 2, &why, kModeF16) : 0;
+  return desc ? tc_supported(*desc, B, &why, kModeF16) : 0;
 }
 
 extern "C" int estk_eval_mlp_bf16_supported(const estk_mlp_desc* desc, int32_t B) {
   const char* why = "";
-  return desc ? tc_supported(*desc, B, 2, &why) : 0;
+  return desc ? tc_supported(*desc, B, &why, kModeBF16) : 0;
 }
-
-#ifdef ESTK_TC_PROFILE
-// triage builds only (not part of estk.h): read and clear the cycle counters written when ESTK_TC_DEBUG has bit 8
-extern "C" __attribute__((visibility("default"))) int estk_debug_tc_profile(unsigned long long* host_out, int n) {
-  if (n > 32) n = 32;
-  cudaDeviceSynchronize();
-  if (cudaMemcpyFromSymbol(host_out, g_tc_prof, sizeof(unsigned long long) * n) != cudaSuccess) return -1;
-  unsigned long long zeros[32] = {};
-  return cudaMemcpyToSymbol(g_tc_prof, zeros, sizeof(zeros)) == cudaSuccess ? 0 : -1;
-}
-#endif

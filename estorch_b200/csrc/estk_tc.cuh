@@ -1,35 +1,23 @@
-// estk_tc.cuh -- raw PTX wrappers shared by the tcgen05 evaluate kernels (sm_100a):
-// mbarriers, cluster ranks, TMA, tcgen05 alloc / mma / commit / ld / st, UMMA descriptors,
-// the 128B-swizzle address map and the 16-bit packing conversions.
+// estk_tc.cuh -- raw PTX wrappers shared by the tensor-core evaluate kernel (sm_90a):
+// mbarriers, warpgroup MMA (wgmma) and its shared-memory descriptors, the 128B-swizzle address
+// map and the 16-bit packing conversions.
 #pragma once
 #include "estk_common.cuh"
-#include <cuda.h>          // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 namespace {
 
-constexpr int kMaxW = 512;            // max layer width (K and N) of the tensor-core paths
+constexpr int kMaxW = 512;            // max layer width (K and N) of the tensor-core path
 constexpr int kBlockK = 64;           // 16-bit elements per 128-byte swizzle row
-constexpr int kKBlockBytes = 128 * kBlockK * 2;   // one [128 x 64] 16-bit tile = 16 KB
 
 // ------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
-// mbarrier waits use the CTA-scope form: ptxas pairs a cluster-scope acquire with
-// CCTL.IVALL (L1 invalidate + drain of outstanding loads)
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -41,137 +29,57 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "DONE:\n"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-template <int CG>
-__device__ __forceinline__ void mbar_arrive_on(uint32_t bar, uint32_t cta) {
-  if constexpr (CG == 1) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-  } else {
-    asm volatile(
-        "{\n"
-        ".reg .b32 ra;\n"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n"
-        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
-        "}" ::"r"(bar), "r"(cta) : "memory");
-  }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// 2-D tiled TMA load into this CTA's shared memory, completion on this CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-// generic-proxy st.shared -> visible to the async proxy (tensor core reads of smem)
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}" : "=r"(pred));
-  return pred != 0;
-}
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32
-template <int CG>
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b),
-        "r"(idesc), "r"(accumulate) : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b),
-        "r"(idesc), "r"(accumulate) : "memory");
-  }
-}
-// all previously issued MMAs complete -> arrive (once) on `bar` in every CTA of the pair
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-  } else {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-  }
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 16 packed-bf16x2 words per lane back into TMEM (the activation stash, see the epilogue)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      :: "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-         "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// generic-proxy st.shared -> visible to the async proxy (wgmma reads of smem)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// 256-bit streaming load (sm_100: LDG.E.256): a whole 32-byte sector per thread; p 32-byte aligned
-__device__ __forceinline__ void ld_noise8(const float* p, float (&v)[8]) {
-  asm volatile("ld.global.nc.L1::no_allocate.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
-}
 __device__ __forceinline__ uint4 ld_noise4u(const uint4* p) {
   uint4 v;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
   return v;
 }
 
-// UMMA shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row atoms 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-//  version=1 [46,48), layout_type=SWIZZLE_128B(2) [61,64)).
+// wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row core-matrix groups 1024 B apart
+// (start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major), SBO>>4 [32,46), layout 1 = 128B swizzle [62,64))
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1<<4), a/b format BF16 (1<<7, 1<<10),
-// K-major A and B, n_dim = N>>3 at [17,23), m_dim = M>>4 at [24,29).
-// (a/b format 0 = F16, 1 = BF16)
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, bool f16) {
-  const uint32_t fmt = f16 ? 0u : ((1u << 7) | (1u << 10));
-  return (1u << 4) | fmt | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// byte offset of the 16-byte chunk (row r, chunk c8 of 8 bf16) inside a swizzled [rows x 64] tile
+// byte offset of the 16-byte chunk (row r, chunk c8 of 8 16-bit values) inside a swizzled [rows x 64] tile
 __device__ __forceinline__ uint32_t sw128_offset(int r, int c8) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c8 ^ (r & 7)) << 4));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+__device__ __forceinline__ void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both operands K-major in shared memory, fp32 accumulators;
+// 16-bit operands: fp16 (F16) or bf16
+template <bool F16>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define ESTK_WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define ESTK_WG_ASM(TYPE)                                                                                        \
+  asm volatile(                                                                                                  \
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"                                                                \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " "                                           \
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,"  \
+      "%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53," \
+      "%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"                                     \
+      : ESTK_WG_D8(0), ESTK_WG_D8(8), ESTK_WG_D8(16), ESTK_WG_D8(24), ESTK_WG_D8(32), ESTK_WG_D8(40),            \
+        ESTK_WG_D8(48), ESTK_WG_D8(56)                                                                           \
+      : "l"(da), "l"(db), "r"(accumulate))
+  if constexpr (F16) ESTK_WG_ASM("f16");
+  else ESTK_WG_ASM("bf16");
+#undef ESTK_WG_ASM
+#undef ESTK_WG_D8
 }
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   uint32_t r;
@@ -219,6 +127,9 @@ __device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
 

@@ -4,7 +4,7 @@ Same class names, constructor signatures, ``train`` / ``terminate`` / ``log``
 API, overridable hooks and public attributes as the reference (SURVEY 8b), but
 the body of a generation runs on the GPU through the C ABI in include/estk.h:
 
-    reference (CPU, estorch.py)                 here (B200)
+    reference (CPU, estorch.py)                 here (H100)
     -------------------------------------------  ------------------------------------------
     _sample_policy :187-193  fresh RNG + cats    noise-table offsets (estk_make_offsets)
     MPI Send/Recv of P x n rows :207-233         nothing to send: every rank regenerates rows
@@ -93,8 +93,7 @@ _EXIT_HOOK = False
 
 def _shutdown_dist():
     """Process exit of a multi-GPU rank.  A CUDA graph that captured NCCL kernels keeps a reference on
-    the communicator, and destroying the communicator first never returns
-    (profiles/r02_launcher_check.log, first run): graphs go first, then the mappings of the peers'
+    the communicator, and destroying the communicator first never returns: graphs go first, then the mappings of the peers'
     workspaces, then -- if this module created it -- the process group.  A script that destroys the process group itself calls ``es.close()`` (or drops the
     instance) first."""
     import gc
@@ -220,7 +219,7 @@ class ES:
             reference behaviour).
         eval_precision: arithmetic of the fused evaluate kernel:
             ``"fp32"``  CUDA-core path, fp32 throughout;
-            ``"f16"``   tcgen05 tensor cores with fp16 operands (11-bit significand, the
+            ``"f16"``   wgmma tensor cores with fp16 operands (11-bit significand, the
                         TF32 class) and fp32 accumulation; every weight is formed in fp32
                         from the fp32 theta and the (exactly 16-bit representable) noise
                         value and rounded once; observations enter as hi + lo halves;
@@ -1148,7 +1147,7 @@ class ES:
         """
         self.n_steps = n_steps
         if hostfile is not None:
-            raise NotImplementedError("hostfile (multi-node MPI launch) has no B200 single-box equivalent")
+            raise NotImplementedError("hostfile (multi-node MPI launch) has no single-box equivalent here")
         if n_proc > 1:
             if self._trained:
                 raise RuntimeError("train function can not be called more than once.")

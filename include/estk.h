@@ -1,5 +1,5 @@
 /*
- * estk.h -- C ABI of the B200 Evolution-Strategies kernel library (libestk.so).
+ * estk.h -- C ABI of the H100 Evolution-Strategies kernel library (libestk.so).
  *
  * This is the drop-in boundary for the ES generation hot path of
  * goktug97/estorch (estorch/estorch.py:211-250, ES._master).  The reference has
@@ -135,7 +135,7 @@ ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, const float
                   void* stream);
 
 /* Opt-in lower-precision tensor-core variant of estk_eval_mlp: same contract, bf16 operands with fp32
- * accumulation on tcgen05 (weights theta+-sigma*eps are rounded to bf16 when the
+ * accumulation on wgmma (weights theta+-sigma*eps are rounded to bf16 when the
  * B-operand tile is formed, activations when they are written back).  Shapes:
  * every layer input width a multiple of 64 in [64,512], every output width a
  * multiple of 32 in [32,512], B a multiple of 256; otherwise
@@ -157,7 +157,7 @@ ESTK_API int estk_eval_mlp_center_bf16(estk_ctx* ctx, const estk_mlp_desc* desc,
 ESTK_API int estk_eval_mlp_bf16_supported(const estk_mlp_desc* desc, int32_t B);
 
 /* DEFAULT tensor-core evaluate ("f16"): same contract as estk_eval_mlp, computed on
- * tcgen05 with fp16 operands (11-bit significand, the TF32 class) and fp32 accumulation.
+ * wgmma with fp16 operands (11-bit significand, the TF32 class) and fp32 accumulation.
  * Every weight is formed in fp32 from the fp32 theta and the noise value and rounded ONCE:
  *   W16 = rn_f16(theta + s*sigma*T[off+i])      (sum in fp32, like estorch.py:192)
  * The noise is streamed from table16, a 16-bit copy of `table` that must be EXACT
@@ -167,8 +167,8 @@ ESTK_API int estk_eval_mlp_bf16_supported(const estk_mlp_desc* desc, int32_t B);
  * table) weights.  Hidden activations are rounded to fp16 when written back (saturating
  * at +-65504), the observations enter as x_hi + x_lo (two fp16 operands), biases and the
  * squared error are fp32.  Shapes as estk_eval_mlp_bf16, plus dims[0] <= 256
- * (estk_eval_mlp_f16_supported()).  Measured agreement with the fp32 path: see
- * tests/test_kernels_gpu.py::test_eval_mlp_f16_* and profiles/. */
+ * (estk_eval_mlp_f16_supported()).  Agreement with the fp32 path: asserted in
+ * tests/test_kernels_gpu.py::test_eval_mlp_f16_*. */
 ESTK_API int estk_shadow_f16(estk_ctx* ctx, const float* src, uint16_t* dst, int64_t n,
                     uint64_t* inexact_count /* device, nullable: += #entries that changed */,
                     void* stream);
@@ -187,9 +187,8 @@ ESTK_API int estk_eval_mlp_f16_supported(const estk_mlp_desc* desc, int32_t B);
 
 /* NOTE on "bf16s": it evaluates F(theta16 +- sigma16 * eps16) while estk_rank_grad* weights the fp32 eps --
  * the estimator multiplies a return by a noise vector that is not exactly the one that produced it
- * (estorch.py:177-178 uses the same eps on both sides).  Measured at the north-star size
- * (profiles/r02_north_star_precision.json): returns 1.6e-5 off the fp32 arithmetic, gradient 5.6e-3 (L2)
- * off the one computed from fp32 returns.  The default mode ("f16") has neither departure.
+ * (estorch.py:177-178 uses the same eps on both sides).  The default mode ("f16") has no such
+ * departure.
  * "bf16s" (opt-in, lower precision): as estk_eval_mlp_bf16, but the weight producers read bf16 SHADOWS of
  * theta and of the noise table (theta16[i] = bf16(theta[i]), table16[i] =
  * bf16(table[i]), built with estk_shadow_bf16) -- half the bytes per weight

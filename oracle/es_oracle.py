@@ -199,7 +199,7 @@ def round_bf16(x: np.ndarray) -> np.ndarray:
 
 
 def mlp_forward_bf16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Numerics of the tcgen05 evaluate path (estk_eval_mlp_bf16): weights and
+    """Numerics of the wgmma evaluate path (estk_eval_mlp_bf16): weights and
     layer inputs rounded to bf16, products accumulated in fp32, bias / ReLU in
     fp32.  ``flat`` is the already-perturbed fp32 row."""
     h = round_bf16(np.asarray(obs, dtype=np.float32))

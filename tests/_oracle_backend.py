@@ -18,7 +18,7 @@ class OracleBackend:
     name = "oracle"
 
     def __init__(self, tensor_core=False):
-        """``tensor_core=True`` also emulates the tcgen05 evaluate modes ("bf16" / "bf16s",
+        """``tensor_core=True`` also emulates the wgmma evaluate modes ("bf16" / "bf16s",
         with the oracle's bf16 rounding model) so that the host logic around them -- shadows,
         the folded post-update rollout -- runs on CPU."""
         self.device = torch.device("cpu")

@@ -1,4 +1,4 @@
-"""A small pass over the hot kernels for compute-sanitizer (memcheck / racecheck / synccheck): the tcgen05 evaluate
+"""A small pass over the hot kernels for compute-sanitizer (memcheck / racecheck / synccheck): the wgmma evaluate
 (default f16 mode, two-tile and one-tile layers, a folded centre task), the fp16-table rank+reduce+Adam and the
 multi-GPU form, each checked against the oracle so that a sanitizer run is also a correctness run."""
 import os, sys, numpy as np, torch

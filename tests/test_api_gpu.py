@@ -1,4 +1,4 @@
-"""The public API on a real B200, through the C ABI (no stand-in): parity with the
+"""The public API on a real H100, through the C ABI (no stand-in): parity with the
 reference-generated goldens and with the oracle."""
 import numpy as np
 import pytest

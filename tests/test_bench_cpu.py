@@ -1,5 +1,5 @@
 """bench.py contract that can be checked without a GPU: the reference arm (the unmodified reference
-from baseline/_ref when __graft_entry__.build() installed it, else the CPU port of its generation,
+from oracle/_ref when __graft_entry__.build() installed it, else the CPU port of its generation,
 oracle/reference_port.py) prints exactly ONE JSON line on stdout with
 the keys the driver reads; our own arm refuses to run without the CUDA library / a GPU."""
 import json

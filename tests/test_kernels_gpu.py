@@ -420,12 +420,12 @@ def test_track_best(be):
     assert float(best.min()) == 3.0 and float(best.max()) == 3.0
 
 
-# ------------------------------------------------------------------ tcgen05 evaluate (bf16 operands)
+# ------------------------------------------------------------------ wgmma evaluate (bf16 operands)
 @pytest.mark.parametrize("dims,B,pairs,bc", [([128, 512, 512, 288], 256, 5, 0), ([64, 64, 32], 256, 3, 0),
                                              ([128, 512, 512, 512, 512, 288], 256, 3, 0),
                                              ([64, 256, 64], 512, 4, 256), ([192, 320, 96], 256, 2, 0)])
 def test_eval_mlp_bf16_tensor_core_path(be, dims, B, pairs, bc):
-    """bf16-operand / fp32-accumulate tcgen05 path: within 5e-4 (max-norm relative) of the
+    """bf16-operand / fp32-accumulate wgmma path: within 5e-4 (max-norm relative) of the
     oracle that emulates its roundings, and within 2e-2 of the exact fp32 forward."""
     rng = np.random.RandomState(7)
     n = orc.mlp_param_count(dims)
@@ -514,7 +514,7 @@ def test_eval_mlp_bf16s_shadow_sources(be, dims, B, pairs):
     assert abs(float(one) - want) < 5e-4 * abs(want)
 
 
-# ------------------------------------------------------------------ tcgen05 evaluate, fp16 operands (default mode)
+# ------------------------------------------------------------------ wgmma evaluate, fp16 operands (default mode)
 def _f16_problem(dims, B, pairs, seed=23):
     rng = np.random.RandomState(seed)
     n = orc.mlp_param_count(dims)
@@ -534,7 +534,7 @@ def _f16_problem(dims, B, pairs, seed=23):
                                              ([64, 256, 64], 512, 4, 256), ([192, 320, 96], 256, 2, 0),
                                              ([256, 512, 32], 256, 2, 0)])
 def test_eval_mlp_f16_tensor_core_path(be, dims, B, pairs, bc):
-    """fp16-operand / fp32-accumulate tcgen05 path formed from fp32 theta + the exact fp16
+    """fp16-operand / fp32-accumulate wgmma path formed from fp32 theta + the exact fp16
     noise table: within 1e-5 (max-norm relative) of the oracle that emulates its roundings and
     within 3e-5 of the EXACT fp32 forward (estorch.py:195-202 + cartpole_es.py:14-20)."""
     n, table, theta, obs, tgt, offs = _f16_problem(dims, B, pairs)

@@ -1,7 +1,8 @@
 """Drop-in check: the reference's own example scripts run against this package.
 
-The scripts are READ at test time from /root/reference/examples (never copied into the
-repo; the tests skip where the reference is not mounted, e.g. on the GPU box).  They are
+The scripts are READ at test time from oracle/_ref/examples, where ``__graft_entry__.build()``
+installs the reference (never copied into the repo's sources; the tests skip where build() had no
+reference source tree to install).  They are
 executed with ``import estorch`` resolving to ``estorch_b200``, a stand-in ``gym`` (the image
 has no gym) and the CPU stand-in backend of tests/_oracle_backend.py.  Only the launch
 parameters are rewritten (``n_proc=2`` would re-exec under torchrun, hundreds of steps
@@ -19,9 +20,9 @@ import torch
 
 import estorch_b200
 from _oracle_backend import OracleBackend
+from oracle.ref_shim import REF_EXAMPLES as EXAMPLES
 
-EXAMPLES = "/root/reference/examples"
-pytestmark = pytest.mark.skipif(not os.path.isdir(EXAMPLES), reason="reference examples are not mounted here")
+pytestmark = pytest.mark.skipif(not os.path.isdir(EXAMPLES), reason="build() installed no reference examples here")
 
 
 class _Space:

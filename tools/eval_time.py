@@ -1,4 +1,4 @@
-"""Time the tcgen05 evaluate kernel alone at the north-star shape (CUDA events, ms per launch)."""
+"""Time the wgmma evaluate kernel alone at the north-star shape (CUDA events, ms per launch)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from estorch_b200.backend import CudaBackend

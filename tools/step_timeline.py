@@ -51,7 +51,7 @@ def wrap(owner, name, label):
 os.environ["ESTORCH_B200_GRAPH"] = "0"
 es = build()
 es.train(5)
-for name, label in (("make_offsets", "offset hash + sort"), ("eval_mlp", "evaluate (tcgen05)"),
+for name, label in (("make_offsets", "offset hash + sort"), ("eval_mlp", "evaluate (wgmma)"),
                     ("track_best", "best tracking"), ("rank_grad", "rank + partial gradient"),
                     ("rank_grad_adam", "rank + gradient + Adam"), ("clamp_adam", "clamp + Adam"),
                     ("rank_grad_xr_adam", "rank + gradient + NVLink sum + Adam")):
