@@ -5,12 +5,17 @@
 // Policy.forward examples/cartpole_es.py:14-20 + synthetic agent of SURVEY 8d),
 // for policies whose dense layers are worth a GEMM.
 //
-// Work unit ("task") = (antithetic pair j, sign s, chunk of 64 observations), one CTA.  Per layer
+// Work unit ("task") = (antithetic pair j, sign s, chunk of 64 observations), one CTA.  A cluster of
+// four CTAs runs the four consecutive chunks of one (j, s) -- the same weights -- at the same time.
+// Per layer
 //   D[obs, out] = H[obs, in] * W_s[out, in]^T       (wgmma m64n128k16, N tiles of 128)
 //   A  activations H, 64 rows, 16-bit, K-major, 128B-swizzled, resident in shared memory:
 //      two buffers (64 KB each) swapped per layer, so a layer's output never overwrites its input;
 //   B  W_s = theta + s*sigma*eps, formed ON THE FLY by producer warps into a ring of
-//      [128 x 64] stages (16 KB) -- the perturbed weights never exist in global memory;
+//      [128 x 64] stages (16 KB) -- the perturbed weights never exist in global memory.  CTA q of
+//      the cluster forms tile rows [q*w/4, (q+1)*w/4) of each stage and copies them into the same
+//      slot of the other three CTAs (cp.async.bulk over distributed shared memory), so every weight
+//      is read from L2 and formed once per 256 observations;
 //   D  64 x 128 fp32 in the registers of the consumer warpgroup; the epilogue adds the bias,
 //      applies ReLU and rounds to 16 bits straight into the other activation buffer.  The last
 //      layer is fused with the squared-error reduction (and the behaviour characterisation).
@@ -21,10 +26,12 @@
 //               16-bit copy of the noise table: W16 = rn_f16(theta + s*sigma*eps), sum in fp32; the
 //               observations enter layer 0 as x_hi + x_lo (two fp16 k-block sets, same B tile)
 // Warp roles: warpgroup 0 = consumer (MMA issue + epilogue), warps 4..11 = weight producers in
-// two groups of four, each group forming every other stage of the flattened
-// (task, layer, N tile, k-block) sequence.  full / empty mbarriers per ring stage.  Persistent:
-// CTAs loop over tasks; the two signs of a pair run on neighbouring CTAs at the same time, so
-// the second read of the noise row is an L2 hit.
+// four groups of two, each group forming every fourth stage of the flattened
+// (task, layer, N tile, k-block) sequence.  full / empty mbarriers per ring stage: full[s] completes
+// on the local group's arrival plus the bytes the three peers copy in; empty[s] counts the consumer
+// warps of all four CTAs, because a producer writes slot s of every CTA.  Persistent: clusters loop
+// over groups of four tasks; the two signs of a pair run on neighbouring clusters at the same time,
+// so the second read of the noise row is an L2 hit.
 #include "estk_tc.cuh"
 #include <type_traits>
 
@@ -36,9 +43,16 @@ constexpr int kHBlockBytes = kRows * kBlockK * 2;  // one [64 x 64] 16-bit k-blo
 constexpr int kHBytes = (kMaxW / kBlockK) * kHBlockBytes;   // 64 KB per activation buffer
 constexpr int kStageBytes = kTileN * kBlockK * 2;  // one [128 x 64] 16-bit B stage = 16 KB
 constexpr int kStages = 5;
-constexpr int kProdWarps = 8, kProdGroups = 2, kProdGroupWarps = kProdWarps / kProdGroups;
+constexpr int kCluster = 4;                        // CTAs (observation chunks) sharing every B stage
+constexpr int kProdWarps = 8, kProdGroups = 4, kProdGroupWarps = kProdWarps / kProdGroups;
 constexpr int kPT = 32 * kProdGroupWarps;          // threads per producer group
 constexpr int kThreadsTC = 128 + 32 * kProdWarps;  // 384
+// A group waits for the release of the slot it is about to fill, kStages stages back; its previous
+// stage, kProdGroups back, already saw the release before that.  So no group runs a full phase ahead of
+// an empty barrier, which a parity wait could not tell apart.
+static_assert(kProdGroups <= kStages, "parity waits need kProdGroups <= kStages");
+// 16-byte items per producer thread per stage: the CTA's quarter of the widest tile, in one batch
+constexpr int kItemsPT = kTileN / kCluster * (kBlockK / 8) / kPT;
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
 
 struct EvalTCParams {
@@ -100,8 +114,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   const int L = p.desc.n_layers;
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(smem_u32(bar_full + s), kProdGroupWarps);
-      mbar_init(smem_u32(bar_empty + s), 4);
+      mbar_init(smem_u32(bar_full + s), 1);                // the forming group's elected thread (+ peer bytes)
+      mbar_init(smem_u32(bar_empty + s), 4 * kCluster);    // every consumer warp of the cluster
     }
     fence_barrier_init();
     int64_t pb = 0;
@@ -113,7 +127,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
       pb = lay[l].bbase + lay[l].N;
     }
   }
-  __syncthreads();
+  cluster_sync();   // barriers initialised in every CTA before any remote arrive or copy
   const bool centre = (p.offsets == nullptr);
 
   if (warp < 4) {
@@ -122,6 +136,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
     const int r0 = warp * 16 + (lane >> 2);          // accumulator rows r0 and r0 + 8
     const int cq = (lane & 3) * 2;                   // accumulator columns 8j + cq, +1
     uint32_t kst = 0;                                // global stage index
+    // gridDim.x and chunks (B % 256 == 0) are multiples of kCluster: the CTAs of a cluster always hold
+    // the kCluster consecutive chunks of one (pair, sign), CTA rank = chunk % kCluster
     for (int task = blockIdx.x; task < p.n_tasks; task += gridDim.x) {
       const TaskId tk = decode_task(p, task, centre);
       const int chunk = tk.chunk, sgn = tk.sgn, slot = tk.slot;
@@ -185,7 +201,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
               }
               wgmma_commit();
               wgmma_wait<1>();             // the previous stage's MMAs are done: release its slot
-              if (kb > 0 && lane == 0) mbar_arrive(smem_u32(bar_empty + prev));
+              if (kb > 0 && lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
               prev = stage;
             }
           };
@@ -193,7 +209,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           else k_loop(std::integral_constant<int, 1>{});
           wgmma_wait<0>();
           fence_acc(d);
-          if (lane == 0) mbar_arrive(smem_u32(bar_empty + prev));
+          if (lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
           // ---- epilogue of the tile
 #pragma unroll
           for (int jb = 0; jb < kTileN / 8; ++jb) {
@@ -252,11 +268,13 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   } else {
     // =================================================================== weight producers
     // Group g forms stages g, g+G, g+2G, ... of the flattened (task, layer, N tile, k-block)
-    // sequence.  Item `it` of a stage = tile row it/8, 16-byte output chunk it%8 (8 weights).
+    // sequence, this CTA's quarter of each: tile rows [rank*w/4, (rank+1)*w/4).  w % 32 == 0, so a
+    // quarter is whole 8-row swizzle atoms, one contiguous 1024-B-aligned byte range of the stage.
+    // Item `it` of the quarter = its row it/8, 16-byte output chunk it%8 (8 weights).
     const int pwarp = warp - 4;
     const int pgroup = pwarp / kProdGroupWarps;
     const int ptid = (pwarp % kProdGroupWarps) * 32 + lane;
-    constexpr int kBatch = (MODE == kModeBF16) ? 4 : 8;    // items whose loads are in flight together
+    const uint32_t rank = cluster_ctarank();
     int cached_task = -1;
     const float* trow = p.theta;
     const uint16_t* trow16 = nullptr;
@@ -288,16 +306,17 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
       const uint32_t stage = kst % kStages, phase = (kst / kStages) & 1u;
       const uint32_t sbase = smem_u32(sB + stage * kStageBytes);
       const int K = lay[l].K;
-      const int n_items = min(kTileN, lay[l].N - n0) * 8;
-      const int64_t rbase = lay[l].wbase + (int64_t)n0 * K + kb * kBlockK;
-      bool waited = false;
-      for (int it0 = 0; it0 < n_items; it0 += kBatch * kPT) {
-        float4 th[kBatch][2], ep[kBatch][2];
-        uint4 t16[kBatch], e16[kBatch];
-        // every load of the batch is issued up front ...
+      const int qrows = min(kTileN, lay[l].N - n0) / kCluster;
+      const int n_items = qrows * 8;
+      const uint32_t qbase = sbase + rank * qrows * 128, qbytes = qrows * 128;
+      const int64_t rbase = lay[l].wbase + (int64_t)(n0 + rank * qrows) * K + kb * kBlockK;
+      {
+        float4 th[kItemsPT][2], ep[kItemsPT][2];
+        uint4 t16[kItemsPT], e16[kItemsPT];
+        // every load of the stage is issued up front ...
 #pragma unroll
-        for (int u = 0; u < kBatch; ++u) {
-          const int it = it0 + u * kPT + ptid;
+        for (int u = 0; u < kItemsPT; ++u) {
+          const int it = u * kPT + ptid;
           if (it < n_items) {
             const int64_t off = rbase + (int64_t)(it >> 3) * K + (it & 7) * 8;
             if constexpr (S16) {
@@ -315,14 +334,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
             }
           }
         }
-        // ... then wait for the ring slot
-        if (!waited) {
-          mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
-          waited = true;
-        }
+        // ... then wait for the ring slot, free in all four CTAs
+        mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
 #pragma unroll
-        for (int u = 0; u < kBatch; ++u) {
-          const int it = it0 + u * kPT + ptid;
+        for (int u = 0; u < kItemsPT; ++u) {
+          const int it = u * kPT + ptid;
           if (it < n_items) {
             const float sg = ssig;
             uint32_t w[4];
@@ -346,18 +362,31 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
               w[2] = pack_bf16(fmaf(sg, ep[u][1].x, th[u][1].x), fmaf(sg, ep[u][1].y, th[u][1].y));
               w[3] = pack_bf16(fmaf(sg, ep[u][1].z, th[u][1].z), fmaf(sg, ep[u][1].w, th[u][1].w));
             }
-            st_shared_v4(sbase + sw128_offset(it >> 3, it & 7), w[0], w[1], w[2], w[3]);
+            st_shared_v4(qbase + sw128_offset(it >> 3, it & 7), w[0], w[1], w[2], w[3]);
           }
         }
       }
-      if (!waited) mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(bar_full + stage));
+      fence_proxy_async();                  // the quarter -> async proxy (local wgmma, bulk copies)
+      named_bar_sync(2 + pgroup, kPT);
+      if (ptid == 0) {
+        // full[stage] of this CTA: this arrival + the three quarters the peers copy in.  A peer's
+        // bytes may land before the expect_tx (the transaction count goes negative meanwhile); the
+        // phase cannot complete before this arrival either way.
+        const uint32_t full = smem_u32(bar_full + stage);
+        mbar_arrive_expect_tx(full, (kCluster - 1) * qbytes);
+        for (uint32_t r = 1; r < kCluster; ++r) {
+          const uint32_t peer = (rank + r) % kCluster;
+          bulk_copy_to_cluster(mapa_shared(qbase, peer), qbase, qbytes, mapa_shared(full, peer));
+        }
+      }
       for (int sk = 0; sk < kProdGroups && has; ++sk) has = advance();
       kst += kProdGroups;
     }
   }
+  // No CTA leaves while a peer may still arrive on its barriers or copy into its ring: every copy into
+  // this CTA completed on its full barriers before its consumer finished, and every peer reaches this
+  // point only after its last remote arrival.
+  cluster_sync();
 }
 
 size_t tc_smem_bytes() {
@@ -365,13 +394,34 @@ size_t tc_smem_bytes() {
          2 * kStages * sizeof(uint64_t) + 4 * sizeof(float);
 }
 
+// Clusters of kCluster CTAs, one per SM, persistent over groups of kCluster tasks.  The number of
+// clusters that fit at once comes from the occupancy API: the GPCs' SM counts need not be multiples of
+// kCluster, so it can be less than sm_count / kCluster.
 template <int MODE>
-int launch_tc(estk_ctx* ctx, const EvalTCParams& p, cudaStream_t stream) {
+int launch_tc(const EvalTCParams& p, cudaStream_t stream) {
   const size_t smem = tc_smem_bytes();
   ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = ctx->sm_count < p.n_tasks ? ctx->sm_count : p.n_tasks;
-  eval_mlp_tc_kernel<MODE><<<grid, kThreadsTC, smem, stream>>>(p);
-  ESTK_CUDA(cudaGetLastError());
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = kCluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(kCluster);
+  cfg.blockDim = dim3(kThreadsTC);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int clusters = 0;
+  ESTK_CUDA(cudaOccupancyMaxActiveClusters(&clusters, eval_mlp_tc_kernel<MODE>, &cfg));
+  if (clusters < 1) {
+    estk_set_error("eval_mlp_tc_kernel: no cluster of %d CTAs fits on this device", kCluster);
+    return ESTK_ERR_CUDA;
+  }
+  const int items = p.n_tasks / kCluster;
+  cfg.gridDim = dim3(kCluster * (clusters < items ? clusters : items));
+  ESTK_CUDA(cudaLaunchKernelEx(&cfg, eval_mlp_tc_kernel<MODE>, p));
   return ESTK_OK;
 }
 
@@ -404,9 +454,9 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
   p.n_tasks = p.n_centre + p.pairs * p.n_signs * p.chunks;
   p.partial = ctx->eval_partial;
   p.counters = ctx->counters;
-  if (p.mode == kModeF16) return launch_tc<kModeF16>(ctx, p, stream);
-  if (p.mode == kModeBF16S) return launch_tc<kModeBF16S>(ctx, p, stream);
-  return launch_tc<kModeBF16>(ctx, p, stream);
+  if (p.mode == kModeF16) return launch_tc<kModeF16>(p, stream);
+  if (p.mode == kModeBF16S) return launch_tc<kModeBF16S>(p, stream);
+  return launch_tc<kModeBF16>(p, stream);
 }
 
 }  // namespace

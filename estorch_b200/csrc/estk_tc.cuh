@@ -29,10 +29,40 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "DONE:\n"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+
+// ---- thread-block clusters: distributed shared memory, remote mbarriers, bulk copies between CTAs
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; release/acquire orders shared-memory accesses around it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the shared::cluster address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// arrive on an mbarrier of any CTA of the cluster (`bar` from mapa_shared).  Default (.release.cta)
+// semantics: enough to release a slot whose reads have completed (wgmma.wait_group).  It publishes
+// no data, and .release.cluster would put a GPU-scope memory barrier in front of every arrival.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// arrive and raise the phase's expected transaction bytes
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// async-proxy copy of `bytes` (multiple of 16) from this CTA's shared memory to `dst` in a CTA of the
+// cluster; completes `bytes` transactions on the mbarrier `bar` of that CTA (both from mapa_shared)
+__device__ __forceinline__ void bulk_copy_to_cluster(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "r"(src), "r"(bytes), "r"(bar) : "memory");
+}
 // generic-proxy st.shared -> visible to the async proxy (wgmma reads of smem)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
