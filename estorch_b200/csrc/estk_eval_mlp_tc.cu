@@ -53,6 +53,7 @@ constexpr int kThreadsTC = 128 + 32 * kProdWarps;  // 384
 static_assert(kProdGroups <= kStages, "parity waits need kProdGroups <= kStages");
 // 16-byte items per producer thread per stage: the CTA's quarter of the widest tile, in one batch
 constexpr int kItemsPT = kTileN / kCluster * (kBlockK / 8) / kPT;
+constexpr int kTgtBatch = 4;                       // last-layer epilogue: column blocks per target batch
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
 
 struct EvalTCParams {
@@ -80,7 +81,23 @@ struct EvalTCParams {
   int n_tasks;              // n_centre + pairs * n_signs * chunks
   int n_signs;              // 2, or 1 for the centre evaluation
   int mode;
+#ifdef ESTK_TC_PROFILE
+  unsigned long long* prof;  // [gridDim.x][warps][kPrBuckets] clock64() cycles, written at exit
+#endif
 };
+
+#ifdef ESTK_TC_PROFILE
+// Profile build only (-DESTK_TC_PROFILE): every warp sums clock64() deltas per role bucket in
+// registers and lane 0 writes them once at exit.  Producer loads are waited for before the empty
+// wait here (in the product they are still in flight during it), so kPrLoad is their full latency.
+enum { kPrFull, kPrMma, kPrDrain, kPrLayer, kPrTask, kPrLoad, kPrEmpty, kPrForm, kPrBuckets };
+unsigned long long* g_prof_buf = nullptr;
+#define ESTK_PROF_DECL long long pr_[kPrBuckets] = {}; long long pr_t_ = clock64();
+#define ESTK_PROF(b) do { const long long n_ = clock64(); pr_[b] += n_ - pr_t_; pr_t_ = n_; } while (0)
+#else
+#define ESTK_PROF_DECL
+#define ESTK_PROF(b) do {} while (0)
+#endif
 
 struct Layer { int K, N; int64_t wbase, bbase; };
 
@@ -129,6 +146,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   }
   cluster_sync();   // barriers initialised in every CTA before any remote arrive or copy
   const bool centre = (p.offsets == nullptr);
+  ESTK_PROF_DECL
 
   if (warp < 4) {
     // =================================================================== consumer warpgroup
@@ -166,6 +184,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           }
         }
       }
+      ESTK_PROF(kPrTask);
       float loss = 0.f;
       for (int l = 0; l < L; ++l) {
         const int K = lay[l].K, N = lay[l].N;
@@ -173,10 +192,24 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
         const uint32_t h_in = smem_u32(sH + (l & 1) * kHBytes);
         const uint32_t h_out = smem_u32(sH + ((l + 1) & 1) * kHBytes);
         named_bar_sync(1, 128);          // previous layer's epilogue (bias reads) done
-        for (int o = tid; o < N; o += 128)
-          sBias[o] = fmaf(ssig, ld_noise1(trow + lay[l].bbase + o), __ldg(p.theta + lay[l].bbase + o));
+        {
+          // every load first: a store between two loads would make each wait for the one before
+          float bz[kMaxW / 128], bt[kMaxW / 128];
+#pragma unroll
+          for (int i = 0; i < kMaxW / 128; ++i) {
+            const int o = tid + i * 128;
+            if (o < N) {
+              bz[i] = ld_noise1(trow + lay[l].bbase + o);
+              bt[i] = __ldg(p.theta + lay[l].bbase + o);
+            }
+          }
+#pragma unroll
+          for (int i = 0; i < kMaxW / 128; ++i)
+            if (tid + i * 128 < N) sBias[tid + i * 128] = fmaf(ssig, bz[i], bt[i]);
+        }
         fence_proxy_async();             // this layer's input (generic-proxy stores) -> wgmma
         named_bar_sync(1, 128);          // ... by every thread; bias[] published
+        ESTK_PROF(kPrLayer);
         const int lo_kb = (F16 && l == 0) ? K / kBlockK : 0;   // layer 0 in fp16: x_lo k-blocks
         for (int n0 = 0; n0 < N; n0 += kTileN) {
           const int width = min(kTileN, N - n0);
@@ -189,6 +222,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
             for (int kb = 0; kb < K / kBlockK; ++kb, ++kst) {
               const uint32_t stage = kst % kStages, phase = (kst / kStages) & 1u;
               mbar_wait(smem_u32(bar_full + stage), phase);
+              ESTK_PROF(kPrFull);
               const uint32_t a_addr = h_in + kb * kHBlockBytes, b_addr = smem_u32(sB + stage * kStageBytes);
               wgmma_fence();
 #pragma unroll
@@ -203,6 +237,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
               wgmma_wait<1>();             // the previous stage's MMAs are done: release its slot
               if (kb > 0 && lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
               prev = stage;
+              ESTK_PROF(kPrMma);
             }
           };
           if (F16 && lo_kb) k_loop(std::integral_constant<int, 2>{});
@@ -211,33 +246,57 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           fence_acc(d);
           if (lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
           // ---- epilogue of the tile
+          if (last) {
+            // the targets of kTgtBatch column blocks are loaded before any is used: the behaviour-
+            // characterisation stores would otherwise hold each load until the one before returned
 #pragma unroll
-          for (int jb = 0; jb < kTileN / 8; ++jb) {
-            if (jb * 8 < width) {
-              const int col = n0 + jb * 8 + cq;
-              const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
+            for (int jg = 0; jg < kTileN / 8; jg += kTgtBatch) {
+              float2 t[kTgtBatch][2];
 #pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int r = r0 + 8 * h;
-                const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
-                if (last) {
-                  const int b = chunk * kRows + r;
-                  const float2 t = __ldg(reinterpret_cast<const float2*>(p.target + (size_t)b * N + col));
-                  const float e0 = y0 - t.x, e1 = y1 - t.y;
-                  loss = fmaf(e0, e0, loss);
-                  loss = fmaf(e1, e1, loss);
-                  if (bc && b < p.bc_obs) {
-                    const int64_t idx = (int64_t)b * N + col;
-                    if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
-                    if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
+              for (int jb = jg; jb < jg + kTgtBatch; ++jb)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                  if (jb * 8 < width)
+                    t[jb - jg][h] = __ldg(reinterpret_cast<const float2*>(
+                        p.target + (size_t)(chunk * kRows + r0 + 8 * h) * N + n0 + jb * 8 + cq));
+#pragma unroll
+              for (int jb = jg; jb < jg + kTgtBatch; ++jb) {
+                if (jb * 8 < width) {
+                  const int col = n0 + jb * 8 + cq;
+                  const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    const int b = chunk * kRows + r0 + 8 * h;
+                    const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                    const float e0 = y0 - t[jb - jg][h].x, e1 = y1 - t[jb - jg][h].y;
+                    loss = fmaf(e0, e0, loss);
+                    loss = fmaf(e1, e1, loss);
+                    if (bc && b < p.bc_obs) {
+                      const int64_t idx = (int64_t)b * N + col;
+                      if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
+                      if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
+                    }
                   }
-                } else {
+                }
+              }
+            }
+          } else {
+#pragma unroll
+            for (int jb = 0; jb < kTileN / 8; ++jb) {
+              if (jb * 8 < width) {
+                const int col = n0 + jb * 8 + cq;
+                const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int r = r0 + 8 * h;
+                  const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
                   st_shared_u32(h_out + (col >> 6) * kHBlockBytes + sw128_offset(r, (col & 63) >> 3) + (col & 7) * 2,
                                 pack16_relu<F16>(y0, y1));
                 }
               }
             }
           }
+          ESTK_PROF(kPrDrain);
         }
       }
       // ---- squared-error partial of this CTA; the last arriver combines them in fixed order
@@ -264,6 +323,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           p.counters[cell] = 0u;
         }
       }
+      ESTK_PROF(kPrTask);
     }
   } else {
     // =================================================================== weight producers
@@ -334,8 +394,20 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
             }
           }
         }
+#ifdef ESTK_TC_PROFILE
+        uint32_t ready = 0;
+#pragma unroll
+        for (int u = 0; u < kItemsPT; ++u) {
+          if constexpr (S16) ready ^= t16[u].x ^ e16[u].x;
+          else if constexpr (F16) ready ^= __float_as_uint(th[u][1].w) ^ e16[u].x;
+          else ready ^= __float_as_uint(th[u][1].w) ^ __float_as_uint(ep[u][1].w);
+        }
+        if (ready == 0x7fc00001u) pr_[kPrForm] -= 1;   // makes the clock read below wait for the data
+        ESTK_PROF(kPrLoad);
+#endif
         // ... then wait for the ring slot, free in all four CTAs
         mbar_wait(smem_u32(bar_empty + stage), phase ^ 1);
+        ESTK_PROF(kPrEmpty);
 #pragma unroll
         for (int u = 0; u < kItemsPT; ++u) {
           const int it = u * kPT + ptid;
@@ -381,8 +453,15 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
       }
       for (int sk = 0; sk < kProdGroups && has; ++sk) has = advance();
       kst += kProdGroups;
+      ESTK_PROF(kPrForm);
     }
   }
+#ifdef ESTK_TC_PROFILE
+  if (lane == 0 && p.prof) {
+    unsigned long long* o = p.prof + ((size_t)blockIdx.x * (blockDim.x / 32) + warp) * kPrBuckets;
+    for (int b = 0; b < kPrBuckets; ++b) o[b] = (unsigned long long)pr_[b];
+  }
+#endif
   // No CTA leaves while a peer may still arrive on its barriers or copy into its ring: every copy into
   // this CTA completed on its full barriers before its consumer finished, and every peer reaches this
   // point only after its last remote arrival.
@@ -454,6 +533,9 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
   p.n_tasks = p.n_centre + p.pairs * p.n_signs * p.chunks;
   p.partial = ctx->eval_partial;
   p.counters = ctx->counters;
+#ifdef ESTK_TC_PROFILE
+  p.prof = g_prof_buf;
+#endif
   if (p.mode == kModeF16) return launch_tc<kModeF16>(p, stream);
   if (p.mode == kModeBF16S) return launch_tc<kModeBF16S>(p, stream);
   return launch_tc<kModeBF16>(p, stream);
@@ -619,6 +701,17 @@ extern "C" int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc
   p.n_signs = 1; p.mode = kModeF16;
   return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center_f16");
 }
+
+#ifdef ESTK_TC_PROFILE
+// Profile build only: the next evaluate launches write their per-warp buckets into `buf` (null: off);
+// reports the block's warp count and how many of them are consumers.
+extern "C" ESTK_API int estk_tc_profile(void* buf, int32_t* warps, int32_t* consumer_warps) {
+  g_prof_buf = static_cast<unsigned long long*>(buf);
+  *warps = kThreadsTC / 32;
+  *consumer_warps = 4;
+  return kPrBuckets;
+}
+#endif
 
 extern "C" int estk_eval_mlp_f16_supported(const estk_mlp_desc* desc, int32_t B) {
   const char* why = "";
