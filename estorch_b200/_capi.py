@@ -65,6 +65,9 @@ SIGNATURES = {
     "estk_eval_mlp_f16_supported": [C.POINTER(EstkMlpDesc), _I32],
     "estk_eval_conv_vbn_scratch_bytes": [_P, _I32, _I32],
     "estk_eval_conv_vbn": [_P, _I32, _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _I32, _P, _P, _P, _I64, _P],
+    "estk_eval_conv_vbn_f16_scratch_bytes": [_P, _I32, _I32],
+    "estk_eval_conv_vbn_f16": [_P, _I32, _P, _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _I32, _P, _P, _P, _I64,
+                               _P],
     "estk_track_best": [_P, _P, _P, _P, _P, _I64, _P],
     "estk_rank_grad_adam": [_P, _P, _P, _F32, _F32, _I32, _P, _P, _P, _I64, _P, _P, _P, _P,
                             C.POINTER(EstkAdamDesc), _P, _P, _P, _P],
@@ -101,7 +104,8 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = (C.c_char_p if name == "estk_last_error" else
-                      C.c_int64 if name in ("estk_eval_conv_vbn_scratch_bytes", "estk_xr_workspace_bytes") else C.c_int)
+                      C.c_int64 if name in ("estk_eval_conv_vbn_scratch_bytes", "estk_eval_conv_vbn_f16_scratch_bytes",
+                                           "estk_xr_workspace_bytes") else C.c_int)
     _lib = lib
     return lib
 

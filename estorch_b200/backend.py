@@ -227,20 +227,35 @@ class CudaBackend:
         _capi.check(rc, "estk_eval_mlp_center[" + precision + "]")
         self.launches += 2 if precision == "f16" else 1
 
-    def conv_scratch_bytes(self, ref_batch, B) -> int:
+    def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
+        if precision == "f16":
+            return int(self.lib.estk_eval_conv_vbn_f16_scratch_bytes(self._ctx, int(ref_batch), int(B)))
+        if precision != "fp32":
+            raise ValueError(f"the conv + VirtualBatchNorm evaluate has no {precision!r} mode")
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, int(ref_batch), int(B)))
 
     def eval_conv_vbn(self, n_actions, theta, table, offsets, order, pairs, sigma, xref, obs, target,
-                      ret_plus, ret_minus, scratch):
-        """Conv + VirtualBatchNorm policy (examples/atari.py:14-37); offsets None = centre."""
-        _capi.check(self.lib.estk_eval_conv_vbn(
-            self._ctx, int(n_actions), self._ptr(theta, torch.float32, "theta"),
-            self._ptr(table, torch.float32, "table"), self._ptr(offsets, torch.int64, "offsets"),
-            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma),
-            self._ptr(xref, torch.float32, "xref"), int(xref.shape[0]), self._ptr(obs, torch.float32, "obs"),
-            self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
-            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
-            self._ptr(scratch, torch.uint8, "scratch"), scratch.numel(), self._stream()), "estk_eval_conv_vbn")
+                      ret_plus, ret_minus, scratch, precision="fp32", table16=None):
+        """Conv + VirtualBatchNorm policy (examples/atari.py:14-37); offsets None = centre.
+        precision "f16": the tensor-core kernel (needs table16 with offsets, and a scratch of
+        conv_scratch_bytes(R, B, "f16") bytes)."""
+        head = (self._ctx, int(n_actions), self._ptr(theta, torch.float32, "theta"),
+                self._ptr(table, torch.float32, "table"))
+        tail = (self._ptr(offsets, torch.int64, "offsets"),
+                self._ptr(order, torch.int32, "order"), int(pairs), float(sigma),
+                self._ptr(xref, torch.float32, "xref"), int(xref.shape[0]), self._ptr(obs, torch.float32, "obs"),
+                self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
+                self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+                self._ptr(scratch, torch.uint8, "scratch"), scratch.numel(), self._stream())
+        if precision == "f16":
+            if offsets is not None and table16 is None:
+                raise ValueError("precision='f16' needs table16, the exact fp16 copy of the table (see shadow_f16)")
+            rc = self.lib.estk_eval_conv_vbn_f16(*head, self._ptr(table16, torch.float16, "table16"), *tail)
+        elif precision == "fp32":
+            rc = self.lib.estk_eval_conv_vbn(*head, *tail)
+        else:
+            raise ValueError(f"the conv + VirtualBatchNorm evaluate has no {precision!r} mode")
+        _capi.check(rc, "estk_eval_conv_vbn[" + precision + "]")
         self.launches += 1
 
     def track_best(self, state, reward, theta, best_theta):

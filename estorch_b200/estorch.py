@@ -223,9 +223,14 @@ class ES:
                         TF32 class) and fp32 accumulation; every weight is formed in fp32
                         from the fp32 theta and the (exactly 16-bit representable) noise
                         value and rounded once; observations enter as hi + lo halves;
-            ``"auto"``  (default) ``"f16"`` when the policy shape supports it, else ``"fp32"``;
+                        For the conv + VirtualBatchNorm policy (examples/atari.py) ``"f16"``
+                        is an opt-in mma.sync kernel whose weights, inputs and normalised
+                        activations all enter as hi + lo fp16 pairs (22-bit operands);
+            ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
+                        (always ``"fp32"`` for the conv policy);
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
-                        ``bf16s`` additionally reads bf16 shadows of theta and the table).
+                        ``bf16s`` additionally reads bf16 shadows of theta and the table);
+                        MLP policies only.
     Attributes as documented at estorch.py:108-117.
     """
 
@@ -269,8 +274,10 @@ class ES:
         if eval_precision not in ("auto", "fp32", "f16", "bf16", "bf16s"):
             raise ValueError("eval_precision must be 'auto', 'fp32', 'f16', 'bf16' or 'bf16s'")
         self._precision = "fp32"
-        if self._fused and self._is_conv and eval_precision not in ("auto", "fp32"):
-            raise ValueError("the conv + VirtualBatchNorm evaluate kernel is fp32 only")
+        if self._fused and self._is_conv and eval_precision in ("bf16", "bf16s"):
+            raise ValueError("the conv + VirtualBatchNorm evaluate kernel has 'fp32' and 'f16' modes only")
+        if self._fused and self._is_conv and eval_precision == "f16":
+            self._precision = "f16"
         if self._fused and not self._is_conv and eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
             supported = getattr(self._be, probe, lambda d, b: False)(self._spec.dims, self.agent.obs.shape[0])
@@ -315,7 +322,7 @@ class ES:
         self._xref = self._conv_scratch = None
         if self._fused and self._is_conv:
             self._xref = self.target.xref.detach().to(self._dev, torch.float32).contiguous()
-            nbytes = be.conv_scratch_bytes(self._xref.shape[0], self._obs.shape[0])
+            nbytes = be.conv_scratch_bytes(self._xref.shape[0], self._obs.shape[0], self._precision)
             self._conv_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self._dev)
 
         self._slots = []
@@ -828,7 +835,8 @@ class ES:
         _nvtx_push("estk:evaluate")
         if self._is_conv:
             be.eval_conv_vbn(self._spec.n_actions, slot.theta, self._table, self._offsets, self._order, pl,
-                             self.sigma, self._xref, self._obs, self._tgt, ret_p, ret_m, self._conv_scratch)
+                             self.sigma, self._xref, self._obs, self._tgt, ret_p, ret_m, self._conv_scratch,
+                             **self._eval_kw(slot))
         else:
             kw = self._eval_kw(slot)
             if folded:        # the previous generation's post-update rollout rides in this launch
@@ -874,7 +882,7 @@ class ES:
             return
         if self._is_conv:
             be.eval_conv_vbn(self._spec.n_actions, slot.theta, None, None, None, 1, 0.0, self._xref, self._obs,
-                             self._tgt, self._episode, None, self._conv_scratch)
+                             self._tgt, self._episode, None, self._conv_scratch, **self._eval_kw(slot, True))
         else:
             be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, **self._eval_kw(slot, True))
         be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)

@@ -223,6 +223,24 @@ ESTK_API int estk_eval_conv_vbn(estk_ctx* ctx, int32_t n_actions, const float* t
                        int32_t B, float* returns_plus, float* returns_minus, void* scratch,
                        int64_t scratch_bytes, void* stream);
 
+/* Opt-in tensor-core variant of estk_eval_conv_vbn ("f16"): same policy, arguments, return
+ * placement (returns_plus[j] / returns_minus[j], j = order[slot] when order is given) and
+ * offsets == NULL centre evaluation.  conv1, conv2 and fc1 run on mma.sync with fp16 operands
+ * and fp32 accumulation; every operand -- the weights theta + s*sigma*T[off+i] (formed in fp32
+ * from the fp32 theta and table16, the EXACT fp16 copy of `table` made by estk_shadow_f16),
+ * the input frames and the normalised activations -- enters as hi + lo, two fp16 values
+ * (22 significant bits), so the returns stay within 1e-5 (max-norm relative) of the fp32
+ * forward.  VBN statistics, normalisation, biases, fc2 and the loss are fp32; no atomics, so
+ * the returns are the same bits run to run.  table and table16 are required with offsets.
+ * scratch: at least estk_eval_conv_vbn_f16_scratch_bytes(ctx, ref_batch, B) bytes, 16-byte
+ * aligned.  Shapes: everything estk_eval_conv_vbn accepts. */
+ESTK_API int64_t estk_eval_conv_vbn_f16_scratch_bytes(estk_ctx* ctx, int32_t ref_batch, int32_t B);
+ESTK_API int estk_eval_conv_vbn_f16(estk_ctx* ctx, int32_t n_actions, const float* theta, const float* table,
+                           const uint16_t* table16, const int64_t* offsets, const int32_t* order,
+                           int32_t pairs, float sigma, const float* xref, int32_t ref_batch,
+                           const float* obs, const float* target, int32_t B, float* returns_plus,
+                           float* returns_minus, void* scratch, int64_t scratch_bytes, void* stream);
+
 /* Unperturbed policy (estorch.py:181-182 `_after_optimize` rollout):
  * return_out[0] = return of theta; bc_out (nullable) [bc_dim]. */
 ESTK_API int estk_eval_mlp_center(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
