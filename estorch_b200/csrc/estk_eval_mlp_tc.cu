@@ -16,7 +16,8 @@
 //      the cluster forms tile rows [q*w/4, (q+1)*w/4) of each stage and copies them into the same
 //      slot of the other three CTAs (cp.async.bulk over distributed shared memory), so every weight
 //      is read from L2 and formed once per 256 observations;
-//   D  64 x 128 fp32 in the registers of the consumer warpgroup; the epilogue adds the bias,
+//   D  64 x 128 fp32 in the registers of the consumer warpgroup that owns the tile (the two
+//      consumer warpgroups take alternate N tiles); the epilogue adds the bias,
 //      applies ReLU and rounds to 16 bits straight into the other activation buffer.  The last
 //      layer is fused with the squared-error reduction (and the behaviour characterisation).
 // Operand modes (template MODE):
@@ -25,11 +26,12 @@
 //   kModeF16    fp16 operands (11-bit significand, the TF32 class) from fp32 theta and the EXACT
 //               16-bit copy of the noise table: W16 = rn_f16(theta + s*sigma*eps), sum in fp32; the
 //               observations enter layer 0 as x_hi + x_lo (two fp16 k-block sets, same B tile)
-// Warp roles: warpgroup 0 = consumer (MMA issue + epilogue), warps 4..11 = weight producers in
+// Warp roles: warpgroups 0 and 1 = consumers (MMA issue + epilogue) of alternate N tiles, so one
+// warpgroup's epilogue runs under the other's MMAs; warps 8..15 = weight producers in
 // four groups of two, each group forming every fourth stage of the flattened
 // (task, layer, N tile, k-block) sequence.  full / empty mbarriers per ring stage: full[s] completes
-// on the local group's arrival plus the bytes the three peers copy in; empty[s] counts the consumer
-// warps of all four CTAs, because a producer writes slot s of every CTA.  Persistent: clusters loop
+// on the local group's arrival plus the bytes the three peers copy in; empty[s] counts the warps of
+// the consuming warpgroup in all four CTAs, because a producer writes slot s of every CTA.  Persistent: clusters loop
 // over groups of four tasks; the two signs of a pair run on neighbouring clusters at the same time,
 // so the second read of the noise row is an L2 hit.
 #include "estk_tc.cuh"
@@ -46,14 +48,31 @@ constexpr int kStages = 5;
 constexpr int kCluster = 4;                        // CTAs (observation chunks) sharing every B stage
 constexpr int kProdWarps = 8, kProdGroups = 4, kProdGroupWarps = kProdWarps / kProdGroups;
 constexpr int kPT = 32 * kProdGroupWarps;          // threads per producer group
-constexpr int kThreadsTC = 128 + 32 * kProdWarps;  // 384
-// A group waits for the release of the slot it is about to fill, kStages stages back; its previous
-// stage, kProdGroups back, already saw the release before that.  So no group runs a full phase ahead of
-// an empty barrier, which a parity wait could not tell apart.
+constexpr int kConsWG = 2, kConsThreads = 128 * kConsWG;   // consumer warpgroups 0 and 1
+constexpr int kThreadsTC = kConsThreads + 32 * kProdWarps; // 512
+// Registers per thread after the role split (setmaxnreg).  At 512 threads the launch allows 128; a
+// consumer holds a 64-float accumulator tile plus the task state and the last layer's target batch,
+// a bf16-mode producer thread four items of 2 x 8 fp32 loads in flight plus their addresses.  The two
+// warpgroups of each role must fit the 64K-register file: 2*128*kConsRegs + 2*128*kProdRegs <= 65536.
+// The consumer spills below 152 and the bf16 producer below 104, so 152/104 is the one split with no
+// local memory in either role for all three modes; it holds with target batches of two column blocks
+// (four spill at 152) and with the producer's barrier id and CTA rank re-read instead of kept live.
+constexpr int kConsRegs = 152, kProdRegs = 104;
+static_assert(kConsRegs + kProdRegs <= 256, "setmaxnreg split exceeds the register file");
+// Named barriers: 0 unused, 1 all consumers, 2..5 the producer groups, kBarOrder + w / kBarLoss + w
+// hand tile ordering / the loss chain to consumer warpgroup w, kBarWG + w warpgroup w alone.
+constexpr int kBarCons = 1, kBarOrder = 6, kBarLoss = 8, kBarWG = 10;
+// Producers: a group waits for the release of the slot it is about to fill, kStages stages back; its
+// previous stage, kProdGroups back, already saw the release before that.  So no group runs a full phase
+// ahead of an empty barrier, which a parity wait could not tell apart.
+// Consumers: the warpgroup that owns tile t waits on full for t's first stage only after the other
+// warpgroup has issued every MMA of tile t-1, so every stage before it has been seen formed and the
+// wait is within one lap of the barrier.  Without that order a warpgroup skipping the other's tile
+// (up to 8 stages) would wait two phases ahead, and the parity wait would return on an unformed stage.
 static_assert(kProdGroups <= kStages, "parity waits need kProdGroups <= kStages");
 // 16-byte items per producer thread per stage: the CTA's quarter of the widest tile, in one batch
 constexpr int kItemsPT = kTileN / kCluster * (kBlockK / 8) / kPT;
-constexpr int kTgtBatch = 4;                       // last-layer epilogue: column blocks per target batch
+constexpr int kTgtBatch = 2;                       // last-layer epilogue: column blocks per target batch
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
 
 struct EvalTCParams {
@@ -90,7 +109,7 @@ struct EvalTCParams {
 // Profile build only (-DESTK_TC_PROFILE): every warp sums clock64() deltas per role bucket in
 // registers and lane 0 writes them once at exit.  Producer loads are waited for before the empty
 // wait here (in the product they are still in flight during it), so kPrLoad is their full latency.
-enum { kPrFull, kPrMma, kPrDrain, kPrLayer, kPrTask, kPrLoad, kPrEmpty, kPrForm, kPrBuckets };
+enum { kPrFull, kPrMma, kPrDrain, kPrLayer, kPrTask, kPrOther, kPrLoad, kPrEmpty, kPrForm, kPrBuckets };
 unsigned long long* g_prof_buf = nullptr;
 #define ESTK_PROF_DECL long long pr_[kPrBuckets] = {}; long long pr_t_ = clock64();
 #define ESTK_PROF(b) do { const long long n_ = clock64(); pr_[b] += n_ - pr_t_; pr_t_ = n_; } while (0)
@@ -121,10 +140,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sH = smem;                                  // 2 activation buffers x 8 k-blocks x 8 KB
   uint8_t* sB = sH + 2 * kHBytes;                      // ring
-  float* sBias = reinterpret_cast<float*>(sB + kStages * kStageBytes);   // [512], one layer at a time
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(sBias + kMaxW);      // [kStages] stage formed
+  float* sBias = reinterpret_cast<float*>(sB + kStages * kStageBytes);   // [2][512], by layer parity
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(sBias + 2 * kMaxW);  // [kStages] stage formed
   uint64_t* bar_empty = bar_full + kStages;                             // [kStages] stage consumed
   float* s_loss = reinterpret_cast<float*>(bar_empty + kStages);        // [4]
+  float* s_chain = s_loss + 4;                                          // [128] loss chain handoff
   __shared__ Layer lay[ESTK_MAX_LAYERS];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -132,7 +152,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(smem_u32(bar_full + s), 1);                // the forming group's elected thread (+ peer bytes)
-      mbar_init(smem_u32(bar_empty + s), 4 * kCluster);    // every consumer warp of the cluster
+      mbar_init(smem_u32(bar_empty + s), 4 * kCluster);    // the consuming warpgroup's warps, every CTA
     }
     fence_barrier_init();
     int64_t pb = 0;
@@ -148,12 +168,19 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   const bool centre = (p.offsets == nullptr);
   ESTK_PROF_DECL
 
-  if (warp < 4) {
-    // =================================================================== consumer warpgroup
-    const int tid = threadIdx.x;                     // 0..127
-    const int r0 = warp * 16 + (lane >> 2);          // accumulator rows r0 and r0 + 8
+  if (warp < 4 * kConsWG) {
+    // =================================================================== consumer warpgroups
+    // Tile t of the CTA's running (task, layer, N tile) sequence belongs to warpgroup t % 2.  The
+    // alternation does not restart per task: a task has an odd number of tiles at the north star (19).
+    setmaxnreg_inc<kConsRegs>();
+    const int cw = warp >> 2;                        // consumer warpgroup
+    const int ctid = threadIdx.x;                    // 0..255
+    const int tid = ctid & 127;                      // thread of the warpgroup
+    const int r0 = (warp & 3) * 16 + (lane >> 2);    // accumulator rows r0 and r0 + 8
     const int cq = (lane & 3) * 2;                   // accumulator columns 8j + cq, +1
     uint32_t kst = 0;                                // global stage index
+    bool mine = (cw == 0);                           // the next tile is this warpgroup's
+    bool after = (cw != 0);                          // a tile precedes this warpgroup's next one
     // gridDim.x and chunks (B % 256 == 0) are multiples of kCluster: the CTAs of a cluster always hold
     // the kCluster consecutive chunks of one (pair, sign), CTA rank = chunk % kCluster
     for (int task = blockIdx.x; task < p.n_tasks; task += gridDim.x) {
@@ -162,11 +189,15 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
       const int j = (!tk.centre && p.order) ? p.order[slot] : slot;
       const float* trow = tk.centre ? p.theta : p.table + p.offsets[j];
       const float ssig = tk.centre ? 0.f : (sgn ? -p.sigma : p.sigma);
-      float* bc = (tk.centre && !centre) ? nullptr : (sgn ? p.bc_minus : p.bc_plus);
+      const bool with_bc = !(tk.centre && !centre) && p.bc_plus;   // the row pointer is formed at use
+      const bool final_task = task + (int)gridDim.x >= p.n_tasks;
+      // every MMA of the previous task has completed (buffer 0 and sBias[0] are free) and its loss
+      // has been combined
+      named_bar_sync(kBarCons, kConsThreads);
       // ---- this CTA's observations as the layer-0 A operand (buffer 0)
       {
         const int K0 = lay[0].K, per_row = K0 / 8;
-        for (int it = tid; it < kRows * per_row; it += 128) {
+        for (int it = ctid; it < kRows * per_row; it += kConsThreads) {
           const int r = it / per_row, c = it % per_row;
           const float* src = p.obs + (size_t)(chunk * kRows + r) * K0 + c * 8;
           const float4 x0 = __ldg(reinterpret_cast<const float4*>(src));
@@ -191,28 +222,40 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
         const bool last = (l == L - 1);
         const uint32_t h_in = smem_u32(sH + (l & 1) * kHBytes);
         const uint32_t h_out = smem_u32(sH + ((l + 1) & 1) * kHBytes);
-        named_bar_sync(1, 128);          // previous layer's epilogue (bias reads) done
+        // Layer l's bias goes to sBias[l & 1].  Its last readers, layer l-2's epilogues, finished
+        // before the barrier that opened layer l-1, which this thread has passed.
+        float* bias = sBias + (l & 1) * kMaxW;
         {
           // every load first: a store between two loads would make each wait for the one before
-          float bz[kMaxW / 128], bt[kMaxW / 128];
+          float bz[kMaxW / kConsThreads], bt[kMaxW / kConsThreads];
 #pragma unroll
-          for (int i = 0; i < kMaxW / 128; ++i) {
-            const int o = tid + i * 128;
+          for (int i = 0; i < kMaxW / kConsThreads; ++i) {
+            const int o = ctid + i * kConsThreads;
             if (o < N) {
               bz[i] = ld_noise1(trow + lay[l].bbase + o);
               bt[i] = __ldg(p.theta + lay[l].bbase + o);
             }
           }
 #pragma unroll
-          for (int i = 0; i < kMaxW / 128; ++i)
-            if (tid + i * 128 < N) sBias[tid + i * 128] = fmaf(ssig, bz[i], bt[i]);
+          for (int i = 0; i < kMaxW / kConsThreads; ++i)
+            if (ctid + i * kConsThreads < N) bias[ctid + i * kConsThreads] = fmaf(ssig, bz[i], bt[i]);
         }
-        fence_proxy_async();             // this layer's input (generic-proxy stores) -> wgmma
-        named_bar_sync(1, 128);          // ... by every thread; bias[] published
+        // This layer's input, written by both warpgroups (generic-proxy stores) -> wgmma.  Past this
+        // barrier every MMA of layer l-1 has completed too, so its input buffer may be overwritten.
+        fence_proxy_async();
+        named_bar_sync(kBarCons, kConsThreads);
         ESTK_PROF(kPrLayer);
         const int lo_kb = (F16 && l == 0) ? K / kBlockK : 0;   // layer 0 in fp16: x_lo k-blocks
-        for (int n0 = 0; n0 < N; n0 += kTileN) {
+        for (int n0 = 0; n0 < N; n0 += kTileN, mine = !mine) {
+          if (!mine) {                       // the other warpgroup's tile
+            kst += K / kBlockK;
+            continue;
+          }
           const int width = min(kTileN, N - n0);
+          const bool last_tile = n0 + kTileN >= N;
+          if (after) named_bar_sync(kBarOrder + cw, kConsThreads);    // the previous tile's MMAs issued
+          after = true;
+          ESTK_PROF(kPrOther);
           float d[64];                     // the first MMA of the tile overwrites (scale-d = 0)
           uint32_t prev = 0;
           // NP = 2: layer 0 in fp16, x_lo on the same B tile (a separate instantiation, so that no
@@ -242,6 +285,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           };
           if (F16 && lo_kb) k_loop(std::integral_constant<int, 2>{});
           else k_loop(std::integral_constant<int, 1>{});
+          if (!(last && last_tile && final_task)) named_bar_arrive(kBarOrder + (cw ^ 1), kConsThreads);
           wgmma_wait<0>();
           fence_acc(d);
           if (lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
@@ -259,11 +303,19 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
                   if (jb * 8 < width)
                     t[jb - jg][h] = __ldg(reinterpret_cast<const float2*>(
                         p.target + (size_t)(chunk * kRows + r0 + 8 * h) * N + n0 + jb * 8 + cq));
+              if (jg == 0 && n0 > 0) {
+                // the squared-error chain continues from the previous tile, which the other
+                // warpgroup drained; thread tid of both warpgroups holds the same rows and columns
+                ESTK_PROF(kPrDrain);
+                named_bar_sync(kBarLoss + cw, kConsThreads);
+                loss = s_chain[tid];
+                ESTK_PROF(kPrOther);
+              }
 #pragma unroll
               for (int jb = jg; jb < jg + kTgtBatch; ++jb) {
                 if (jb * 8 < width) {
                   const int col = n0 + jb * 8 + cq;
-                  const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
+                  const float2 bv = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
                   for (int h = 0; h < 2; ++h) {
                     const int b = chunk * kRows + r0 + 8 * h;
@@ -271,7 +323,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
                     const float e0 = y0 - t[jb - jg][h].x, e1 = y1 - t[jb - jg][h].y;
                     loss = fmaf(e0, e0, loss);
                     loss = fmaf(e1, e1, loss);
-                    if (bc && b < p.bc_obs) {
+                    if (with_bc && b < p.bc_obs) {
+                      float* bc = sgn ? p.bc_minus : p.bc_plus;
                       const int64_t idx = (int64_t)b * N + col;
                       if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
                       if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
@@ -280,12 +333,16 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
                 }
               }
             }
+            if (!last_tile) {                // hand the chain to the warpgroup of the next tile
+              s_chain[tid] = loss;
+              named_bar_arrive(kBarLoss + (cw ^ 1), kConsThreads);
+            }
           } else {
 #pragma unroll
             for (int jb = 0; jb < kTileN / 8; ++jb) {
               if (jb * 8 < width) {
                 const int col = n0 + jb * 8 + cq;
-                const float2 bv = *reinterpret_cast<const float2*>(sBias + col);
+                const float2 bv = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int r = r0 + 8 * h;
@@ -299,10 +356,12 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           ESTK_PROF(kPrDrain);
         }
       }
-      // ---- squared-error partial of this CTA; the last arriver combines them in fixed order
+      // ---- squared-error partial of this CTA, from the warpgroup that drained the task's last tile;
+      // the last arriver combines them in fixed order
+      if (mine) continue;
       loss = warp_sum_f(loss);
-      if (lane == 0) s_loss[warp] = loss;
-      named_bar_sync(1, 128);
+      if (lane == 0) s_loss[warp & 3] = loss;
+      named_bar_sync(kBarWG + cw, 128);
       if (tid == 0) {
         const float tot = (s_loss[0] + s_loss[1]) + (s_loss[2] + s_loss[3]);
         const int parts = p.chunks;
@@ -331,11 +390,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
     // sequence, this CTA's quarter of each: tile rows [rank*w/4, (rank+1)*w/4).  w % 32 == 0, so a
     // quarter is whole 8-row swizzle atoms, one contiguous 1024-B-aligned byte range of the stage.
     // Item `it` of the quarter = its row it/8, 16-byte output chunk it%8 (8 weights).
-    const int pwarp = warp - 4;
+    setmaxnreg_dec<kProdRegs>();
+    const int pwarp = warp - 4 * kConsWG;
     const int pgroup = pwarp / kProdGroupWarps;
     const int ptid = (pwarp % kProdGroupWarps) * 32 + lane;
-    const uint32_t rank = cluster_ctarank();
-    int cached_task = -1;
+    bool new_task = true;                 // the per-task row pointers are stale
     const float* trow = p.theta;
     const uint16_t* trow16 = nullptr;
     float ssig = 0.f;
@@ -346,7 +405,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
         n0 += kTileN;
         if (n0 >= lay[l].N) {
           n0 = 0;
-          if (++l == L) { l = 0; task += gridDim.x; }
+          if (++l == L) { l = 0; task += gridDim.x; new_task = true; }
         }
       }
       return task < p.n_tasks;
@@ -355,8 +414,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
     for (int sk = 0; sk < pgroup && has; ++sk) has = advance();
     uint32_t kst = pgroup;
     while (has) {
-      if (task != cached_task) {            // two dependent global loads: once per task, not per stage
-        cached_task = task;
+      if (new_task) {                       // two dependent global loads: once per task, not per stage
+        new_task = false;
         const TaskId tk = decode_task(p, task, centre);
         const int jj = (!tk.centre && p.order) ? p.order[tk.slot] : tk.slot;
         trow = tk.centre ? p.theta : p.table + p.offsets[jj];
@@ -368,6 +427,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
       const int K = lay[l].K;
       const int qrows = min(kTileN, lay[l].N - n0) / kCluster;
       const int n_items = qrows * 8;
+      const uint32_t rank = cluster_ctarank();
       const uint32_t qbase = sbase + rank * qrows * 128, qbytes = qrows * 128;
       const int64_t rbase = lay[l].wbase + (int64_t)(n0 + rank * qrows) * K + kb * kBlockK;
       {
@@ -439,7 +499,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
         }
       }
       fence_proxy_async();                  // the quarter -> async proxy (local wgmma, bulk copies)
-      named_bar_sync(2 + pgroup, kPT);
+      named_bar_sync(2 + (int)(threadIdx.x / kPT) - kConsThreads / kPT, kPT);   // 2 + pgroup
       if (ptid == 0) {
         // full[stage] of this CTA: this arrival + the three quarters the peers copy in.  A peer's
         // bytes may land before the expect_tx (the transaction count goes negative meanwhile); the
@@ -469,8 +529,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
 }
 
 size_t tc_smem_bytes() {
-  return 1024 + 2 * (size_t)kHBytes + (size_t)kStages * kStageBytes + kMaxW * sizeof(float) +
-         2 * kStages * sizeof(uint64_t) + 4 * sizeof(float);
+  return 1024 + 2 * (size_t)kHBytes + (size_t)kStages * kStageBytes + 2 * kMaxW * sizeof(float) +
+         2 * kStages * sizeof(uint64_t) + (4 + 128) * sizeof(float);
 }
 
 // Clusters of kCluster CTAs, one per SM, persistent over groups of kCluster tasks.  The number of
@@ -708,7 +768,7 @@ extern "C" int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc
 extern "C" ESTK_API int estk_tc_profile(void* buf, int32_t* warps, int32_t* consumer_warps) {
   g_prof_buf = static_cast<unsigned long long*>(buf);
   *warps = kThreadsTC / 32;
-  *consumer_warps = 4;
+  *consumer_warps = 4 * kConsWG;
   return kPrBuckets;
 }
 #endif

@@ -4,7 +4,9 @@ Needs the profile build of the library:
     ESTK_VARIANT=prof ESTK_EXTRA_FLAGS=-DESTK_TC_PROFILE bash estorch_b200/csrc/build.sh
     ESTK_LIBRARY=estorch_b200/lib/libestk_prof.so python tools/eval_profile.py [pairs] [f16|bf16|bf16s]
 Every warp sums clock64() deltas per bucket; the table gives, per role, the mean share of a warp's
-cycles and the mean cycles per ring stage the warp handled (a producer group forms every fourth stage).
+cycles and the mean cycles per ring stage the warp handled (a producer group forms every fourth stage, a
+consumer warpgroup drains every second tile).  "wait other warpgroup" is the tile-order handoff and the
+last layer's loss-chain handoff between the two consumer warpgroups.
 """
 import ctypes as C
 import os
@@ -17,7 +19,7 @@ from estorch_b200 import _capi  # noqa: E402
 from estorch_b200.backend import CudaBackend  # noqa: E402
 
 CONSUMER = ["wait full", "MMA issue .. wait_group", "tile drain + epilogue", "layer: bias + barriers",
-            "task: obs load + loss"]
+            "task: obs load + loss", "wait other warpgroup"]
 PRODUCER = ["load issue .. data in registers", "wait empty", "form + store + publish"]
 
 
@@ -66,7 +68,7 @@ def main():
     cons, prod = t[:, :cwarps.value].reshape(-1, nb), t[:, cwarps.value:].reshape(-1, nb)
     print(f"eval {mode} pairs={pairs}: {ms:.3f} ms (profiled launch), {t.shape[0]} CTAs, "
           f"{warps.value} warps/CTA ({cwarps.value} consumer), {stages} stages per CTA")
-    for role, rows, names, first, per in (("consumer", cons, CONSUMER, 0, cwarps.value // 4), ("producer", prod, PRODUCER, 5, 4)):
+    for role, rows, names, first, per in (("consumer", cons, CONSUMER, 0, cwarps.value // 4), ("producer", prod, PRODUCER, len(CONSUMER), 4)):
         tot = rows[:, first:first + len(names)].sum(dim=1).mean().item()
         print(f"  {role} warp: {tot / 1e6:.2f} Mcycles")
         for i, name in enumerate(names):
