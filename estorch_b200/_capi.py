@@ -15,6 +15,10 @@ LIB_PATH = os.environ.get("ESTK_LIBRARY") or os.path.join(_HERE, "lib", "libestk
 
 ESTK_MAX_LAYERS = 8
 ESTK_MAX_POPULATION = 32768
+# estk_mlp_desc.activation bit fields: hidden activation in bits 0-7, output activation in bits 8-15
+ESTK_ACT_RELU = 0
+ESTK_ACT_TANH = 1
+ESTK_ACT_OUT_TANH = 1 << 8
 
 
 class EstkState(C.Structure):

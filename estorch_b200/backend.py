@@ -41,14 +41,15 @@ def write_state(state: torch.Tensor, **fields):
     state.copy_(torch.from_numpy(rec.view(np.uint8).copy()))
 
 
-def mlp_desc(dims: Sequence[int]) -> _capi.EstkMlpDesc:
+def mlp_desc(dims: Sequence[int], act: int = 0) -> _capi.EstkMlpDesc:
+    """``act``: the ``estk_mlp_desc.activation`` code (``MLPSpec.act``; 0 = ReLU hidden, identity output)."""
     if not (2 <= len(dims) <= _capi.ESTK_MAX_LAYERS + 1):
         raise ValueError(f"MLP with {len(dims) - 1} Linear layers is outside 1..{_capi.ESTK_MAX_LAYERS}")
     d = _capi.EstkMlpDesc()
     d.n_layers = len(dims) - 1
     for i, w in enumerate(dims):
         d.dims[i] = int(w)
-    d.activation = 0
+    d.activation = int(act)
     return d
 
 
@@ -144,12 +145,12 @@ class CudaBackend:
         self.launches += 1
 
     # ---------------------------------------------------------------- evaluate
-    def eval_supports_bf16(self, dims, B) -> bool:
-        d = mlp_desc(dims)
+    def eval_supports_bf16(self, dims, B, act=0) -> bool:
+        d = mlp_desc(dims, act)
         return bool(self.lib.estk_eval_mlp_bf16_supported(C.byref(d), int(B)))
 
-    def eval_supports_f16(self, dims, B) -> bool:
-        d = mlp_desc(dims)
+    def eval_supports_f16(self, dims, B, act=0) -> bool:
+        d = mlp_desc(dims, act)
         return bool(self.lib.estk_eval_mlp_f16_supported(C.byref(d), int(B)))
 
     def shadow_f16(self, src, dst, check=True) -> int:
@@ -173,8 +174,8 @@ class CudaBackend:
 
     def eval_mlp(self, dims, theta, table, offsets, order, pairs, sigma, obs, target,
                  ret_plus, ret_minus, bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32",
-                 theta16=None, table16=None, centre_out=None):
-        d = mlp_desc(dims)
+                 theta16=None, table16=None, centre_out=None, act=0):
+        d = mlp_desc(dims, act)
         if obs.shape != (obs.shape[0], dims[0]) or target.shape != (obs.shape[0], dims[-1]):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match dims {list(dims)}")
         common = (self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
@@ -209,8 +210,8 @@ class CudaBackend:
         self.launches += 2 if precision == "f16" else 1      # f16: observation image + evaluate
 
     def eval_mlp_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
-                        precision="fp32", theta16=None):
-        d = mlp_desc(dims)
+                        precision="fp32", theta16=None, act=0):
+        d = mlp_desc(dims, act)
         tail = (self._ptr(obs, torch.float32, "obs"), self._ptr(target, torch.float32, "target"),
                 int(obs.shape[0]), self._ptr(ret_out, torch.float32, "ret_out"),
                 self._ptr(bc_out, torch.float32, "bc_out"), int(bc_obs), int(bc_dim), self._stream())

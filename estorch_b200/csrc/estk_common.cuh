@@ -33,6 +33,11 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
+// estk_mlp_desc.activation: the four defined codes (hidden ReLU / Tanh x output identity / Tanh)
+static inline bool estk_act_valid(int a) {
+  return a == ESTK_ACT_RELU || a == ESTK_ACT_TANH || a == ESTK_ACT_OUT_TANH || a == (ESTK_ACT_TANH | ESTK_ACT_OUT_TANH);
+}
+
 // ---------------------------------------------------------------- context
 struct estk_ctx {
   int device;

@@ -4,7 +4,8 @@
 // Replaces (reference file:line, /root/reference):
 //   ES._sample_policy        estorch/estorch.py:187-193   theta +- sigma*eps, never materialised
 //   ES._calculate_returns    estorch/estorch.py:195-202   vector_to_parameters + rollout per row
-//   Policy.forward           examples/cartpole_es.py:14-20 (Linear-ReLU-Linear-ReLU-Linear)
+//   Policy.forward           examples/cartpole_es.py:14-20 (Linear-ReLU-Linear-ReLU-Linear; or Tanh
+//                            hidden and / or output activations, estk.h ESTK_ACT_*)
 //   Agent.rollout            synthetic agent of SURVEY 8d: -mean((policy(obs)-y)^2)
 //                            (+ behaviour characteristic, examples/nsra_es.py:45-49)
 //
@@ -47,8 +48,11 @@ struct EvalParams {
   unsigned int* counters;  // [pairs], zero on entry, zero on exit
 };
 
-template <int ROWS>
+// ACT = estk_mlp_desc.activation (a compile-time constant, so the ReLU instantiations are
+// the code they were before Tanh existed)
+template <int ROWS, int ACT>
 __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) {
+  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr int OT = 4096 / ROWS;  // output features per tile
   constexpr int OTP = OT + 4;      // padded row of the weight tile (keeps float4 alignment)
   constexpr int TC = OT / 4;       // thread columns
@@ -132,7 +136,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
           acc[3][2] = fmaf(x.w, w.z, acc[3][2]); acc[3][3] = fmaf(x.w, w.w, acc[3][3]);
         }
       }
-      // ---- tile epilogue: bias (+-), ReLU or loss
+      // ---- tile epilogue: bias (+-), hidden activation or (output activation +) loss
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         const int o = o0 + tc * 4 + c;
@@ -145,9 +149,13 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
         for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
         if (!last) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) y[i] = fmaxf(y[i], 0.f);
+          for (int i = 0; i < 4; ++i) y[i] = HID_TANH ? tanhf(y[i]) : fmaxf(y[i], 0.f);
           *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
         } else {
+          if constexpr (OUT_TANH) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) y[i] = tanhf(y[i]);
+          }
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const int b = b0 + ((r0 + i) % BC);
@@ -203,18 +211,29 @@ size_t smem_bytes(int rows, int maxw) {
   return sizeof(float) * ((size_t)2 * maxw * rows + (size_t)2 * KT * (ot + 4));
 }
 
-template <int ROWS>
-int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
-  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_kernel<ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  eval_mlp_kernel<ROWS><<<p.pairs * p.chunks, kThreads, smem, stream>>>(p);
+template <int ROWS, int ACT>
+int launch_act(const EvalParams& p, size_t smem, cudaStream_t stream) {
+  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_kernel<ROWS, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  eval_mlp_kernel<ROWS, ACT><<<p.pairs * p.chunks, kThreads, smem, stream>>>(p);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
+}
+
+template <int ROWS>
+int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
+  switch (p.desc.activation) {
+    case ESTK_ACT_TANH: return launch_act<ROWS, ESTK_ACT_TANH>(p, smem, stream);
+    case ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_OUT_TANH>(p, smem, stream);
+    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, smem, stream);
+    default: return launch_act<ROWS, ESTK_ACT_RELU>(p, smem, stream);
+  }
 }
 
 int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who) {
   const estk_mlp_desc& d = p.desc;
   ESTK_CHECK_ARG(d.n_layers >= 1 && d.n_layers <= ESTK_MAX_LAYERS, "%s: n_layers=%d", who, d.n_layers);
-  ESTK_CHECK_ARG(d.activation == 0, "%s: only ReLU (activation=0) is implemented", who);
+  ESTK_CHECK_ARG(estk_act_valid(d.activation), "%s: activation=0x%x is not a defined ESTK_ACT_* combination",
+                 who, d.activation);
   int maxw = 0;
   for (int l = 0; l <= d.n_layers; ++l) {
     ESTK_CHECK_ARG(d.dims[l] >= 1, "%s: dims[%d]=%d", who, l, d.dims[l]);

@@ -18,8 +18,9 @@
 //      is read from L2 and formed once per 256 observations;
 //   D  64 x 128 fp32 in the registers of the consumer warpgroup that owns the tile (the two
 //      consumer warpgroups take alternate N tiles); the epilogue adds the bias,
-//      applies ReLU and rounds to 16 bits straight into the other activation buffer.  The last
-//      layer is fused with the squared-error reduction (and the behaviour characterisation).
+//      applies the hidden activation (ReLU, or tanhf in fp32) and rounds to 16 bits straight into
+//      the other activation buffer.  The last layer is fused with the optional output tanhf (fp32),
+//      the squared-error reduction and the behaviour characterisation.
 // Operand modes (template MODE):
 //   kModeBF16   bf16 operands formed from fp32 theta + fp32 table (one FMA in fp32, one rounding)
 //   kModeBF16S  bf16 operands formed from bf16 shadows of theta and table (fma.rn.bf16x2)
@@ -133,9 +134,12 @@ __device__ __forceinline__ TaskId decode_task(const EvalTCParams& p, int task, b
   return t;
 }
 
-template <int MODE>
+// ACT = estk_mlp_desc.activation, a compile-time constant: the ReLU / identity instantiations are
+// the code they were before Tanh existed, and no epilogue carries a branch on the activation.
+template <int MODE, int ACT>
 __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTCParams p) {
   constexpr bool S16 = (MODE == kModeBF16S), F16 = (MODE == kModeF16);
+  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sH = smem;                                  // 2 activation buffers x 8 k-blocks x 8 KB
@@ -319,7 +323,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
 #pragma unroll
                   for (int h = 0; h < 2; ++h) {
                     const int b = chunk * kRows + r0 + 8 * h;
-                    const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                    float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                    if constexpr (OUT_TANH) { y0 = tanhf(y0); y1 = tanhf(y1); }
                     const float e0 = y0 - t[jb - jg][h].x, e1 = y1 - t[jb - jg][h].y;
                     loss = fmaf(e0, e0, loss);
                     loss = fmaf(e1, e1, loss);
@@ -347,8 +352,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
                 for (int h = 0; h < 2; ++h) {
                   const int r = r0 + 8 * h;
                   const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                  // Tanh: fp32 tanhf, then the one rounding to 16 bits (|tanh| <= 1: satfinite never fires)
                   st_shared_u32(h_out + (col >> 6) * kHBlockBytes + sw128_offset(r, (col & 63) >> 3) + (col & 7) * 2,
-                                pack16_relu<F16>(y0, y1));
+                                HID_TANH ? pack16<F16>(tanhf(y0), tanhf(y1)) : pack16_relu<F16>(y0, y1));
                 }
               }
             }
@@ -536,10 +542,10 @@ size_t tc_smem_bytes() {
 // Clusters of kCluster CTAs, one per SM, persistent over groups of kCluster tasks.  The number of
 // clusters that fit at once comes from the occupancy API: the GPCs' SM counts need not be multiples of
 // kCluster, so it can be less than sm_count / kCluster.
-template <int MODE>
+template <int MODE, int ACT>
 int launch_tc(const EvalTCParams& p, cudaStream_t stream) {
   const size_t smem = tc_smem_bytes();
-  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = kCluster;
@@ -553,14 +559,14 @@ int launch_tc(const EvalTCParams& p, cudaStream_t stream) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int clusters = 0;
-  ESTK_CUDA(cudaOccupancyMaxActiveClusters(&clusters, eval_mlp_tc_kernel<MODE>, &cfg));
+  ESTK_CUDA(cudaOccupancyMaxActiveClusters(&clusters, eval_mlp_tc_kernel<MODE, ACT>, &cfg));
   if (clusters < 1) {
     estk_set_error("eval_mlp_tc_kernel: no cluster of %d CTAs fits on this device", kCluster);
     return ESTK_ERR_CUDA;
   }
   const int items = p.n_tasks / kCluster;
   cfg.gridDim = dim3(kCluster * (clusters < items ? clusters : items));
-  ESTK_CUDA(cudaLaunchKernelEx(&cfg, eval_mlp_tc_kernel<MODE>, p));
+  ESTK_CUDA(cudaLaunchKernelEx(&cfg, eval_mlp_tc_kernel<MODE, ACT>, p));
   return ESTK_OK;
 }
 
@@ -569,7 +575,7 @@ int tc_supported(const estk_mlp_desc& d, int B, const char** why, int mode) {
     *why = "fp16 mode splits the observations into hi + lo halves: input width <= 256"; return 0;
   }
   if (d.n_layers < 1 || d.n_layers > ESTK_MAX_LAYERS) { *why = "n_layers"; return 0; }
-  if (d.activation != 0) { *why = "activation"; return 0; }
+  if (!estk_act_valid(d.activation)) { *why = "activation is not a defined ESTK_ACT_* combination"; return 0; }
   for (int l = 0; l < d.n_layers; ++l) {
     if (d.dims[l] % 64 || d.dims[l] > kMaxW || d.dims[l] < 64) { *why = "layer input width must be a multiple of 64 in [64,512]"; return 0; }
     const int N = d.dims[l + 1];
@@ -577,6 +583,16 @@ int tc_supported(const estk_mlp_desc& d, int B, const char** why, int mode) {
   }
   if (B % 256) { *why = "batch must be a multiple of 256"; return 0; }
   return 1;
+}
+
+template <int MODE>
+int launch_tc_act(const EvalTCParams& p, cudaStream_t stream) {
+  switch (p.desc.activation) {
+    case ESTK_ACT_TANH: return launch_tc<MODE, ESTK_ACT_TANH>(p, stream);
+    case ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_OUT_TANH>(p, stream);
+    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, stream);
+    default: return launch_tc<MODE, ESTK_ACT_RELU>(p, stream);
+  }
 }
 
 int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who) {
@@ -596,9 +612,9 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
 #ifdef ESTK_TC_PROFILE
   p.prof = g_prof_buf;
 #endif
-  if (p.mode == kModeF16) return launch_tc<kModeF16>(p, stream);
-  if (p.mode == kModeBF16S) return launch_tc<kModeBF16S>(p, stream);
-  return launch_tc<kModeBF16>(p, stream);
+  if (p.mode == kModeF16) return launch_tc_act<kModeF16>(p, stream);
+  if (p.mode == kModeBF16S) return launch_tc_act<kModeBF16S>(p, stream);
+  return launch_tc_act<kModeBF16>(p, stream);
 }
 
 }  // namespace

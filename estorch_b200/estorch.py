@@ -227,7 +227,7 @@ class ES:
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
             ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
-                        (always ``"fp32"`` for the conv policy);
+                        (ReLU and Tanh MLPs alike; always ``"fp32"`` for the conv policy);
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
                         ``bf16s`` additionally reads bf16 shadows of theta and the table);
                         MLP policies only.
@@ -280,7 +280,9 @@ class ES:
             self._precision = "f16"
         if self._fused and not self._is_conv and eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
-            supported = getattr(self._be, probe, lambda d, b: False)(self._spec.dims, self.agent.obs.shape[0])
+            act_kw = {"act": self._spec.act} if self._spec.act else {}     # ReLU: the backends' default
+            supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
+                                                                          **act_kw)
             if eval_precision != "auto" and not supported:
                 raise ValueError(f"eval_precision={eval_precision!r} needs layer widths that are multiples of 64 "
                                  "(in) / 32 (out), at most 512 (f16: input width at most 256), and a batch that "
@@ -386,7 +388,7 @@ class ES:
         if getattr(self, "_pending_centre", False):
             slot = self._active
             self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
-                                     **self._eval_kw(slot, True))
+                                     **self._mlp_kw(slot, True))
             self._be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
             self._pending_centre = False
             self._host_cache = {}
@@ -782,6 +784,14 @@ class ES:
             kw["table16"] = self._table_h if self._precision == "f16" else self._table16
         return kw
 
+    def _mlp_kw(self, slot, centre=False):
+        """``_eval_kw`` plus the MLP policy's activation code (include/estk.h ESTK_ACT_*).  It is
+        left out for ReLU hidden + identity output, the default of every backend."""
+        kw = self._eval_kw(slot, centre)
+        if self._spec.act:
+            kw["act"] = self._spec.act
+        return kw
+
     _streaming = False          # the agent hands a new observation batch to every generation
     _next_batch = None
     _next_batch_ptrs = None
@@ -838,7 +848,7 @@ class ES:
                              self.sigma, self._xref, self._obs, self._tgt, ret_p, ret_m, self._conv_scratch,
                              **self._eval_kw(slot))
         else:
-            kw = self._eval_kw(slot)
+            kw = self._mlp_kw(slot)
             if folded:        # the previous generation's post-update rollout rides in this launch
                 kw["centre_out"] = self._episode
             be.eval_mlp(dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
@@ -884,7 +894,7 @@ class ES:
             be.eval_conv_vbn(self._spec.n_actions, slot.theta, None, None, None, 1, 0.0, self._xref, self._obs,
                              self._tgt, self._episode, None, self._conv_scratch, **self._eval_kw(slot, True))
         else:
-            be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, **self._eval_kw(slot, True))
+            be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, **self._mlp_kw(slot, True))
         be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
 
     # ------------------------------------------------------------------ CUDA-graph replay of a generation
@@ -1281,7 +1291,7 @@ class NS_ES(ES):
             slot = self._slots[-1]
             self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
                                      self._bc_center[0], self.agent.bc_obs, self.agent.bc_dim,
-                                     **self._eval_kw(slot, True))
+                                     **self._mlp_kw(slot, True))
             return float(self._episode.item()), self._bc_center[0].cpu().numpy().copy()
         with torch.no_grad():
             return self.agent.rollout(policy)
@@ -1346,7 +1356,7 @@ class NS_ES(ES):
         nov = []
         for s in self._slots:
             be.eval_mlp_center(dims, s.theta, self._obs, self._tgt, self._episode, self._bc_center[0],
-                               self.agent.bc_obs, self.agent.bc_dim, **self._eval_kw(s, True))
+                               self.agent.bc_obs, self.agent.bc_dim, **self._mlp_kw(s, True))
             be.knn_novelty(self._bc_center, arch, self.k, self._nov_center)
             nov.append(self._nov_center.clone())
         total = torch.cat(nov).double().cpu().numpy()
@@ -1380,7 +1390,7 @@ class NS_ES(ES):
         be.eval_mlp(dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
                     self._obs, self._tgt, ret_p, ret_m,
                     BC[pb: pb + pl], BC[pairs + pb: pairs + pb + pl], ag.bc_obs, ag.bc_dim,
-                    **self._eval_kw(slot))
+                    **self._mlp_kw(slot))
         be.knn_novelty(BC[pb: pb + pl], self._arch_dev, self.k, nov_p)
         be.knn_novelty(BC[pairs + pb: pairs + pb + pl], self._arch_dev, self.k, nov_m)
         ad = self._adam_desc(slot.optimizer)
@@ -1410,7 +1420,7 @@ class NS_ES(ES):
         # _after_optimize (estorch.py:427-432 / :650-662): rollout of the updated
         # policy, archive append, best tracking, NSRA schedule (host scalars)
         be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, self._bc_center[0],
-                           ag.bc_obs, ag.bc_dim, **self._eval_kw(slot, True))
+                           ag.bc_obs, ag.bc_dim, **self._mlp_kw(slot, True))
         episode = float(self._episode.item())
         self._archive.append(self._bc_center[0].cpu().numpy().copy())
         self.episode_reward = episode

@@ -3,10 +3,11 @@
 The reference accepts any ``nn.Module`` class as ``policy`` and runs it on the
 host (estorch.py:136,142,195-202).  The fused evaluate kernel needs the
 architecture, so the module is inspected once: a chain
-``Linear -> ReLU -> ... -> Linear`` whose parameters are registered in forward
-order (examples/cartpole_es.py:6-20, examples/nsra_es.py:52-67) becomes an
-``MLPSpec``.  Anything else returns ``None`` and the engine uses the
-materialising path (rows built on the device, rollout on the host).
+``Linear -> act -> ... -> Linear [-> Tanh]`` with ``act`` ReLU or Tanh (the same on
+every hidden layer) whose parameters are registered in forward order
+(examples/cartpole_es.py:6-20, examples/nsra_es.py:52-67) becomes an ``MLPSpec``.
+Anything else returns ``None`` and the engine uses the materialising path (rows
+built on the device, rollout on the host).
 """
 from __future__ import annotations
 
@@ -17,9 +18,20 @@ import torch
 from torch import nn
 
 
+_HIDDEN_CODES = {"relu": 0, "tanh": 1}          # estk.h ESTK_ACT_RELU / ESTK_ACT_TANH
+_OUTPUT_CODES = {"identity": 0, "tanh": 1 << 8}  # 0 / ESTK_ACT_OUT_TANH
+
+
 @dataclass(frozen=True)
 class MLPSpec:
     dims: tuple  # (in, h1, ..., out)
+    hidden: str = "relu"        # activation after every Linear but the last: "relu" or "tanh"
+    output: str = "identity"    # after the last Linear: "identity" or "tanh"
+
+    @property
+    def act(self) -> int:
+        """The ``estk_mlp_desc.activation`` code of this policy (include/estk.h)."""
+        return _HIDDEN_CODES[self.hidden] | _OUTPUT_CODES[self.output]
 
     @property
     def n_parameters(self) -> int:
@@ -31,18 +43,42 @@ def _leaf_modules(module: nn.Module) -> List[nn.Module]:
     return [m for m in module.modules() if len(list(m.children())) == 0]
 
 
+def _chain(x, linears, weights, hidden, output):
+    h = x
+    for i, (l, (w, b)) in enumerate(zip(linears, weights)):
+        h = torch.nn.functional.linear(h, w, b)
+        if i + 1 < len(linears):
+            h = torch.relu(h) if hidden == "relu" else torch.tanh(h)
+    return torch.tanh(h) if output == "tanh" else h
+
+
+def _matches(y, h) -> bool:
+    return y.shape == h.shape and bool(torch.allclose(y, h, rtol=1e-4, atol=1e-5))
+
+
 def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPSpec]:
     """Return the MLPSpec of ``module`` or None.
 
-    Structural test: the leaf modules are only Linear / ReLU; every Linear has a
-    bias; widths chain; parameters are registered in layer order.
+    Structural test: the leaf modules are only Linear / ReLU / Tanh; every Linear
+    has a bias; widths chain; parameters are registered in layer order.
     Behavioural test (``probe``): a random batch through the module equals the
     chain evaluated from its flat parameters -- this rejects modules whose
     ``forward`` does something else with the same layers.
+
+    The activations are found by the probe.  A kind (ReLU / Tanh) is a candidate if
+    a leaf module of that type is registered, or if no activation module is (a
+    ``forward`` calling ``torch.relu`` / ``torch.tanh``); the output is identity or,
+    when Tanh is a candidate, Tanh.  Every (hidden, output) candidate pair is
+    compared with the module's forward under parameters redrawn at a scale that
+    keeps each layer's output O(1) (weights N(0, 1/fan_in), biases N(0, 1); the
+    module's own parameters may be too small to tell ``tanh(y)`` from ``y``), and the
+    module is accepted only when exactly one pair matches -- and matches under its
+    own parameters too.  A single Linear has no hidden layer: its hidden kind is
+    ``relu`` and only the output is probed.
     """
     leaves = _leaf_modules(module)
     linears = [m for m in leaves if isinstance(m, nn.Linear)]
-    others = [m for m in leaves if not isinstance(m, (nn.Linear, nn.ReLU))]
+    others = [m for m in leaves if not isinstance(m, (nn.Linear, nn.ReLU, nn.Tanh))]
     if not linears or others or len(linears) > 8:
         return None
     if any(l.bias is None for l in linears):
@@ -56,23 +92,37 @@ def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPS
     expect = [p for l in linears for p in (l.weight, l.bias)]
     if len(params) != len(expect) or any(a is not b for a, b in zip(params, expect)):
         return None
-    spec = MLPSpec(tuple(dims))
-    if probe:
-        with torch.no_grad():
-            dev = params[0].device
-            x = torch.randn(3, dims[0], device=dev, dtype=params[0].dtype)
-            try:
-                y = module(x)
-            except Exception:
-                return None
-            h = x
-            for i, l in enumerate(linears):
-                h = torch.nn.functional.linear(h, l.weight, l.bias)
-                if i + 1 < len(linears):
-                    h = torch.relu(h)
-            if y.shape != h.shape or not torch.allclose(y, h, rtol=1e-4, atol=1e-5):
-                return None
-    return spec
+    kinds = [k for k, t in (("relu", nn.ReLU), ("tanh", nn.Tanh)) if any(isinstance(m, t) for m in leaves)]
+    kinds = kinds or ["relu", "tanh"]
+    hiddens = kinds if len(linears) > 1 else ["relu"]
+    outputs = ["identity"] + (["tanh"] if "tanh" in kinds else [])
+    cands = [(h, o) for h in hiddens for o in outputs]
+    if not probe:                       # structure only: a Tanh needs the probe to be placed
+        return None if any(isinstance(m, nn.Tanh) for m in leaves) else MLPSpec(tuple(dims))
+    with torch.no_grad():
+        dev, dt = params[0].device, params[0].dtype
+        # the same global-RNG draw as before Tanh was recognised: module initialisations that
+        # follow the recognition (ES.__init__) see the same random stream
+        x = torch.randn(3, dims[0], device=dev, dtype=dt)
+        try:
+            y = module(x)
+        except Exception:
+            return None
+        own = [(l.weight, l.bias) for l in linears]
+        # redrawn parameters from a private generator: the global RNG is not touched
+        g = torch.Generator().manual_seed(0x5EED)
+        xr = torch.randn(8, dims[0], generator=g, dtype=dt).to(dev)
+        redrawn = [((torch.randn(l.out_features, l.in_features, generator=g, dtype=dt) / l.in_features ** 0.5).to(dev),
+                    torch.randn(l.out_features, generator=g, dtype=dt).to(dev)) for l in linears]
+        names = [n for n, _ in module.named_parameters()]
+        try:
+            yr = torch.func.functional_call(module, dict(zip(names, [t for wb in redrawn for t in wb])), (xr,))
+        except Exception:
+            return None
+        hits = [c for c in cands if _matches(yr, _chain(xr, linears, redrawn, *c))]
+        if len(hits) != 1 or not _matches(y, _chain(x, linears, own, *hits[0])):
+            return None
+    return MLPSpec(tuple(dims), *hits[0])
 
 
 @dataclass(frozen=True)

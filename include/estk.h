@@ -65,13 +65,28 @@ typedef struct {
   int32_t reserved;
 } estk_state;
 
-/* Policy description: Linear -> act -> ... -> Linear over a flat parameter
- * vector in torch.nn.utils.parameters_to_vector order (weight [out,in]
- * row-major, then bias, per layer) -- examples/cartpole_es.py:6-20. */
+/* Policy description: Linear -> act -> ... -> Linear [-> out_act] over a flat
+ * parameter vector in torch.nn.utils.parameters_to_vector order (weight [out,in]
+ * row-major, then bias, per layer) -- examples/cartpole_es.py:6-20.
+ *
+ * `activation` is two bit fields:
+ *   bits 0-7   hidden activation, applied after every Linear but the last:
+ *              ESTK_ACT_RELU (0) max(y, 0), ESTK_ACT_TANH (1) tanh(y);
+ *   bits 8-15  output activation, applied after the last Linear, before the squared
+ *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y).
+ * 0 is ReLU hidden + identity output.  Any other value is ESTK_ERR_INVALID in
+ * estk_eval_mlp* and makes estk_eval_mlp_{f16,bf16}_supported return 0.
+ * Arithmetic of tanh: IEEE tanhf (libdevice, ~1-2 ulp, no tanh.approx) on the fp32
+ * value acc + bias.  fp32 path: the result stays fp32.  Tensor-core paths: a hidden
+ * tanh is rounded ONCE to the 16-bit operand type when the activation is written back
+ * (|tanh| <= 1, so the fp16 saturation never applies); the output tanh stays fp32. */
+#define ESTK_ACT_RELU 0
+#define ESTK_ACT_TANH 1
+#define ESTK_ACT_OUT_TANH (1 << 8)
 typedef struct {
   int32_t n_layers;                  /* number of Linear layers, 1..ESTK_MAX_LAYERS */
   int32_t dims[ESTK_MAX_LAYERS + 1]; /* dims[0] = obs dim, dims[n_layers] = out dim */
-  int32_t activation;                /* 0 = ReLU between layers (none after the last) */
+  int32_t activation;                /* ESTK_ACT_* bit fields above; 0 = ReLU between layers, none after the last */
 } estk_mlp_desc;
 
 /* torch.optim.Adam hyper-parameters (torch/optim/adam.py:457-546; the
