@@ -19,6 +19,11 @@ ESTK_MAX_POPULATION = 32768
 ESTK_ACT_RELU = 0
 ESTK_ACT_TANH = 1
 ESTK_ACT_OUT_TANH = 1 << 8
+# evaluate precision codes (estk_eval_mlp, estk_eval_conv_vbn)
+ESTK_PREC_FP32 = 0
+ESTK_PREC_F16 = 1
+ESTK_PREC_BF16 = 2
+ESTK_PREC_BF16S = 3
 
 
 class EstkState(C.Structure):
@@ -41,7 +46,8 @@ class EstkAdamDesc(C.Structure):
 _P = C.c_void_p
 _I32, _I64, _U64, _F32 = C.c_int32, C.c_int64, C.c_uint64, C.c_float
 
-# name -> argtypes; every function returns int except estk_last_error.
+# name -> argtypes; every function returns int except estk_last_error (a string) and these:
+_INT64_RESULTS = {"estk_eval_conv_vbn_scratch_bytes", "estk_xr_workspace_bytes"}
 SIGNATURES = {
     "estk_version": [],
     "estk_last_error": [],
@@ -51,41 +57,25 @@ SIGNATURES = {
     "estk_fill_noise_table": [_P, _P, _I64, _U64, _P],
     "estk_make_offsets": [_P, _U64, _P, _I64, _I64, _I32, _I64, _I64, _P, _P, _P],
     "estk_perturb_rows": [_P, _P, _I64, _P, _P, _I32, _F32, _I32, _I32, _P, _P, _P],
-    "estk_eval_mlp": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _F32, _P, _P, _I32,
-                      _P, _P, _P, _P, _I32, _I32, _P],
-    "estk_eval_mlp_center": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _I32, _P, _P, _I32, _I32, _P],
-    "estk_eval_mlp_bf16": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _F32, _P, _P, _I32,
-                           _P, _P, _P, _P, _I32, _I32, _P, _P],
-    "estk_eval_mlp_center_bf16": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _I32, _P, _P, _I32, _I32, _P],
-    "estk_eval_mlp_bf16_supported": [C.POINTER(EstkMlpDesc), _I32],
-    "estk_shadow_bf16": [_P, _P, _P, _I64, _P],
-    "estk_eval_mlp_bf16s": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _P, _P, _I32, _F32, _P, _P, _I32,
-                            _P, _P, _P, _P, _I32, _I32, _P, _P],
-    "estk_eval_mlp_center_bf16s": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _P, _P, _I32, _I32, _P],
     "estk_shadow_f16": [_P, _P, _P, _I64, _P, _P],
-    "estk_eval_mlp_f16": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _P, _I32, _F32, _P, _P, _I32,
-                          _P, _P, _P, _P, _I32, _I32, _P, _P],
-    "estk_eval_mlp_center_f16": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _I32, _P, _P, _I32, _I32, _P],
-    "estk_eval_mlp_f16_supported": [C.POINTER(EstkMlpDesc), _I32],
-    "estk_eval_conv_vbn_scratch_bytes": [_P, _I32, _I32],
-    "estk_eval_conv_vbn": [_P, _I32, _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _I32, _P, _P, _P, _I64, _P],
-    "estk_eval_conv_vbn_f16_scratch_bytes": [_P, _I32, _I32],
-    "estk_eval_conv_vbn_f16": [_P, _I32, _P, _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _I32, _P, _P, _P, _I64,
-                               _P],
+    "estk_shadow_bf16": [_P, _P, _P, _I64, _P],
+    "estk_eval_mlp": [_P, C.POINTER(EstkMlpDesc), _I32, _P, _P, _P, _P, _P, _P, _I32, _F32, _P, _P, _I32,
+                      _P, _P, _P, _P, _I32, _I32, _P, _P],
+    "estk_eval_mlp_supported": [C.POINTER(EstkMlpDesc), _I32, _I32],
+    "estk_eval_conv_vbn_scratch_bytes": [_P, _I32, _I32, _I32],
+    "estk_eval_conv_vbn": [_P, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _I32, _P, _P, _P, _I64,
+                           _P],
     "estk_track_best": [_P, _P, _P, _P, _P, _I64, _P],
-    "estk_rank_grad_adam": [_P, _P, _P, _F32, _F32, _I32, _P, _P, _P, _I64, _P, _P, _P, _P,
+    "estk_rank_grad_adam": [_P, _P, _P, _F32, _F32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P,
                             C.POINTER(EstkAdamDesc), _P, _P, _P, _P],
-    "estk_rank_grad": [_P, _P, _P, _F32, _F32, _I32, _P, _P, _P, _I32, _I32, _I64, _P, _P, _P, _P],
-    "estk_rank_grad_adam_h": [_P, _P, _P, _F32, _F32, _I32, _P, _P, _P, _I64, _P, _P, _P, _P,
-                              C.POINTER(EstkAdamDesc), _P, _P, _P, _P],
-    "estk_rank_grad_h": [_P, _P, _P, _F32, _F32, _I32, _I32, _P, _P, _P, _I32, _I32, _I64, _P, _P, _P, _P],
+    "estk_rank_grad": [_P, _P, _P, _F32, _F32, _I32, _I32, _P, _P, _P, _P, _I32, _I32, _I64, _P, _P, _P, _P],
     "estk_xr_workspace_bytes": [_I64],
     "estk_peer_alloc": [_P, _I64, C.POINTER(C.c_void_p), C.c_char_p],
     "estk_peer_open": [_P, C.c_char_p, C.POINTER(C.c_void_p)],
     "estk_peer_close": [_P, _P],
     "estk_peer_free": [_P, _P],
-    "estk_rank_grad_xr_adam_h": [_P, _P, _P, _F32, _F32, _I32, _I32, _I32, _P, _P, _P, _I32, _I32, _I64,
-                                 C.POINTER(C.c_void_p), _P, _P, _P, _P, C.POINTER(EstkAdamDesc), _P, _P, _P, _P],
+    "estk_rank_grad_xr_adam": [_P, _P, _P, _F32, _F32, _I32, _I32, _I32, _P, _P, _P, _I32, _I32, _I64,
+                               C.POINTER(C.c_void_p), _P, _P, _P, _P, C.POINTER(EstkAdamDesc), _P, _P, _P, _P],
     "estk_clamp_adam": [_P, _P, _I32, _I64, _P, _P, _P, _P, C.POINTER(EstkAdamDesc), _P, _P],
     "estk_knn_novelty": [_P, _P, _I32, _P, _I32, _I32, _I32, _P, _P],
 }
@@ -108,8 +98,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = (C.c_char_p if name == "estk_last_error" else
-                      C.c_int64 if name in ("estk_eval_conv_vbn_scratch_bytes", "estk_eval_conv_vbn_f16_scratch_bytes",
-                                           "estk_xr_workspace_bytes") else C.c_int)
+                      C.c_int64 if name in _INT64_RESULTS else C.c_int)
     _lib = lib
     return lib
 

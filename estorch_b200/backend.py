@@ -60,6 +60,11 @@ def adam_desc(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, clamp=1.0
     return a
 
 
+# eval_precision -> (ESTK_PREC_* code, dtype of its 16-bit theta16 / table16 buffers)
+_PRECISIONS = {"fp32": (_capi.ESTK_PREC_FP32, None), "f16": (_capi.ESTK_PREC_F16, torch.float16),
+               "bf16": (_capi.ESTK_PREC_BF16, None), "bf16s": (_capi.ESTK_PREC_BF16S, torch.bfloat16)}
+
+
 class CudaBackend:
     """Kernel interface over libestk.so on one CUDA device."""
 
@@ -145,13 +150,20 @@ class CudaBackend:
         self.launches += 1
 
     # ---------------------------------------------------------------- evaluate
+    def _precision(self, precision):
+        """ESTK_PREC_* code and the dtype of the 16-bit buffers (theta16 / table16) of an evaluate precision."""
+        try:
+            return _PRECISIONS[precision]
+        except KeyError:
+            raise ValueError(f"unknown precision {precision!r}") from None
+
     def eval_supports_bf16(self, dims, B, act=0) -> bool:
         d = mlp_desc(dims, act)
-        return bool(self.lib.estk_eval_mlp_bf16_supported(C.byref(d), int(B)))
+        return bool(self.lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_BF16, int(B)))
 
     def eval_supports_f16(self, dims, B, act=0) -> bool:
         d = mlp_desc(dims, act)
-        return bool(self.lib.estk_eval_mlp_f16_supported(C.byref(d), int(B)))
+        return bool(self.lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16, int(B)))
 
     def shadow_f16(self, src, dst, check=True) -> int:
         """dst (float16, same numel) = src; returns how many entries were NOT exactly
@@ -175,88 +187,48 @@ class CudaBackend:
     def eval_mlp(self, dims, theta, table, offsets, order, pairs, sigma, obs, target,
                  ret_plus, ret_minus, bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32",
                  theta16=None, table16=None, centre_out=None, act=0):
+        """Population evaluate (estk_eval_mlp); ``offsets`` None = the centre evaluation into ``ret_plus[0]``."""
+        code, dt16 = self._precision(precision)
         d = mlp_desc(dims, act)
         if obs.shape != (obs.shape[0], dims[0]) or target.shape != (obs.shape[0], dims[-1]):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match dims {list(dims)}")
-        common = (self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
-                  float(sigma), self._ptr(obs, torch.float32, "obs"), self._ptr(target, torch.float32, "target"),
-                  int(obs.shape[0]), self._ptr(ret_plus, torch.float32, "ret_plus"),
-                  self._ptr(ret_minus, torch.float32, "ret_minus"), self._ptr(bc_plus, torch.float32, "bc_plus"),
-                  self._ptr(bc_minus, torch.float32, "bc_minus"), int(bc_obs), int(bc_dim))
-        stream = (self._stream(),)
-        if precision in ("f16", "bf16", "bf16s"):
-            stream = (self._ptr(centre_out, torch.float32, "centre_out"), self._stream())
-        elif centre_out is not None:
-            raise ValueError("centre_out (folded post-update rollout) needs a tensor-core precision mode")
-        common = common + stream
-        th, tb = self._ptr(theta, torch.float32, "theta"), self._ptr(table, torch.float32, "table")
-        if precision == "f16":
-            if table16 is None:
-                raise ValueError("precision='f16' needs table16, the exact fp16 copy of the table (see shadow_f16)")
-            rc = self.lib.estk_eval_mlp_f16(self._ctx, C.byref(d), th, tb,
-                                            self._ptr(table16, torch.float16, "table16"), *common)
-        elif precision == "bf16s":
-            if theta16 is None or table16 is None:
-                raise ValueError("precision='bf16s' needs theta16 and table16 (see shadow_bf16)")
-            rc = self.lib.estk_eval_mlp_bf16s(self._ctx, C.byref(d), th, self._ptr(theta16, torch.bfloat16, "theta16"),
-                                              tb, self._ptr(table16, torch.bfloat16, "table16"), *common)
-        elif precision == "bf16":
-            rc = self.lib.estk_eval_mlp_bf16(self._ctx, C.byref(d), th, tb, *common)
-        elif precision == "fp32":
-            rc = self.lib.estk_eval_mlp(self._ctx, C.byref(d), th, tb, *common)
-        else:
-            raise ValueError(f"unknown precision {precision!r}")
-        _capi.check(rc, "estk_eval_mlp[" + precision + "]")
-        self.launches += 2 if precision == "f16" else 1      # f16: observation image + evaluate
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"),
+            self._ptr(theta16, dt16, "theta16"), self._ptr(table, torch.float32, "table"),
+            self._ptr(table16, dt16, "table16"), self._ptr(offsets, torch.int64, "offsets"),
+            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
+            self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
+            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
+            int(bc_obs), int(bc_dim), self._ptr(centre_out, torch.float32, "centre_out"), self._stream()),
+            f"estk_eval_mlp[{precision}]")
+        self.launches += 1
 
     def eval_mlp_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
                         precision="fp32", theta16=None, act=0):
-        d = mlp_desc(dims, act)
-        tail = (self._ptr(obs, torch.float32, "obs"), self._ptr(target, torch.float32, "target"),
-                int(obs.shape[0]), self._ptr(ret_out, torch.float32, "ret_out"),
-                self._ptr(bc_out, torch.float32, "bc_out"), int(bc_obs), int(bc_dim), self._stream())
-        th = self._ptr(theta, torch.float32, "theta")
-        if precision == "f16":
-            rc = self.lib.estk_eval_mlp_center_f16(self._ctx, C.byref(d), th, *tail)
-        elif precision == "bf16s":
-            rc = self.lib.estk_eval_mlp_center_bf16s(self._ctx, C.byref(d), th,
-                                                     self._ptr(theta16, torch.bfloat16, "theta16"), *tail)
-        elif precision == "bf16":
-            rc = self.lib.estk_eval_mlp_center_bf16(self._ctx, C.byref(d), th, *tail)
-        else:
-            rc = self.lib.estk_eval_mlp_center(self._ctx, C.byref(d), th, *tail)
-        _capi.check(rc, "estk_eval_mlp_center[" + precision + "]")
-        self.launches += 2 if precision == "f16" else 1
+        """Unperturbed policy: ``ret_out[0]`` = return of theta, ``bc_out`` its behaviour characteristic."""
+        self.eval_mlp(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs, bc_dim,
+                      precision=precision, theta16=theta16, act=act)
 
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
-        if precision == "f16":
-            return int(self.lib.estk_eval_conv_vbn_f16_scratch_bytes(self._ctx, int(ref_batch), int(B)))
-        if precision != "fp32":
-            raise ValueError(f"the conv + VirtualBatchNorm evaluate has no {precision!r} mode")
-        return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, int(ref_batch), int(B)))
+        return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),
+                                                             int(B)))
 
     def eval_conv_vbn(self, n_actions, theta, table, offsets, order, pairs, sigma, xref, obs, target,
                       ret_plus, ret_minus, scratch, precision="fp32", table16=None):
         """Conv + VirtualBatchNorm policy (examples/atari.py:14-37); offsets None = centre.
         precision "f16": the tensor-core kernel (needs table16 with offsets, and a scratch of
         conv_scratch_bytes(R, B, "f16") bytes)."""
-        head = (self._ctx, int(n_actions), self._ptr(theta, torch.float32, "theta"),
-                self._ptr(table, torch.float32, "table"))
-        tail = (self._ptr(offsets, torch.int64, "offsets"),
-                self._ptr(order, torch.int32, "order"), int(pairs), float(sigma),
-                self._ptr(xref, torch.float32, "xref"), int(xref.shape[0]), self._ptr(obs, torch.float32, "obs"),
-                self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
-                self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
-                self._ptr(scratch, torch.uint8, "scratch"), scratch.numel(), self._stream())
-        if precision == "f16":
-            if offsets is not None and table16 is None:
-                raise ValueError("precision='f16' needs table16, the exact fp16 copy of the table (see shadow_f16)")
-            rc = self.lib.estk_eval_conv_vbn_f16(*head, self._ptr(table16, torch.float16, "table16"), *tail)
-        elif precision == "fp32":
-            rc = self.lib.estk_eval_conv_vbn(*head, *tail)
-        else:
-            raise ValueError(f"the conv + VirtualBatchNorm evaluate has no {precision!r} mode")
-        _capi.check(rc, "estk_eval_conv_vbn[" + precision + "]")
+        code, dt16 = self._precision(precision)
+        _capi.check(self.lib.estk_eval_conv_vbn(
+            self._ctx, code, int(n_actions), self._ptr(theta, torch.float32, "theta"),
+            self._ptr(table, torch.float32, "table"), self._ptr(table16, dt16, "table16"),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+            float(sigma), self._ptr(xref, torch.float32, "xref"), int(xref.shape[0]),
+            self._ptr(obs, torch.float32, "obs"), self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
+            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+            self._ptr(scratch, torch.uint8, "scratch"), scratch.numel(), self._stream()),
+            f"estk_eval_conv_vbn[{precision}]")
         self.launches += 1
 
     def track_best(self, state, reward, theta, best_theta):
@@ -267,16 +239,19 @@ class CudaBackend:
         self.launches += 1
 
     # ---------------------------------------------------------------- rank + grad + Adam
+    def _tables(self, table):
+        """(table, table16) pointers of estk_rank_grad*: ``table`` is float32, or float16 = the exact 16-bit
+        copy (half the bytes, same result)."""
+        if table.dtype == torch.float16:
+            return None, self._ptr(table, torch.float16, "table16")
+        return self._ptr(table, torch.float32, "table"), None
+
     def rank_grad_adam(self, returns, novelty, w_rew, w_nov, P, table, offsets, order, theta, m, v,
                        state, adam, ranks_out=None, ranks2_out=None, grad_out=None):
-        """``table`` float32, or float16 = the exact 16-bit copy (half the bytes, same result)."""
-        h = table.dtype == torch.float16
-        fn = self.lib.estk_rank_grad_adam_h if h else self.lib.estk_rank_grad_adam
-        _capi.check(fn(
+        _capi.check(self.lib.estk_rank_grad_adam(
             self._ctx, self._ptr(returns, torch.float32, "returns"),
-            self._ptr(novelty, torch.float32, "novelty"), float(w_rew), float(w_nov), int(P),
-            self._ptr(table, table.dtype if h else torch.float32, "table"), self._ptr(offsets, torch.int64, "offsets"),
-            self._ptr(order, torch.int32, "order"), theta.numel(),
+            self._ptr(novelty, torch.float32, "novelty"), float(w_rew), float(w_nov), int(P), *self._tables(table),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), theta.numel(),
             self._ptr(theta, torch.float32, "theta"), self._ptr(m, torch.float32, "m"),
             self._ptr(v, torch.float32, "v"), self._ptr(state, torch.uint8, "state"), C.byref(adam),
             self._ptr(ranks_out, torch.int32, "ranks_out"), self._ptr(ranks2_out, torch.int32, "ranks2_out"),
@@ -285,22 +260,14 @@ class CudaBackend:
 
     def rank_grad(self, returns, novelty, w_rew, w_nov, P, table, offsets, order, pair_begin,
                   pairs_local, n, grad_sum_out, ranks_out=None, ranks2_out=None, world=1):
-        """``table`` float32 (member-order returns only), or float16 = the exact 16-bit copy;
-        with the latter ``world > 1`` declares rank-major returns ``[world][2][pairs/world]``."""
-        tail = (self._ptr(offsets, torch.int64, "offsets"),
-                self._ptr(order, torch.int32, "order"), int(pair_begin), int(pairs_local), int(n),
-                self._ptr(grad_sum_out, torch.float32, "grad_sum_out"),
-                self._ptr(ranks_out, torch.int32, "ranks_out"), self._ptr(ranks2_out, torch.int32, "ranks2_out"),
-                self._stream())
-        head = (self._ctx, self._ptr(returns, torch.float32, "returns"),
-                self._ptr(novelty, torch.float32, "novelty"), float(w_rew), float(w_nov), int(P))
-        if table.dtype == torch.float16:
-            rc = self.lib.estk_rank_grad_h(*head, int(world), self._ptr(table, torch.float16, "table16"), *tail)
-        else:
-            if world != 1:
-                raise ValueError("rank-major returns (world > 1) need the fp16 table entry point")
-            rc = self.lib.estk_rank_grad(*head, self._ptr(table, torch.float32, "table"), *tail)
-        _capi.check(rc, "estk_rank_grad")
+        """``world > 1`` declares rank-major returns ``[world][2][pairs/world]``."""
+        _capi.check(self.lib.estk_rank_grad(
+            self._ctx, self._ptr(returns, torch.float32, "returns"), self._ptr(novelty, torch.float32, "novelty"),
+            float(w_rew), float(w_nov), int(P), int(world), *self._tables(table),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pair_begin),
+            int(pairs_local), int(n), self._ptr(grad_sum_out, torch.float32, "grad_sum_out"),
+            self._ptr(ranks_out, torch.int32, "ranks_out"), self._ptr(ranks2_out, torch.int32, "ranks2_out"),
+            self._stream()), "estk_rank_grad")
         self.launches += 1
 
     # ---------------------------------------------------------------- peer memory (CUDA IPC)
@@ -339,14 +306,14 @@ class CudaBackend:
         """Rank + partial gradient + cross-GPU sum over peer memory + Adam in one launch (estk.h).
         ``returns`` / ``novelty`` rank-major; ``peer_ptrs`` = every rank's workspace as mapped here."""
         arr = (C.c_void_p * world)(*[C.c_void_p(x) for x in peer_ptrs])
-        _capi.check(self.lib.estk_rank_grad_xr_adam_h(
+        _capi.check(self.lib.estk_rank_grad_xr_adam(
             self._ctx, self._ptr(returns, torch.float32, "returns"), self._ptr(novelty, torch.float32, "novelty"),
             float(w_rew), float(w_nov), int(P), int(world), int(rank), self._ptr(table16, torch.float16, "table16"),
             self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pair_begin),
             int(pairs_local), theta.numel(), arr, self._ptr(theta, torch.float32, "theta"),
             self._ptr(m, torch.float32, "m"), self._ptr(v, torch.float32, "v"), self._ptr(state, torch.uint8, "state"),
             C.byref(adam), self._ptr(ranks_out, torch.int32, "ranks_out"), self._ptr(ranks2_out, torch.int32, "ranks2_out"),
-            self._ptr(grad_out, torch.float32, "grad_out"), self._stream()), "estk_rank_grad_xr_adam_h")
+            self._ptr(grad_out, torch.float32, "grad_out"), self._stream()), "estk_rank_grad_xr_adam")
         self.launches += 1
 
     def clamp_adam(self, grad_sum, P, theta, m, v, state, adam, grad_out=None):
@@ -355,7 +322,7 @@ class CudaBackend:
             self._ptr(theta, torch.float32, "theta"), self._ptr(m, torch.float32, "m"),
             self._ptr(v, torch.float32, "v"), self._ptr(state, torch.uint8, "state"), C.byref(adam),
             self._ptr(grad_out, torch.float32, "grad_out"), self._stream()), "estk_clamp_adam")
-        self.launches += 2 if theta is not None else 1
+        self.launches += 1
 
     # ---------------------------------------------------------------- novelty
     def knn_novelty(self, bc, archive, k, novelty_out):
@@ -364,4 +331,4 @@ class CudaBackend:
             self._ctx, self._ptr(bc, torch.float32, "bc"), int(count),
             self._ptr(archive, torch.float32, "archive"), int(archive.shape[0]), int(dim), int(k),
             self._ptr(novelty_out, torch.float32, "novelty_out"), self._stream()), "estk_knn_novelty")
-        self.launches += 2
+        self.launches += 2      # frob_kernel + knn_novelty_kernel

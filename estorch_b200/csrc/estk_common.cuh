@@ -52,6 +52,52 @@ struct estk_ctx {
 };
 static const int kEvalMaxChunks = 64;   // the tensor-core evaluate writes up to 2 * kEvalMaxChunks partials per member
 
+// ---------------------------------------------------------------- evaluate back ends
+// estk_eval_mlp and estk_eval_conv_vbn check their arguments once, then hand the call to the
+// kernel file of the requested precision.  A centre call (offsets == NULL) arrives with table =
+// theta, pairs = 1, sigma = 0 and no minus outputs; buffers the precision does not read are null.
+struct EvalMlpCall {
+  estk_mlp_desc desc;
+  int precision;  // ESTK_PREC_*
+  const float* theta;
+  const uint16_t* theta16;
+  const float* table;
+  const uint16_t* table16;
+  const int64_t* offsets;
+  const int32_t* order;
+  int pairs;
+  float sigma;
+  const float* obs;
+  const float* target;
+  int B;
+  float* ret_plus;
+  float* ret_minus;
+  float* bc_plus;
+  float* bc_minus;
+  int bc_obs, bc_dim;
+  float* centre_out;
+};
+int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);     // estk_eval_mlp_tc.cu
+
+struct EvalConvCall {
+  int A, R, B;  // n_actions, ref_batch, batch
+  const float* theta;
+  const float* table;
+  const uint16_t* table16;
+  const int64_t* offsets;
+  const int32_t* order;
+  int pairs;
+  float sigma;
+  const float* xref;
+  const float* obs;
+  const float* target;
+  float* ret_plus;
+  float* ret_minus;
+  void* scratch;
+};
+int64_t eval_conv_tc_scratch_per_cta(int R, int B);                              // estk_eval_conv_tc.cu
+int eval_conv_tc(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream);
+
 // ---------------------------------------------------------------- hashing
 // splitmix64 finaliser; must stay in lock-step with oracle/es_oracle.py:mix64
 // and estorch_b200/noise.py.

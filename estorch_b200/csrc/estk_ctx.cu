@@ -75,7 +75,7 @@ extern "C" int estk_ctx_info(estk_ctx* c, int* sm_count, int* cc_major, int* cc_
 
 
 // ------------------------------------------------------------------ peer memory (CUDA IPC)
-// Device memory another process on the same node can map (estk.h: estk_rank_grad_xr_adam_h).
+// Device memory another process on the same node can map (estk.h: estk_rank_grad_xr_adam).
 extern "C" int estk_peer_alloc(estk_ctx* ctx, int64_t bytes, void** ptr_out, unsigned char* handle_out) {
   ESTK_CHECK_ARG(ctx && ptr_out && handle_out && bytes > 0, "estk_peer_alloc: bad argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == ESTK_PEER_HANDLE_BYTES, "handle size");

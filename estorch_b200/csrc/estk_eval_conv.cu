@@ -302,24 +302,40 @@ size_t conv_smem_bytes() {
 
 }  // namespace
 
-extern "C" int64_t estk_eval_conv_vbn_scratch_bytes(estk_ctx* ctx, int32_t ref_batch, int32_t B) {
+extern "C" int64_t estk_eval_conv_vbn_scratch_bytes(estk_ctx* ctx, int32_t precision, int32_t ref_batch, int32_t B) {
   if (!ctx || ref_batch < 2 || B < 1) return -1;
+  if (precision == ESTK_PREC_F16) return (int64_t)ctx->sm_count * eval_conv_tc_scratch_per_cta(ref_batch, B);
+  if (precision != ESTK_PREC_FP32) return -1;
   return (int64_t)ctx->sm_count * ((int64_t)ref_batch * P1 + (int64_t)B * P2) * (int64_t)sizeof(float);
 }
 
-extern "C" int estk_eval_conv_vbn(estk_ctx* ctx, int32_t n_actions, const float* theta, const float* table,
+extern "C" int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_actions, const float* theta,
+                                  const float* table, const uint16_t* table16,
                                   const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
                                   const float* xref, int32_t ref_batch, const float* obs, const float* target,
                                   int32_t B, float* returns_plus, float* returns_minus, void* scratch,
                                   int64_t scratch_bytes, void* stream) {
+  const bool f16 = precision == ESTK_PREC_F16;
   ESTK_CHECK_ARG(ctx && theta && xref && obs && target && returns_plus && scratch, "estk_eval_conv_vbn: null argument");
-  ESTK_CHECK_ARG(offsets == nullptr || (table && returns_minus), "estk_eval_conv_vbn: table/returns_minus required with offsets");
+  ESTK_CHECK_ARG(offsets == nullptr || (table && (table16 || !f16) && returns_minus),
+                 "estk_eval_conv_vbn: table%s/returns_minus required with offsets", f16 ? "/table16" : "");
   ESTK_CHECK_ARG(n_actions >= 1 && n_actions <= 64, "estk_eval_conv_vbn: n_actions=%d", n_actions);
   ESTK_CHECK_ARG(ref_batch >= 2 && B >= 1, "estk_eval_conv_vbn: ref_batch must be >= 2 (unbiased variance), B >= 1");
   ESTK_CHECK_ARG(pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2, "estk_eval_conv_vbn: pairs=%d", pairs);
   ESTK_CHECK_ARG(ESTK_ALIGNED16(xref) && ESTK_ALIGNED16(obs), "estk_eval_conv_vbn: images must be 16-byte aligned");
-  const int64_t need = estk_eval_conv_vbn_scratch_bytes(ctx, ref_batch, B);
+  ESTK_CHECK_ARG(!f16 || (ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(scratch) && (table16 == nullptr || ESTK_ALIGNED16(table16))),
+                 "estk_eval_conv_vbn: f16 needs theta, table16 and scratch 16-byte aligned");
+  if (!f16 && precision != ESTK_PREC_FP32) {
+    estk_set_error("estk_eval_conv_vbn: precision %d is not supported (ESTK_PREC_FP32 or ESTK_PREC_F16)", precision);
+    return ESTK_ERR_UNSUPPORTED;
+  }
+  const int64_t need = estk_eval_conv_vbn_scratch_bytes(ctx, precision, ref_batch, B);
   ESTK_CHECK_ARG(scratch_bytes >= need, "estk_eval_conv_vbn: scratch %lld < %lld bytes", (long long)scratch_bytes, (long long)need);
+  if (f16) {
+    const EvalConvCall c = {n_actions, ref_batch, B, theta, table, table16, offsets, order, pairs, sigma,
+                            xref, obs, target, returns_plus, returns_minus, scratch};
+    return eval_conv_tc(ctx, c, (cudaStream_t)stream);
+  }
   ConvParams p = {};
   p.theta = theta; p.table = table; p.offsets = offsets; p.order = order; p.pairs = pairs; p.sigma = sigma;
   p.A = n_actions; p.R = ref_batch; p.B = B; p.xref = xref; p.obs = obs; p.target = target;

@@ -447,47 +447,27 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
   }
 }
 
-int64_t per_cta_bytes(int R, int B) {
+}  // namespace
+
+int64_t eval_conv_tc_scratch_per_cta(int R, int B) {
   return (int64_t)R * P1 * (int64_t)sizeof(float) + 2 * (int64_t)B * P2 * (int64_t)sizeof(__half);
 }
 
-}  // namespace
-
-extern "C" int64_t estk_eval_conv_vbn_f16_scratch_bytes(estk_ctx* ctx, int32_t ref_batch, int32_t B) {
-  if (!ctx || ref_batch < 2 || B < 1) return -1;
-  return (int64_t)ctx->sm_count * per_cta_bytes(ref_batch, B);
-}
-
-extern "C" int estk_eval_conv_vbn_f16(estk_ctx* ctx, int32_t n_actions, const float* theta, const float* table,
-                                      const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                                      int32_t pairs, float sigma, const float* xref, int32_t ref_batch,
-                                      const float* obs, const float* target, int32_t B, float* returns_plus,
-                                      float* returns_minus, void* scratch, int64_t scratch_bytes, void* stream) {
-  ESTK_CHECK_ARG(ctx && theta && xref && obs && target && returns_plus && scratch, "estk_eval_conv_vbn_f16: null argument");
-  ESTK_CHECK_ARG(offsets == nullptr || (table && table16 && returns_minus),
-                 "estk_eval_conv_vbn_f16: table/table16/returns_minus required with offsets");
-  ESTK_CHECK_ARG(n_actions >= 1 && n_actions <= 64, "estk_eval_conv_vbn_f16: n_actions=%d", n_actions);
-  ESTK_CHECK_ARG(ref_batch >= 2 && B >= 1, "estk_eval_conv_vbn_f16: ref_batch must be >= 2 (unbiased variance), B >= 1");
-  ESTK_CHECK_ARG(pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2, "estk_eval_conv_vbn_f16: pairs=%d", pairs);
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(xref) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(scratch) &&
-                 (table16 == nullptr || ESTK_ALIGNED16(table16)),
-                 "estk_eval_conv_vbn_f16: theta, images, table16 and scratch must be 16-byte aligned");
-  const int64_t need = estk_eval_conv_vbn_f16_scratch_bytes(ctx, ref_batch, B);
-  ESTK_CHECK_ARG(scratch_bytes >= need, "estk_eval_conv_vbn_f16: scratch %lld < %lld bytes", (long long)scratch_bytes,
-                 (long long)need);
+// estk_eval_conv_vbn with ESTK_PREC_F16 (estk_eval_conv.cu has checked the arguments)
+int eval_conv_tc(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream) {
   ConvTcParams p = {};
-  p.theta = theta; p.table16 = reinterpret_cast<const __half*>(table16); p.offsets = offsets; p.order = order;
-  p.pairs = pairs; p.sigma = sigma;
-  p.A = n_actions; p.R = ref_batch; p.B = B; p.xref = xref; p.obs = obs; p.target = target;
-  p.ret_plus = returns_plus; p.ret_minus = returns_minus;
-  p.scratch = reinterpret_cast<unsigned char*>(scratch);
-  p.scratch_per_cta = per_cta_bytes(ref_batch, B);
-  p.members = offsets ? 2 * pairs : 1;
+  p.theta = c.theta; p.table16 = reinterpret_cast<const __half*>(c.table16); p.offsets = c.offsets; p.order = c.order;
+  p.pairs = c.pairs; p.sigma = c.sigma;
+  p.A = c.A; p.R = c.R; p.B = c.B; p.xref = c.xref; p.obs = c.obs; p.target = c.target;
+  p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
+  p.scratch = reinterpret_cast<unsigned char*>(c.scratch);
+  p.scratch_per_cta = eval_conv_tc_scratch_per_cta(c.R, c.B);
+  p.members = c.offsets ? 2 * c.pairs : 1;
   const size_t smem = sizeof(Smem);
   ESTK_CUDA(cudaFuncSetAttribute(eval_conv_vbn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = ctx->sm_count;
   if (grid > p.members) grid = p.members;
-  eval_conv_vbn_tc_kernel<<<grid, kT, smem, (cudaStream_t)stream>>>(p);
+  eval_conv_vbn_tc_kernel<<<grid, kT, smem, stream>>>(p);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
 }

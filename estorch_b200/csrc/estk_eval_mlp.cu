@@ -268,33 +268,49 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
 
 }  // namespace
 
-extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                             const float* table, const int64_t* offsets, const int32_t* order,
-                             int32_t pairs, float sigma, const float* obs, const float* target,
-                             int32_t B, float* returns_plus, float* returns_minus, float* bc_plus,
-                             float* bc_minus, int32_t bc_obs, int32_t bc_dim, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && table && offsets && obs && target && returns_plus && returns_minus,
-                 "estk_eval_mlp: null argument");
-  ESTK_CHECK_ARG((bc_plus == nullptr) == (bc_minus == nullptr), "estk_eval_mlp: bc_plus/bc_minus must both be set or both null");
+// The one MLP evaluate entry point of every precision: the argument checks of all of them, then
+// run_eval (fp32, here) or eval_mlp_tc (estk_eval_mlp_tc.cu).
+extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t precision, const float* theta,
+                             const uint16_t* theta16, const float* table, const uint16_t* table16,
+                             const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
+                             const float* obs, const float* target, int32_t B, float* returns_plus,
+                             float* returns_minus, float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
+                             float* centre_return_out, void* stream) {
+  const bool tc = precision == ESTK_PREC_F16 || precision == ESTK_PREC_BF16 || precision == ESTK_PREC_BF16S;
+  const bool shadows = precision == ESTK_PREC_BF16S;                 // reads theta16, and table16 as a bf16 shadow
+  const bool t16 = shadows || precision == ESTK_PREC_F16;            // a population reads table16
+  const bool centre = offsets == nullptr;
+  ESTK_CHECK_ARG(tc || precision == ESTK_PREC_FP32, "estk_eval_mlp: unknown precision %d", precision);
+  ESTK_CHECK_ARG(ctx && desc && theta && obs && target && returns_plus && (theta16 || !shadows) &&
+                 (centre || (table && (table16 || !t16) && returns_minus)), "estk_eval_mlp: null argument");
+  ESTK_CHECK_ARG(centre || (bc_plus == nullptr) == (bc_minus == nullptr),
+                 "estk_eval_mlp: bc_plus/bc_minus must both be set or both null");
   ESTK_CHECK_ARG(!bc_plus || (bc_obs > 0 && bc_dim > 0), "estk_eval_mlp: bc_obs/bc_dim must be positive with bc outputs");
+  ESTK_CHECK_ARG(!centre_return_out || !centre, "estk_eval_mlp: centre_return_out needs a population (offsets)");
+  ESTK_CHECK_ARG(!tc || (ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target) &&
+                         (!shadows || ESTK_ALIGNED16(theta16)) &&
+                         (centre || (ESTK_ALIGNED16(table) && (!t16 || ESTK_ALIGNED16(table16))))),
+                 "estk_eval_mlp: tensor-core buffers must be 16-byte aligned");
+  if (centre_return_out && !tc) {
+    estk_set_error("estk_eval_mlp: centre_return_out (folded centre rollout) needs a tensor-core precision");
+    return ESTK_ERR_UNSUPPORTED;
+  }
+  EvalMlpCall c = {};
+  c.desc = *desc; c.precision = precision; c.theta = theta; c.obs = obs; c.target = target; c.B = B;
+  c.ret_plus = returns_plus; c.bc_plus = bc_plus; c.bc_obs = bc_obs; c.bc_dim = bc_dim;
+  c.theta16 = shadows ? theta16 : nullptr;
+  if (centre) {
+    c.table = theta; c.table16 = c.theta16; c.pairs = 1; c.sigma = 0.f;
+  } else {
+    c.table = table; c.table16 = t16 ? table16 : nullptr; c.offsets = offsets; c.order = order;
+    c.pairs = pairs; c.sigma = sigma; c.ret_minus = returns_minus; c.bc_minus = bc_minus;
+    c.centre_out = centre_return_out;
+  }
+  if (tc) return eval_mlp_tc(ctx, c, (cudaStream_t)stream);
   EvalParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = table; p.offsets = offsets; p.order = order;
-  p.pairs = pairs; p.sigma = sigma; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.ret_minus = returns_minus;
-  p.bc_plus = bc_plus; p.bc_minus = bc_minus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
+  p.desc = c.desc; p.theta = c.theta; p.table = c.table; p.offsets = c.offsets; p.order = c.order;
+  p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.target = c.target; p.B = c.B;
+  p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
+  p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
   return run_eval(ctx, p, (cudaStream_t)stream, "estk_eval_mlp");
-}
-
-extern "C" int estk_eval_mlp_center(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                    const float* obs, const float* target, int32_t B,
-                                    float* return_out, float* bc_out, int32_t bc_obs,
-                                    int32_t bc_dim, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && obs && target && return_out, "estk_eval_mlp_center: null argument");
-  ESTK_CHECK_ARG(!bc_out || (bc_obs > 0 && bc_dim > 0), "estk_eval_mlp_center: bc_obs/bc_dim must be positive with bc_out");
-  EvalParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = theta; p.offsets = nullptr; p.order = nullptr;
-  p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = return_out; p.ret_minus = nullptr;
-  p.bc_plus = bc_out; p.bc_minus = nullptr; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  return run_eval(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center");
 }

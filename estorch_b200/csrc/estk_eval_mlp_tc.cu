@@ -76,6 +76,12 @@ constexpr int kItemsPT = kTileN / kCluster * (kBlockK / 8) / kPT;
 constexpr int kTgtBatch = 2;                       // last-layer epilogue: column blocks per target batch
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
 
+// ESTK_PREC_* -> operand mode; -1 for a precision without a tensor-core kernel
+constexpr int mode_of(int precision) {
+  return precision == ESTK_PREC_F16 ? kModeF16 : precision == ESTK_PREC_BF16 ? kModeBF16
+       : precision == ESTK_PREC_BF16S ? kModeBF16S : -1;
+}
+
 struct EvalTCParams {
   estk_mlp_desc desc;
   const float* theta;
@@ -619,38 +625,16 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
 
 }  // namespace
 
-extern "C" int estk_eval_mlp_bf16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                  const float* table, const int64_t* offsets, const int32_t* order,
-                                  int32_t pairs, float sigma, const float* obs, const float* target,
-                                  int32_t B, float* returns_plus, float* returns_minus, float* bc_plus,
-                                  float* bc_minus, int32_t bc_obs, int32_t bc_dim, float* centre_return_out,
-                                  void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && table && offsets && obs && target && returns_plus && returns_minus,
-                 "estk_eval_mlp_bf16: null argument");
-  ESTK_CHECK_ARG((bc_plus == nullptr) == (bc_minus == nullptr), "estk_eval_mlp_bf16: bc_plus/bc_minus must both be set or both null");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(table) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target),
-                 "estk_eval_mlp_bf16: theta/table/obs/target must be 16-byte aligned");
+// estk_eval_mlp with a tensor-core precision (estk_eval_mlp.cu has checked the arguments)
+int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = table; p.offsets = offsets; p.order = order;
-  p.pairs = pairs; p.sigma = sigma; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.ret_minus = returns_minus;
-  p.bc_plus = bc_plus; p.bc_minus = bc_minus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 2; p.centre_out = centre_return_out; p.mode = kModeBF16;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_bf16");
-}
-
-extern "C" int estk_eval_mlp_center_bf16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                         const float* obs, const float* target, int32_t B,
-                                         float* return_out, float* bc_out, int32_t bc_obs,
-                                         int32_t bc_dim, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && obs && target && return_out, "estk_eval_mlp_center_bf16: null argument");
-  EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = theta; p.offsets = nullptr; p.order = nullptr;
-  p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = return_out; p.ret_minus = nullptr;
-  p.bc_plus = bc_out; p.bc_minus = nullptr; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 1; p.mode = kModeBF16;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center_bf16");
+  p.desc = c.desc; p.theta = c.theta; p.table = c.table; p.theta16 = c.theta16; p.table16 = c.table16;
+  p.offsets = c.offsets; p.order = c.order;
+  p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.target = c.target; p.B = c.B;
+  p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
+  p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
+  p.n_signs = c.offsets ? 2 : 1; p.centre_out = c.centre_out; p.mode = mode_of(c.precision);
+  return run_tc(ctx, p, stream, "estk_eval_mlp");
 }
 
 __global__ void __launch_bounds__(256) shadow_bf16_kernel(const float4* __restrict__ src, uint2* __restrict__ dst, int64_t n4) {
@@ -673,43 +657,6 @@ extern "C" int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, 
                                                              reinterpret_cast<uint2*>(dst), n / 4);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
-}
-
-extern "C" int estk_eval_mlp_bf16s(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                   const uint16_t* theta16, const float* table, const uint16_t* table16,
-                                   const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
-                                   const float* obs, const float* target, int32_t B, float* returns_plus,
-                                   float* returns_minus, float* bc_plus, float* bc_minus, int32_t bc_obs,
-                                   int32_t bc_dim, float* centre_return_out, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && theta16 && table && table16 && offsets && obs && target &&
-                 returns_plus && returns_minus, "estk_eval_mlp_bf16s: null argument");
-  ESTK_CHECK_ARG((bc_plus == nullptr) == (bc_minus == nullptr), "estk_eval_mlp_bf16s: bc_plus/bc_minus must both be set or both null");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(table) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target) &&
-                 ESTK_ALIGNED16(theta16) && ESTK_ALIGNED16(table16),
-                 "estk_eval_mlp_bf16s: buffers must be 16-byte aligned");
-  EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = table; p.theta16 = theta16; p.table16 = table16;
-  p.offsets = offsets; p.order = order;
-  p.pairs = pairs; p.sigma = sigma; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.ret_minus = returns_minus;
-  p.bc_plus = bc_plus; p.bc_minus = bc_minus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 2; p.centre_out = centre_return_out; p.mode = kModeBF16S;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_bf16s");
-}
-
-extern "C" int estk_eval_mlp_center_bf16s(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                          const uint16_t* theta16, const float* obs, const float* target,
-                                          int32_t B, float* return_out, float* bc_out, int32_t bc_obs,
-                                          int32_t bc_dim, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && theta16 && obs && target && return_out, "estk_eval_mlp_center_bf16s: null argument");
-  EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = theta; p.theta16 = theta16; p.table16 = theta16;
-  p.offsets = nullptr; p.order = nullptr;
-  p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = return_out; p.ret_minus = nullptr;
-  p.bc_plus = bc_out; p.bc_minus = nullptr; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 1; p.mode = kModeBF16S;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center_bf16s");
 }
 
 // ---- fp16 operands from fp32 theta + the exact 16-bit noise table (the default tensor-core mode).
@@ -743,41 +690,6 @@ extern "C" int estk_shadow_f16(estk_ctx* ctx, const float* src, uint16_t* dst, i
   return ESTK_OK;
 }
 
-extern "C" int estk_eval_mlp_f16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta, const float* table,
-                                 const uint16_t* table16, const int64_t* offsets, const int32_t* order, int32_t pairs,
-                                 float sigma, const float* obs, const float* target, int32_t B, float* returns_plus,
-                                 float* returns_minus, float* bc_plus, float* bc_minus, int32_t bc_obs,
-                                 int32_t bc_dim, float* centre_return_out, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && table && table16 && offsets && obs && target && returns_plus && returns_minus,
-                 "estk_eval_mlp_f16: null argument");
-  ESTK_CHECK_ARG((bc_plus == nullptr) == (bc_minus == nullptr), "estk_eval_mlp_f16: bc_plus/bc_minus must both be set or both null");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(table) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target) &&
-                 ESTK_ALIGNED16(table16), "estk_eval_mlp_f16: buffers must be 16-byte aligned");
-  EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = table; p.table16 = table16;
-  p.offsets = offsets; p.order = order;
-  p.pairs = pairs; p.sigma = sigma; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.ret_minus = returns_minus;
-  p.bc_plus = bc_plus; p.bc_minus = bc_minus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 2; p.centre_out = centre_return_out; p.mode = kModeF16;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_f16");
-}
-
-extern "C" int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                                        const float* obs, const float* target, int32_t B, float* return_out,
-                                        float* bc_out, int32_t bc_obs, int32_t bc_dim, void* stream) {
-  ESTK_CHECK_ARG(ctx && desc && theta && obs && target && return_out, "estk_eval_mlp_center_f16: null argument");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target),
-                 "estk_eval_mlp_center_f16: buffers must be 16-byte aligned");
-  EvalTCParams p = {};
-  p.desc = *desc; p.theta = theta; p.table = theta; p.offsets = nullptr; p.order = nullptr;
-  p.pairs = 1; p.sigma = 0.f; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = return_out; p.ret_minus = nullptr;
-  p.bc_plus = bc_out; p.bc_minus = nullptr; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  p.n_signs = 1; p.mode = kModeF16;
-  return run_tc(ctx, p, (cudaStream_t)stream, "estk_eval_mlp_center_f16");
-}
-
 #ifdef ESTK_TC_PROFILE
 // Profile build only: the next evaluate launches write their per-warp buckets into `buf` (null: off);
 // reports the block's warp count and how many of them are consumers.
@@ -789,12 +701,8 @@ extern "C" ESTK_API int estk_tc_profile(void* buf, int32_t* warps, int32_t* cons
 }
 #endif
 
-extern "C" int estk_eval_mlp_f16_supported(const estk_mlp_desc* desc, int32_t B) {
+extern "C" int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B) {
   const char* why = "";
-  return desc ? tc_supported(*desc, B, &why, kModeF16) : 0;
-}
-
-extern "C" int estk_eval_mlp_bf16_supported(const estk_mlp_desc* desc, int32_t B) {
-  const char* why = "";
-  return desc ? tc_supported(*desc, B, &why, kModeBF16) : 0;
+  const int mode = mode_of(precision);
+  return desc && mode >= 0 ? tc_supported(*desc, B, &why, mode) : 0;
 }

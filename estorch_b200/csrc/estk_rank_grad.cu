@@ -62,7 +62,7 @@ struct RankGradParams {
   float* v;
   estk_state* state;
   estk_adam_desc adam;
-  // cross-GPU reduction over peer memory (estk_rank_grad_xr_adam_h): xr = world size (0: off)
+  // cross-GPU reduction over peer memory (estk_rank_grad_xr_adam): xr = world size (0: off)
   int xr, xr_rank;
   unsigned char* peer[ESTK_MAX_PEERS];   // every rank's workspace as mapped here; [xr_rank] is this GPU's own
 };
@@ -138,7 +138,7 @@ __device__ __forceinline__ void epilogue(const RankGradParams& p, const AdamScal
   }
 }
 
-// Phase X of rank_grad_kernel (estk_rank_grad_xr_adam_h): this GPU's partial gradient sum is complete in its own
+// Phase X of rank_grad_kernel (estk_rank_grad_xr_adam): this GPU's partial gradient sum is complete in its own
 // workspace; sum over the GPUs through peer memory, then apply the (replicated) Adam step.  Inlined into the XR
 // instantiations only (out of line it copied the 400-byte parameter block to local memory in every thread: 9 us).
 __device__ __forceinline__ void xr_phase(const RankGradParams& p, const AdamScalars& adam, int kThreads) {
@@ -629,13 +629,39 @@ int launch_rank_grad(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
   return ESTK_OK;
 }
 
-int check_common(estk_ctx* ctx, const float* returns, int P, const void* table,
-                 const int64_t* offsets, int64_t n, const char* who) {
-  ESTK_CHECK_ARG(ctx && returns && table && offsets, "%s: null argument", who);
+// Checks the arguments every rank + gradient launch shares and fills their fields of `p`.
+int init_common(RankGradParams& p, estk_ctx* ctx, const float* returns, const float* novelty, float w_rew,
+                float w_nov, int P, int world, const float* table, const uint16_t* table16, const int64_t* offsets,
+                const int32_t* order, int pair_begin, int pairs_local, int64_t n, int32_t* ranks_out,
+                int32_t* ranks2_out, const char* who) {
+  ESTK_CHECK_ARG(ctx && returns && offsets, "%s: null argument", who);
+  ESTK_CHECK_ARG((table == nullptr) != (table16 == nullptr), "%s: exactly one of table / table16 must be given", who);
   ESTK_CHECK_ARG(P >= 2 && (P % 2) == 0 && P <= ESTK_MAX_POPULATION,
                  "%s: population_size %d must be even, >= 2 and <= %d", who, P, ESTK_MAX_POPULATION);
   ESTK_CHECK_ARG(n > 0, "%s: n must be positive", who);
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(table), "%s: noise table must be 16-byte aligned", who);
+  ESTK_CHECK_ARG(ESTK_ALIGNED16(table ? (const void*)table : (const void*)table16),
+                 "%s: noise table must be 16-byte aligned", who);
+  ESTK_CHECK_ARG(world >= 1 && (P / 2) % world == 0, "%s: world=%d does not divide %d pairs", who, world, P / 2);
+  ESTK_CHECK_ARG(pair_begin >= 0 && pairs_local > 0 && pair_begin + pairs_local <= P / 2,
+                 "%s: local pairs [%d,+%d) outside %d", who, pair_begin, pairs_local, P / 2);
+  p = {};
+  p.returns = returns; p.novelty = novelty; p.w_rew = w_rew; p.w_nov = w_nov;
+  p.P = P; p.pairs = P / 2; p.pair_begin = pair_begin; p.pairs_local = pairs_local;
+  p.table = table; p.table16 = table16; p.world = world; p.offsets = offsets; p.order = order;
+  p.n = n; p.n4 = (n + 3) / 4;
+  p.cvals = ctx->cvals; p.partial = ctx->partial;
+  p.ranks_out = ranks_out; p.ranks2_out = ranks2_out;
+  return ESTK_OK;
+}
+
+// The in-place Adam epilogue's fields (estk_rank_grad_adam, estk_rank_grad_xr_adam).
+int init_adam(RankGradParams& p, float* theta, float* m, float* v, estk_state* state, const estk_adam_desc* adam,
+              float* grad_out, const char* who) {
+  ESTK_CHECK_ARG(theta && m && v && state && adam, "%s: null optimizer argument", who);
+  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(m) && ESTK_ALIGNED16(v) && (!grad_out || ESTK_ALIGNED16(grad_out)),
+                 "%s: theta/m/v/grad_out must be 16-byte aligned", who);
+  p.fused_adam = 1; p.grad_out = grad_out;
+  p.theta = theta; p.m = m; p.v = v; p.state = state; p.adam = *adam;
   return ESTK_OK;
 }
 
@@ -659,127 +685,56 @@ int dispatch(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
 
 }  // namespace
 
-static int rank_grad_adam_impl(estk_ctx* ctx, const float* returns, const float* novelty,
-                               float w_rew, float w_nov, int32_t P, const float* table, const uint16_t* table16,
-                               const int64_t* offsets, const int32_t* order, int64_t n,
-                               float* theta, float* m, float* v, estk_state* state,
-                               const estk_adam_desc* adam, int32_t* ranks_out,
-                               int32_t* ranks2_out, float* grad_out, void* stream) {
-  int rc = check_common(ctx, returns, P, table ? (const void*)table : (const void*)table16, offsets, n, "estk_rank_grad_adam");
-  if (rc) return rc;
-  ESTK_CHECK_ARG(theta && m && v && state && adam, "estk_rank_grad_adam: null optimizer argument");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(m) && ESTK_ALIGNED16(v) &&
-                 (!grad_out || ESTK_ALIGNED16(grad_out)),
-                 "estk_rank_grad_adam: theta/m/v/grad_out must be 16-byte aligned");
-  RankGradParams p = {};
-  p.returns = returns; p.novelty = novelty; p.w_rew = w_rew; p.w_nov = w_nov;
-  p.P = P; p.pairs = P / 2; p.pair_begin = 0; p.pairs_local = P / 2;
-  p.table = table; p.table16 = table16; p.world = 1; p.offsets = offsets; p.order = order;
-  p.n = n; p.n4 = (n + 3) / 4;
-  p.cvals = ctx->cvals; p.partial = ctx->partial;
-  p.ranks_out = ranks_out; p.ranks2_out = ranks2_out;
-  p.fused_adam = 1; p.grad_out = grad_out;
-  p.theta = theta; p.m = m; p.v = v; p.state = state; p.adam = *adam;
-  return dispatch(ctx, p, (cudaStream_t)stream);
-}
-
 extern "C" int estk_rank_grad_adam(estk_ctx* ctx, const float* returns, const float* novelty,
-                                   float w_rew, float w_nov, int32_t P, const float* table,
+                                   float w_rew, float w_nov, int32_t P, const float* table, const uint16_t* table16,
                                    const int64_t* offsets, const int32_t* order, int64_t n,
                                    float* theta, float* m, float* v, estk_state* state,
                                    const estk_adam_desc* adam, int32_t* ranks_out,
                                    int32_t* ranks2_out, float* grad_out, void* stream) {
-  ESTK_CHECK_ARG(table != nullptr, "estk_rank_grad_adam: null table");
-  return rank_grad_adam_impl(ctx, returns, novelty, w_rew, w_nov, P, table, nullptr, offsets, order, n, theta, m, v,
-                             state, adam, ranks_out, ranks2_out, grad_out, stream);
-}
-
-extern "C" int estk_rank_grad_adam_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                                     float w_rew, float w_nov, int32_t P, const uint16_t* table16,
-                                     const int64_t* offsets, const int32_t* order, int64_t n,
-                                     float* theta, float* m, float* v, estk_state* state,
-                                     const estk_adam_desc* adam, int32_t* ranks_out,
-                                     int32_t* ranks2_out, float* grad_out, void* stream) {
-  ESTK_CHECK_ARG(table16 != nullptr, "estk_rank_grad_adam_h: null table16");
-  return rank_grad_adam_impl(ctx, returns, novelty, w_rew, w_nov, P, nullptr, table16, offsets, order, n, theta, m, v,
-                             state, adam, ranks_out, ranks2_out, grad_out, stream);
-}
-
-static int rank_grad_impl(estk_ctx* ctx, const float* returns, const float* novelty,
-                          float w_rew, float w_nov, int32_t P, int32_t world, const float* table, const uint16_t* table16,
-                          const int64_t* offsets, const int32_t* order, int32_t pair_begin,
-                          int32_t pairs_local, int64_t n, float* grad_sum_out,
-                          int32_t* ranks_out, int32_t* ranks2_out, void* stream) {
-  int rc = check_common(ctx, returns, P, table ? (const void*)table : (const void*)table16, offsets, n, "estk_rank_grad");
-  if (rc) return rc;
-  ESTK_CHECK_ARG(world >= 1 && (P / 2) % world == 0, "estk_rank_grad: world=%d does not divide %d pairs", world, P / 2);
-  ESTK_CHECK_ARG(grad_sum_out && ESTK_ALIGNED16(grad_sum_out), "estk_rank_grad: grad_sum_out null or unaligned");
-  ESTK_CHECK_ARG(pair_begin >= 0 && pairs_local > 0 && pair_begin + pairs_local <= P / 2,
-                 "estk_rank_grad: local pairs [%d,+%d) outside %d", pair_begin, pairs_local, P / 2);
-  RankGradParams p = {};
-  p.returns = returns; p.novelty = novelty; p.w_rew = w_rew; p.w_nov = w_nov;
-  p.P = P; p.pairs = P / 2; p.pair_begin = pair_begin; p.pairs_local = pairs_local;
-  p.table = table; p.table16 = table16; p.world = world; p.offsets = offsets; p.order = order;
-  p.n = n; p.n4 = (n + 3) / 4;
-  p.cvals = ctx->cvals; p.partial = ctx->partial;
-  p.ranks_out = ranks_out; p.ranks2_out = ranks2_out;
-  p.fused_adam = 0; p.grad_sum_out = grad_sum_out;
-  p.adam.clamp = 0.f;
-  return dispatch(ctx, p, (cudaStream_t)stream);
+  const char* who = "estk_rank_grad_adam";
+  RankGradParams p;
+  int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, 1, table, table16, offsets, order, 0, P / 2, n,
+                       ranks_out, ranks2_out, who);
+  if (!rc) rc = init_adam(p, theta, m, v, state, adam, grad_out, who);
+  return rc ? rc : dispatch(ctx, p, (cudaStream_t)stream);
 }
 
 extern "C" int estk_rank_grad(estk_ctx* ctx, const float* returns, const float* novelty,
-                              float w_rew, float w_nov, int32_t P, const float* table,
-                              const int64_t* offsets, const int32_t* order, int32_t pair_begin,
-                              int32_t pairs_local, int64_t n, float* grad_sum_out,
+                              float w_rew, float w_nov, int32_t P, int32_t world, const float* table,
+                              const uint16_t* table16, const int64_t* offsets, const int32_t* order,
+                              int32_t pair_begin, int32_t pairs_local, int64_t n, float* grad_sum_out,
                               int32_t* ranks_out, int32_t* ranks2_out, void* stream) {
-  ESTK_CHECK_ARG(table != nullptr, "estk_rank_grad: null table");
-  return rank_grad_impl(ctx, returns, novelty, w_rew, w_nov, P, 1, table, nullptr, offsets, order, pair_begin,
-                        pairs_local, n, grad_sum_out, ranks_out, ranks2_out, stream);
-}
-
-extern "C" int estk_rank_grad_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                                float w_rew, float w_nov, int32_t P, int32_t world, const uint16_t* table16,
-                                const int64_t* offsets, const int32_t* order, int32_t pair_begin,
-                                int32_t pairs_local, int64_t n, float* grad_sum_out,
-                                int32_t* ranks_out, int32_t* ranks2_out, void* stream) {
-  ESTK_CHECK_ARG(table16 != nullptr, "estk_rank_grad_h: null table16");
-  return rank_grad_impl(ctx, returns, novelty, w_rew, w_nov, P, world, nullptr, table16, offsets, order, pair_begin,
-                        pairs_local, n, grad_sum_out, ranks_out, ranks2_out, stream);
+  RankGradParams p;
+  const int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, world, table, table16, offsets, order,
+                             pair_begin, pairs_local, n, ranks_out, ranks2_out, "estk_rank_grad");
+  if (rc) return rc;
+  ESTK_CHECK_ARG(grad_sum_out && ESTK_ALIGNED16(grad_sum_out), "estk_rank_grad: grad_sum_out null or unaligned");
+  p.fused_adam = 0; p.grad_sum_out = grad_sum_out;
+  return dispatch(ctx, p, (cudaStream_t)stream);
 }
 
 extern "C" int64_t estk_xr_workspace_bytes(int64_t n) { return n > 0 ? kXrDataOff + 2 * xr_image_bytes(n) : 0; }
 
-extern "C" int estk_rank_grad_xr_adam_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                                        float w_rew, float w_nov, int32_t P, int32_t world, int32_t rank,
-                                        const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                                        int32_t pair_begin, int32_t pairs_local, int64_t n,
-                                        void* const* peer_ws, float* theta, float* m, float* v,
-                                        estk_state* state, const estk_adam_desc* adam,
-                                        int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream) {
-  ESTK_CHECK_ARG(table16 != nullptr, "estk_rank_grad_xr_adam_h: null table16");
-  int rc = check_common(ctx, returns, P, table16, offsets, n, "estk_rank_grad_xr_adam_h");
-  if (rc) return rc;
+extern "C" int estk_rank_grad_xr_adam(estk_ctx* ctx, const float* returns, const float* novelty,
+                                      float w_rew, float w_nov, int32_t P, int32_t world, int32_t rank,
+                                      const uint16_t* table16, const int64_t* offsets, const int32_t* order,
+                                      int32_t pair_begin, int32_t pairs_local, int64_t n,
+                                      void* const* peer_ws, float* theta, float* m, float* v,
+                                      estk_state* state, const estk_adam_desc* adam,
+                                      int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream) {
+  const char* who = "estk_rank_grad_xr_adam";
+  ESTK_CHECK_ARG(table16 != nullptr, "%s: null table16", who);
   ESTK_CHECK_ARG(world >= 2 && world <= ESTK_MAX_PEERS && rank >= 0 && rank < world,
-                 "estk_rank_grad_xr_adam_h: world=%d rank=%d (2 <= world <= %d)", world, rank, ESTK_MAX_PEERS);
-  ESTK_CHECK_ARG((P / 2) % world == 0, "estk_rank_grad_xr_adam_h: world=%d does not divide %d pairs", world, P / 2);
-  ESTK_CHECK_ARG(pair_begin >= 0 && pairs_local > 0 && pair_begin + pairs_local <= P / 2,
-                 "estk_rank_grad_xr_adam_h: local pairs [%d,+%d) outside %d", pair_begin, pairs_local, P / 2);
-  ESTK_CHECK_ARG(theta && m && v && state && adam && peer_ws, "estk_rank_grad_xr_adam_h: null argument");
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(m) && ESTK_ALIGNED16(v) && (!grad_out || ESTK_ALIGNED16(grad_out)),
-                 "estk_rank_grad_xr_adam_h: theta/m/v/grad_out must be 16-byte aligned");
-  RankGradParams p = {};
-  p.returns = returns; p.novelty = novelty; p.w_rew = w_rew; p.w_nov = w_nov;
-  p.P = P; p.pairs = P / 2; p.pair_begin = pair_begin; p.pairs_local = pairs_local;
-  p.table = nullptr; p.table16 = table16; p.world = world; p.offsets = offsets; p.order = order;
-  p.n = n; p.n4 = (n + 3) / 4;
-  p.cvals = ctx->cvals; p.partial = ctx->partial;
-  p.ranks_out = ranks_out; p.ranks2_out = ranks2_out;
-  p.fused_adam = 1; p.grad_out = grad_out;
-  p.theta = theta; p.m = m; p.v = v; p.state = state; p.adam = *adam;
+                 "%s: world=%d rank=%d (2 <= world <= %d)", who, world, rank, ESTK_MAX_PEERS);
+  ESTK_CHECK_ARG(peer_ws != nullptr, "%s: null peer_ws", who);
+  RankGradParams p;
+  int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, world, nullptr, table16, offsets, order,
+                       pair_begin, pairs_local, n, ranks_out, ranks2_out, who);
+  if (!rc) rc = init_adam(p, theta, m, v, state, adam, grad_out, who);
+  if (rc) return rc;
   p.xr = world; p.xr_rank = rank;
   for (int q = 0; q < world; ++q) {
-    ESTK_CHECK_ARG(peer_ws[q] && ESTK_ALIGNED16(peer_ws[q]), "estk_rank_grad_xr_adam_h: peer workspace %d null or unaligned", q);
+    ESTK_CHECK_ARG(peer_ws[q] && ESTK_ALIGNED16(peer_ws[q]), "%s: peer workspace %d null or unaligned", who, q);
     p.peer[q] = static_cast<unsigned char*>(peer_ws[q]);
   }
   p.grad_sum_out = reinterpret_cast<float*>(p.peer[rank] + kXrDataOff);   // this rank's partial sum

@@ -11,7 +11,7 @@ the body of a generation runs on the GPU through the C ABI in include/estk.h:
     _calculate_returns :195-202 (python loop)    estk_eval_mlp (fused) | host rollouts (plumbing)
     rank_transformation + torch.mm :174-179      estk_rank_grad[_adam] (+ one NCCL all-reduce)
     grad scatter/clamp :236-244, Adam.step :245  fused Adam epilogue (or torch optimizer.step)
-    _after_optimize :181-185                     estk_eval_mlp_center + estk_track_best
+    _after_optimize :181-185                     estk_eval_mlp (centre, offsets NULL) + estk_track_best
 
 Two execution modes, chosen per instance:
 
@@ -650,7 +650,7 @@ class ES:
 
     # -- rank-major returns: every rank's evaluate kernel writes its (+, -) halves straight into its
     #    block of a [W, 2, pairs/W] buffer, ONE in-place all-gather completes it, and the rank kernel
-    #    (estk_rank_grad_h, `world`) reads that layout: no staging copies (estorch.py:228-233 Recv loop)
+    #    (estk_rank_grad, `world`) reads that layout: no staging copies (estorch.py:228-233 Recv loop)
     def _member_order(self, t_rm):
         return t_rm.view(self.n_workers, 2, self._pairs_local).permute(1, 0, 2).reshape(-1)
 
@@ -667,7 +667,7 @@ class ES:
 
     def _peer_workspaces(self):
         """Device pointers of every rank's cross-GPU workspace as mapped in this process (``estk.h``:
-        estk_rank_grad_xr_adam_h sums the partial gradients over NVLink peer memory inside the kernel), or
+        estk_rank_grad_xr_adam sums the partial gradients over NVLink peer memory inside the kernel), or
         None when peer memory is not available -- then the NCCL all-reduce path runs.  Set up once, at the
         first fused generation, collectively: every rank takes the same decision."""
         if "_peer_ptrs" in self.__dict__:
@@ -820,14 +820,52 @@ class ES:
             self._obs.copy_(obs, non_blocking=True)
             self._tgt.copy_(tgt, non_blocking=True)
 
+    def _update_step(self, slot, R, N, w_rew, w_nov, rm):
+        """Ranks, gradient estimate and Adam step of a fused generation from the returns ``R`` (and the
+        novelty ``N``, None for ES) -- rank-major ``[W, 2, pairs/W]`` buffers when ``rm``, member order
+        otherwise.  One GPU: one launch.  Several: the rows are all-gathered, then ONE launch that also
+        sums the gradient over NVLink peer memory, or, without peer memory, rank + partial gradient ->
+        NCCL all-reduce -> clamp + Adam."""
+        be, P, W, pb, pl = self._be, self.population_size, self.n_workers, self._pair_begin, self._pairs_local
+        gt, ad = self._grad_table(), self._adam_desc(slot.optimizer)
+        ranks2 = None if N is None else self._ranks2
+        _nvtx_push("estk:rank_grad_adam")
+        if W == 1:
+            be.rank_grad_adam(R, N, w_rew, w_nov, P, gt, self._offsets, self._order,
+                              slot.theta, slot.m, slot.v, slot.state, ad, self._ranks, ranks2, self._grad)
+        else:
+            peers = self._peer_workspaces() if rm else None
+            gather = self._all_gather_rm if rm else self._all_gather_halves
+            for t in ([R] if N is None else [R, N]):
+                gather(t)
+            nov = None if N is None else N.view(-1)
+            if peers is not None:
+                be.rank_grad_xr_adam(R.view(-1), nov, w_rew, w_nov, P, W, self.rank, gt, self._offsets, self._order,
+                                     pb, pl, peers, slot.theta, slot.m, slot.v, slot.state, ad, self._ranks, ranks2,
+                                     self._grad)
+            else:
+                be.rank_grad(R.view(-1), nov, w_rew, w_nov, P, gt, self._offsets, self._order, pb, pl,
+                             self.n_parameters, self._grad, self._ranks, ranks2, world=W if rm else 1)
+                self._all_reduce(self._grad)
+                be.clamp_adam(self._grad, P, slot.theta, slot.m, slot.v, slot.state, ad, None)
+        _nvtx_pop()
+
+    def _defers_centre(self):
+        """Whether this generation's post-update rollout (estorch.py:181-185) is deferred and folded into the
+        next generation's evaluate launch: it is a single 30 us task, so it waits when nobody can observe it
+        before then (no log() due, not the last generation, the observation batch does not change).  Only
+        the tensor-core MLP evaluate can carry it."""
+        return (self._precision in ("f16", "bf16", "bf16s") and not self._is_conv and not self._stop
+                and not self._streaming
+                and (self.step + 1) % self._log_interval != 0 and self.step + 1 < self.n_steps)
+
     def _fused_generation(self, slot):
         """One generation, entirely on the device (no host synchronisation).  The body only
         enqueues work whose arguments do not depend on host scalars that change from one
         generation to the next (the generation index and the Adam step live in
         ``estk_state``), so it can be captured once and replayed as a CUDA graph
         (``_graphed_generation``)."""
-        be, P, pairs, pl, pb, W = self._be, self.population_size, self._pairs, self._pairs_local, self._pair_begin, \
-            self.n_workers
+        be, pairs, pl, pb, W = self._be, self._pairs, self._pairs_local, self._pair_begin, self.n_workers
         dims = None if self._is_conv else self._spec.dims
         self._upload_batch()
         slot.theta_prev.copy_(slot.theta)
@@ -857,37 +895,9 @@ class ES:
                 be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
                 self._pending_centre = False
         _nvtx_pop()
-        _nvtx_push("estk:rank_grad_adam")
-        ad = self._adam_desc(slot.optimizer)
-        if W == 1:
-            be.rank_grad_adam(R, None, 1.0, 0.0, P, gt, self._offsets, self._order,
-                              slot.theta, slot.m, slot.v, slot.state, ad, self._ranks, None, self._grad)
-        else:
-            peers = self._peer_workspaces() if rm else None
-            if peers is not None:
-                # ONE launch: ranks, partial gradient, sum over the GPUs through NVLink peer memory, Adam
-                self._all_gather_rm(R)
-                be.rank_grad_xr_adam(R.view(-1), None, 1.0, 0.0, P, W, self.rank, gt, self._offsets, self._order,
-                                     pb, pl, peers, slot.theta, slot.m, slot.v, slot.state, ad, self._ranks, None,
-                                     self._grad)
-            else:
-                if rm:
-                    self._all_gather_rm(R)
-                else:
-                    self._all_gather_halves(R)
-                be.rank_grad(R.view(-1), None, 1.0, 0.0, P, gt, self._offsets, self._order, pb, pl,
-                             self.n_parameters, self._grad, self._ranks, None, world=W if rm else 1)
-                self._all_reduce(self._grad)
-                be.clamp_adam(self._grad, P, slot.theta, slot.m, slot.v, slot.state, ad, None)
-        _nvtx_pop()
+        self._update_step(slot, R, None, 1.0, 0.0, rm)
         self._best_slot = slot
-        # post-update rollout (estorch.py:181-185).  It is a single 30 us task, so when nobody
-        # can observe it before the next generation (no log() due, not the last generation, the
-        # observation batch does not change) it is deferred and folded into the next generation's
-        # evaluate launch.
-        if (self._precision in ("f16", "bf16", "bf16s") and not self._is_conv and not self._stop
-                and not self._streaming
-                and (self.step + 1) % self._log_interval != 0 and self.step + 1 < self.n_steps):
+        if self._defers_centre():
             self._pending_centre = True
             return
         if self._is_conv:
@@ -904,11 +914,8 @@ class ES:
                 or getattr(self, "_graph_broken", False) or type(self)._fused_generation is not ES._fused_generation):
             return None
         g = slot.optimizer.param_groups[0]
-        will_defer = (self._precision in ("f16", "bf16", "bf16s") and not self._is_conv and not self._stop
-                      and not self._streaming
-                      and (self.step + 1) % self._log_interval != 0 and self.step + 1 < self.n_steps)
         nb = self._next_batch_ptrs
-        return (id(slot), bool(self._pending_centre), will_defer, float(g["lr"]), tuple(g["betas"]), float(g["eps"]),
+        return (id(slot), bool(self._pending_centre), self._defers_centre(), float(g["lr"]), tuple(g["betas"]), float(g["eps"]),
                 float(g["weight_decay"]), float(self.sigma), self._table._version, nb,
                 self._obs.data_ptr(), self._tgt.data_ptr(), torch.cuda.current_stream(self._dev).cuda_stream)
 
@@ -1370,8 +1377,7 @@ class NS_ES(ES):
         return self._slots[self.idx]
 
     def _fused_generation(self, slot):
-        be, P, pairs, pl, pb, W = self._be, self.population_size, self._pairs, self._pairs_local, self._pair_begin, \
-            self.n_workers
+        be, pairs, pl, pb, W = self._be, self._pairs, self._pairs_local, self._pair_begin, self.n_workers
         dims, ag = self._spec.dims, self.agent
         self._upload_batch()
         slot.theta_prev.copy_(slot.theta)
@@ -1393,30 +1399,7 @@ class NS_ES(ES):
                     **self._mlp_kw(slot))
         be.knn_novelty(BC[pb: pb + pl], self._arch_dev, self.k, nov_p)
         be.knn_novelty(BC[pairs + pb: pairs + pb + pl], self._arch_dev, self.k, nov_m)
-        ad = self._adam_desc(slot.optimizer)
-        w_rew, w_nov = np.float32(self._w_rew()), np.float32(self._w_nov())
-        if W == 1:
-            be.rank_grad_adam(R, N, w_rew, w_nov, P, gt, self._offsets, self._order,
-                              slot.theta, slot.m, slot.v, slot.state, ad, self._ranks, self._ranks2, self._grad)
-        else:
-            peers = self._peer_workspaces() if rm else None
-            if peers is not None:
-                self._all_gather_rm(R)
-                self._all_gather_rm(N)
-                be.rank_grad_xr_adam(R.view(-1), N.view(-1), w_rew, w_nov, P, W, self.rank, gt, self._offsets,
-                                     self._order, pb, pl, peers, slot.theta, slot.m, slot.v, slot.state, ad,
-                                     self._ranks, self._ranks2, self._grad)
-            else:
-                if rm:
-                    self._all_gather_rm(R)
-                    self._all_gather_rm(N)
-                else:
-                    self._all_gather_halves(R)
-                    self._all_gather_halves(N)
-                be.rank_grad(R.view(-1), N.view(-1), w_rew, w_nov, P, gt, self._offsets, self._order, pb, pl,
-                             self.n_parameters, self._grad, self._ranks, self._ranks2, world=W if rm else 1)
-                self._all_reduce(self._grad)
-                be.clamp_adam(self._grad, P, slot.theta, slot.m, slot.v, slot.state, ad, None)
+        self._update_step(slot, R, N, np.float32(self._w_rew()), np.float32(self._w_nov()), rm)
         # _after_optimize (estorch.py:427-432 / :650-662): rollout of the updated
         # policy, archive append, best tracking, NSRA schedule (host scalars)
         be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, self._bc_center[0],

@@ -38,7 +38,7 @@ extern "C" {
 #define ESTK_API
 #endif
 
-#define ESTK_VERSION 100          /* 0.1.0 */
+#define ESTK_VERSION 200          /* 0.2.0 */
 #define ESTK_MAX_LAYERS 8
 #define ESTK_MAX_POPULATION 32768 /* P; rank phase is O(P^2) */
 
@@ -75,7 +75,8 @@ typedef struct {
  *   bits 8-15  output activation, applied after the last Linear, before the squared
  *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y).
  * 0 is ReLU hidden + identity output.  Any other value is ESTK_ERR_INVALID in
- * estk_eval_mlp* and makes estk_eval_mlp_{f16,bf16}_supported return 0.
+ * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
+ * and makes estk_eval_mlp_supported return 0.
  * Arithmetic of tanh: IEEE tanhf (libdevice, ~1-2 ulp, no tanh.approx) on the fp32
  * value acc + bias.  fp32 path: the result stays fp32.  Tensor-core paths: a hidden
  * tanh is rounded ONCE to the 16-bit operand type when the activation is written back
@@ -83,6 +84,13 @@ typedef struct {
 #define ESTK_ACT_RELU 0
 #define ESTK_ACT_TANH 1
 #define ESTK_ACT_OUT_TANH (1 << 8)
+
+/* Arithmetic of the evaluate kernels (estk_eval_mlp, estk_eval_conv_vbn); what each one
+ * computes is stated at those functions. */
+#define ESTK_PREC_FP32 0   /* CUDA cores, exact fp32 */
+#define ESTK_PREC_F16 1    /* tensor cores, fp16 operands formed from fp32 sums (the default) */
+#define ESTK_PREC_BF16 2   /* tensor cores, bf16 operands (opt-in, lower precision) */
+#define ESTK_PREC_BF16S 3  /* tensor cores, bf16 operands from bf16 shadows (opt-in, lower precision) */
 typedef struct {
   int32_t n_layers;                  /* number of Linear layers, 1..ESTK_MAX_LAYERS */
   int32_t dims[ESTK_MAX_LAYERS + 1]; /* dims[0] = obs dim, dims[n_layers] = out dim */
@@ -133,135 +141,116 @@ ESTK_API int estk_perturb_rows(estk_ctx* ctx, const float* theta, int64_t n, con
                       int32_t member_begin, int32_t member_count,
                       float* rows_out, float* eps_out, void* stream);
 
+/* ---- 16-bit copies for the tensor-core evaluate ---- */
+
+/* dst[i] = rn_f16(src[i]); inexact_count (device, nullable) += the number of entries that
+ * changed.  A table made by estk_fill_noise_table comes back with 0: its fp16 copy is then
+ * EXACT (every consumer converts it back to the very fp32 value the table holds), which is
+ * what ESTK_PREC_F16 and the fp16-table form of estk_rank_grad* require.
+ * n % 4 == 0; src 16-byte, dst 8-byte aligned. */
+ESTK_API int estk_shadow_f16(estk_ctx* ctx, const float* src, uint16_t* dst, int64_t n,
+                    uint64_t* inexact_count, void* stream);
+/* dst[i] = rn_bf16(src[i]): the bf16 SHADOWS of theta and of the table that ESTK_PREC_BF16S
+ * reads.  Same shape and alignment rules as estk_shadow_f16. */
+ESTK_API int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, int64_t n, void* stream);
+
 /* ---- kernel 1: population evaluate (estorch.py:195-202 `_calculate_returns`
  *      + Policy.forward examples/cartpole_es.py:14-20 + the synthetic agent
  *      return -mean((policy(obs)-target)^2), SURVEY 8d) ---- */
 
-/* For each local pair j: returns_plus[j] / returns_minus[j] = return of
- * theta +/- sigma*T[offsets[j]].  obs [B, dims[0]], target [B, dims[L]] fp32
- * row-major.  bc_plus/bc_minus (nullable) [pairs, bc_dim] receive the behaviour
- * characteristic policy(obs[:bc_obs]).flatten()[:bc_dim] (examples/nsra_es.py:45-49).
- * order (nullable) = evaluation order from estk_make_offsets. */
-ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                  const float* table, const int64_t* offsets, const int32_t* order,
-                  int32_t pairs, float sigma, const float* obs, const float* target, int32_t B,
+/* MLP policy `desc` over the observation batch obs [B, dims[0]], target [B, dims[L]] (fp32,
+ * row-major).
+ *
+ * Population (offsets != NULL): for each local pair j, returns_plus[j] / returns_minus[j] =
+ * return of theta +/- sigma*T[offsets[j]].  order (nullable) = evaluation order from
+ * estk_make_offsets.  bc_plus / bc_minus (both or neither) [pairs, bc_dim] receive the
+ * behaviour characteristic policy(obs[:bc_obs]).flatten()[:bc_dim] (examples/nsra_es.py:45-49).
+ * centre_return_out (nullable; tensor-core precisions only, ESTK_ERR_UNSUPPORTED with FP32):
+ * additionally evaluate theta itself (sigma = 0) in the same launch and write its return there
+ * -- the estorch.py:182 rollout of the previous update folded into this generation's launch.
+ *
+ * Centre (offsets == NULL; the estorch.py:181-182 `_after_optimize` rollout): returns_plus[0] =
+ * return of theta, bc_plus (nullable) [bc_dim] its behaviour characteristic.  table, table16,
+ * order, pairs, sigma, returns_minus and bc_minus are not read; centre_return_out must be NULL.
+ *
+ * bc_obs and bc_dim must be positive when behaviour-characteristic outputs are given.
+ *
+ * precision -- the arithmetic, and the buffers it needs besides theta / obs / target / returns:
+ *   ESTK_PREC_FP32   CUDA cores, exact fp32 with the reference's two roundings (eps = sigma*t,
+ *                    then theta +- eps).  Population: table.  Any widths that fit in shared memory.
+ *   ESTK_PREC_F16    the default: wgmma with fp16 operands (11-bit significand, the TF32 class)
+ *                    and fp32 accumulation.  Every weight is formed in fp32 from the fp32 theta
+ *                    and the noise value and rounded ONCE: W16 = rn_f16(theta + s*sigma*T[off+i])
+ *                    (sum in fp32, like estorch.py:192).  The noise is read from table16, the EXACT
+ *                    fp16 copy of `table` (estk_shadow_f16 with inexact_count 0), so the kernel
+ *                    evaluates exactly the members the gradient estimate (estk_rank_grad*) weights.
+ *                    Hidden activations are rounded to fp16 when written back (saturating at
+ *                    +-65504), the observations enter as x_hi + x_lo (two fp16 operands), biases and
+ *                    the squared error are fp32.  Population: table, table16.
+ *   ESTK_PREC_BF16   opt-in, lower precision: wgmma with bf16 operands, fp32 accumulation; weights
+ *                    are rounded to bf16 when the B-operand tile is formed, activations when they
+ *                    are written back.  Returns agree with FP32 to ~1e-2 relative.  Population: table.
+ *   ESTK_PREC_BF16S  opt-in, lower precision: as BF16, but the weights are formed from bf16
+ *                    SHADOWS (estk_shadow_bf16): W = bf16(theta16 + s*sigma*table16[off+i]), half the
+ *                    bytes per weight element; biases still come from the fp32 theta / table.
+ *                    NOTE: it evaluates F(theta16 +- sigma16*eps16) while estk_rank_grad* weights
+ *                    the fp32 eps -- the estimator multiplies a return by a noise vector that is
+ *                    not exactly the one that produced it (estorch.py:177-178 uses the same eps on
+ *                    both sides); F16 has no such departure.  Always: theta16.  Population: table,
+ *                    table16 (the bf16 shadow of the table).
+ *   Buffers a precision does not list are not read.
+ * Tensor-core precisions (F16, BF16, BF16S): theta, obs, target and the listed table / table16 /
+ * theta16 must be 16-byte aligned.  Every layer input width a multiple of 64 in [64,512], every
+ * output width a multiple of 32 in [32,512], B a multiple of 256, and for F16 dims[0] <= 256;
+ * other shapes are ESTK_ERR_UNSUPPORTED (estk_eval_mlp_supported tells in advance).
+ * Agreement with FP32 is asserted in tests/test_kernels_gpu.py and tests/test_eval_mlp_act_gpu.py. */
+ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t precision,
+                  const float* theta, const uint16_t* theta16,
+                  const float* table, const uint16_t* table16,
+                  const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
+                  const float* obs, const float* target, int32_t B,
                   float* returns_plus, float* returns_minus,
                   float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
-                  void* stream);
+                  float* centre_return_out, void* stream);
 
-/* Opt-in lower-precision tensor-core variant of estk_eval_mlp: same contract, bf16 operands with fp32
- * accumulation on wgmma (weights theta+-sigma*eps are rounded to bf16 when the
- * B-operand tile is formed, activations when they are written back).  Shapes:
- * every layer input width a multiple of 64 in [64,512], every output width a
- * multiple of 32 in [32,512], B a multiple of 256; otherwise
- * ESTK_ERR_UNSUPPORTED (estk_eval_mlp_bf16_supported() tells in advance).
- * Returns agree with the fp32 path to ~1e-2 relative (stated in the tests).
- * centre_return_out (nullable): additionally evaluate theta itself (sigma = 0) in
- * the same launch and write its return there -- the estorch.py:182 rollout of the
- * previous update folded into this generation's launch. */
-ESTK_API int estk_eval_mlp_bf16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                       const float* table, const int64_t* offsets, const int32_t* order,
-                       int32_t pairs, float sigma, const float* obs, const float* target, int32_t B,
-                       float* returns_plus, float* returns_minus,
-                       float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
-                       float* centre_return_out, void* stream);
-ESTK_API int estk_eval_mlp_center_bf16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                              const float* obs, const float* target, int32_t B,
-                              float* return_out, float* bc_out, int32_t bc_obs, int32_t bc_dim,
-                              void* stream);
-ESTK_API int estk_eval_mlp_bf16_supported(const estk_mlp_desc* desc, int32_t B);
-
-/* DEFAULT tensor-core evaluate ("f16"): same contract as estk_eval_mlp, computed on
- * wgmma with fp16 operands (11-bit significand, the TF32 class) and fp32 accumulation.
- * Every weight is formed in fp32 from the fp32 theta and the noise value and rounded ONCE:
- *   W16 = rn_f16(theta + s*sigma*T[off+i])      (sum in fp32, like estorch.py:192)
- * The noise is streamed from table16, a 16-bit copy of `table` that must be EXACT
- * (table16[i] == table[i] for all i: build it with estk_shadow_f16, whose inexact_count
- * must come back 0 -- true for tables made by estk_fill_noise_table); the kernel
- * therefore evaluates exactly the members the gradient estimate (estk_rank_grad*, fp32
- * table) weights.  Hidden activations are rounded to fp16 when written back (saturating
- * at +-65504), the observations enter as x_hi + x_lo (two fp16 operands), biases and the
- * squared error are fp32.  Shapes as estk_eval_mlp_bf16, plus dims[0] <= 256
- * (estk_eval_mlp_f16_supported()).  Agreement with the fp32 path: asserted in
- * tests/test_kernels_gpu.py::test_eval_mlp_f16_*. */
-ESTK_API int estk_shadow_f16(estk_ctx* ctx, const float* src, uint16_t* dst, int64_t n,
-                    uint64_t* inexact_count /* device, nullable: += #entries that changed */,
-                    void* stream);
-ESTK_API int estk_eval_mlp_f16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                      const float* table, const uint16_t* table16,
-                      const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
-                      const float* obs, const float* target, int32_t B,
-                      float* returns_plus, float* returns_minus,
-                      float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
-                      float* centre_return_out, void* stream);
-ESTK_API int estk_eval_mlp_center_f16(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                             const float* obs, const float* target, int32_t B,
-                             float* return_out, float* bc_out, int32_t bc_obs, int32_t bc_dim,
-                             void* stream);
-ESTK_API int estk_eval_mlp_f16_supported(const estk_mlp_desc* desc, int32_t B);
-
-/* NOTE on "bf16s": it evaluates F(theta16 +- sigma16 * eps16) while estk_rank_grad* weights the fp32 eps --
- * the estimator multiplies a return by a noise vector that is not exactly the one that produced it
- * (estorch.py:177-178 uses the same eps on both sides).  The default mode ("f16") has no such
- * departure.
- * "bf16s" (opt-in, lower precision): as estk_eval_mlp_bf16, but the weight producers read bf16 SHADOWS of
- * theta and of the noise table (theta16[i] = bf16(theta[i]), table16[i] =
- * bf16(table[i]), built with estk_shadow_bf16) -- half the bytes per weight
- * element, W = bf16(theta16 + s*sigma*table16[off+i]).  Biases still come from the
- * fp32 theta / table.  The gradient estimate (estk_rank_grad*) always uses the
- * fp32 table.  Tolerance vs the fp32 path is stated in tests/test_kernels_gpu.py. */
-ESTK_API int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, int64_t n, void* stream);
-ESTK_API int estk_eval_mlp_bf16s(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                        const uint16_t* theta16, const float* table, const uint16_t* table16,
-                        const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
-                        const float* obs, const float* target, int32_t B,
-                        float* returns_plus, float* returns_minus,
-                        float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
-                        float* centre_return_out, void* stream);
-ESTK_API int estk_eval_mlp_center_bf16s(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                               const uint16_t* theta16, const float* obs, const float* target, int32_t B,
-                               float* return_out, float* bc_out, int32_t bc_obs, int32_t bc_dim,
-                               void* stream);
+/* 1 when the tensor-core `precision` (F16, BF16 or BF16S) can evaluate `desc` at batch B (the
+ * shape rules above, and a defined activation code), else 0 -- also for a null desc and for any
+ * other precision code. */
+ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B);
 
 /* ---- conv + VirtualBatchNorm policy of examples/atari.py:14-37 (BASELINE config 5):
  * conv1 4->16 k8 s4, VBN(16), ReLU, conv2 16->32 k4 s2, VBN(32), ReLU, fc1 2592->256,
  * ReLU, fc2 256->n_actions; VBN statistics = per-(C,H,W) mean / unbiased variance of
  * the reference batch xref [ref_batch,4,84,84] under the member's own weights
  * (estorch/modules.py:48-58).  obs [B,4,84,84], target [B,n_actions]; return =
- * -mean((policy(obs)-target)^2).  offsets == NULL evaluates theta itself into
- * returns_plus[0].  scratch: caller-owned device slab of at least
- * estk_eval_conv_vbn_scratch_bytes(ctx, ref_batch, B) bytes.  fp32 throughout. */
-ESTK_API int64_t estk_eval_conv_vbn_scratch_bytes(estk_ctx* ctx, int32_t ref_batch, int32_t B);
-ESTK_API int estk_eval_conv_vbn(estk_ctx* ctx, int32_t n_actions, const float* theta, const float* table,
+ * -mean((policy(obs)-target)^2).
+ *
+ * Population (offsets != NULL): returns_plus[j] / returns_minus[j] = return of
+ * theta +/- sigma*T[offsets[j]] (j = order[slot] when order is given).  Centre (offsets == NULL):
+ * returns_plus[0] = return of theta; table, table16, order and returns_minus are not read.
+ * scratch: caller-owned device slab of at least as many bytes as estk_eval_conv_vbn_scratch_bytes
+ * returns for the same precision, ref_batch and B (it returns -1 for bad arguments or a precision
+ * without a conv kernel).  Shapes: ref_batch >= 2 (unbiased variance), B >= 1, 1 <= n_actions <= 64; xref and
+ * obs 16-byte aligned.
+ *
+ * precision:
+ *   ESTK_PREC_FP32  fp32 throughout.  Population: table.
+ *   ESTK_PREC_F16   conv1, conv2 and fc1 on mma.sync with fp16 operands and fp32 accumulation;
+ *                   every operand -- the weights theta + s*sigma*T[off+i] (formed in fp32 from the
+ *                   fp32 theta and table16, the EXACT fp16 copy of `table` made by estk_shadow_f16),
+ *                   the input frames and the normalised activations -- enters as hi + lo, two fp16
+ *                   values (22 significant bits), so the returns stay within 1e-5 (max-norm
+ *                   relative) of the fp32 forward.  VBN statistics, normalisation, biases, fc2 and
+ *                   the loss are fp32; no atomics, so the returns are the same bits run to run.
+ *                   Population: table, table16.  theta, scratch and table16 16-byte aligned.
+ *   any other       ESTK_ERR_UNSUPPORTED. */
+ESTK_API int64_t estk_eval_conv_vbn_scratch_bytes(estk_ctx* ctx, int32_t precision, int32_t ref_batch, int32_t B);
+ESTK_API int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_actions, const float* theta,
+                       const float* table, const uint16_t* table16,
                        const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
                        const float* xref, int32_t ref_batch, const float* obs, const float* target,
                        int32_t B, float* returns_plus, float* returns_minus, void* scratch,
                        int64_t scratch_bytes, void* stream);
-
-/* Opt-in tensor-core variant of estk_eval_conv_vbn ("f16"): same policy, arguments, return
- * placement (returns_plus[j] / returns_minus[j], j = order[slot] when order is given) and
- * offsets == NULL centre evaluation.  conv1, conv2 and fc1 run on mma.sync with fp16 operands
- * and fp32 accumulation; every operand -- the weights theta + s*sigma*T[off+i] (formed in fp32
- * from the fp32 theta and table16, the EXACT fp16 copy of `table` made by estk_shadow_f16),
- * the input frames and the normalised activations -- enters as hi + lo, two fp16 values
- * (22 significant bits), so the returns stay within 1e-5 (max-norm relative) of the fp32
- * forward.  VBN statistics, normalisation, biases, fc2 and the loss are fp32; no atomics, so
- * the returns are the same bits run to run.  table and table16 are required with offsets.
- * scratch: at least estk_eval_conv_vbn_f16_scratch_bytes(ctx, ref_batch, B) bytes, 16-byte
- * aligned.  Shapes: everything estk_eval_conv_vbn accepts. */
-ESTK_API int64_t estk_eval_conv_vbn_f16_scratch_bytes(estk_ctx* ctx, int32_t ref_batch, int32_t B);
-ESTK_API int estk_eval_conv_vbn_f16(estk_ctx* ctx, int32_t n_actions, const float* theta, const float* table,
-                           const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                           int32_t pairs, float sigma, const float* xref, int32_t ref_batch,
-                           const float* obs, const float* target, int32_t B, float* returns_plus,
-                           float* returns_minus, void* scratch, int64_t scratch_bytes, void* stream);
-
-/* Unperturbed policy (estorch.py:181-182 `_after_optimize` rollout):
- * return_out[0] = return of theta; bc_out (nullable) [bc_dim]. */
-ESTK_API int estk_eval_mlp_center(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta,
-                         const float* obs, const float* target, int32_t B,
-                         float* return_out, float* bc_out, int32_t bc_obs, int32_t bc_dim,
-                         void* stream);
 
 /* estorch.py:182-185: episode_reward = *reward; if it beats state->best_reward,
  * take it and copy theta -> best_theta (the device analogue of
@@ -272,60 +261,56 @@ ESTK_API int estk_track_best(estk_ctx* ctx, estk_state* state, const float* rewa
 /* ---- kernel 2: centred-rank transform + weighted noise reduction + Adam
  *      (estorch.py:15-39 rank_transformation, :174-179 _calculate_grad and the
  *      NS/NSR/NSRA variants :419-425/:542-549/:640-648, :236-244 negate+clamp,
- *      :245 optimizer.step -> torch Adam) ---- */
+ *      :245 optimizer.step -> torch Adam) ----
+ *
+ * Common to the three rank + gradient functions below:
+ *   returns [P] (reward column), novelty [P] or NULL.  Blend row c = w_rew*c(reward) +
+ *   w_nov*c(novelty) in fp32 when novelty is given (ES: novelty NULL -> c(reward)).  Ranks are
+ *   bit-exact vs _compute_ranks on tie-free input (ties: stable by member index; NaN returns sort
+ *   last like numpy's argsort, among themselves by index); centring in fp64 then fp32 as
+ *   estorch.py:17-19,:176.  The gradient estimate is
+ *     g = (1/P) * sum_j (c_j - c_{j+pairs}) * T[off_j : off_j+n]
+ *   over pair j's offset offsets[j] (order, nullable = reduction order from estk_make_offsets).
+ *   The noise table: exactly one of `table` (fp32) and `table16` (the EXACT fp16 copy made by
+ *   estk_shadow_f16: 8 noise values per 128-bit load, half the bytes per pair row, the same
+ *   results because every fp16 value converts exactly to the fp32 value the table holds) is
+ *   non-null; 16-byte aligned.
+ *   `world` > 1 (where taken): `returns` / `novelty` are laid out RANK-MAJOR,
+ *   [world][2][pairs/world] -- exactly what an in-place all-gather of each rank's
+ *   (returns_plus[pairs_local], returns_minus[pairs_local]) block produces, so no re-ordering copy
+ *   is needed (member j < pairs of rank r, local index i, sits at ((2r + 0) * pairs_local + i), its
+ *   mirror at ((2r + 1) * pairs_local + i)); ranks_out stays in member order and ties are still
+ *   broken by member index.  world must divide pairs.
+ *   ranks_out / ranks2_out (nullable, int32 [P]) and grad_out (nullable, fp32 [n], the reference's
+ *   un-negated estimate g) are for inspection / parity.
+ *   With Adam: grad = clamp(-g), Adam(theta, m, v) in place (theta / m / v / grad_out 16-byte
+ *   aligned); state->adam_step += 1. */
 
-/* Single-GPU fused form.  returns [P] (reward column), novelty [P] or NULL.
- * Blend row c = w_rew*c(reward) + w_nov*c(novelty) in fp32 when novelty is
- * given (ES: novelty NULL -> c(reward)).  Ranks are bit-exact vs
- * _compute_ranks on tie-free input (ties: stable by member index; NaN returns
- * sort last like numpy's argsort, among themselves by index); centring in
- * fp64 then fp32 as estorch.py:17-19,:176.
- *   g = (1/P) * sum_j (c_j - c_{j+pairs}) * T[off_j : off_j+n]
- * then grad = clamp(-g), Adam(theta, m, v) in place; state->adam_step += 1.
- * ranks_out / ranks2_out (nullable, int32 [P]) and grad_out (nullable, fp32
- * [n], the reference's un-negated estimate) are for inspection / parity. */
+/* Single-GPU fused form: all P/2 pairs, member-order returns, Adam. */
 ESTK_API int estk_rank_grad_adam(estk_ctx* ctx, const float* returns, const float* novelty,
                         float w_rew, float w_nov, int32_t P,
-                        const float* table, const int64_t* offsets, const int32_t* order,
+                        const float* table, const uint16_t* table16,
+                        const int64_t* offsets, const int32_t* order,
                         int64_t n, float* theta, float* m, float* v, estk_state* state,
                         const estk_adam_desc* adam,
                         int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream);
 
-/* Multi-GPU form: same rank phase over all P returns, reduction over the local
- * pairs [pair_begin, pair_begin+pairs_local) only; grad_sum_out[n] receives the
- * RAW partial sum (no 1/P) to be all-reduced (SUM) by the caller
+/* Multi-GPU form: same rank phase over all P returns (member order, or rank-major with
+ * world > 1), reduction over the local pairs [pair_begin, pair_begin+pairs_local) only
+ * (offsets / order index those); grad_sum_out[n] (16-byte aligned) receives the RAW partial sum
+ * (no 1/P) to be all-reduced (SUM) by the caller, then estk_clamp_adam
  * (replaces the Send/Recv star of estorch.py:207-233). */
 ESTK_API int estk_rank_grad(estk_ctx* ctx, const float* returns, const float* novelty,
-                   float w_rew, float w_nov, int32_t P,
-                   const float* table, const int64_t* offsets, const int32_t* order,
+                   float w_rew, float w_nov, int32_t P, int32_t world,
+                   const float* table, const uint16_t* table16,
+                   const int64_t* offsets, const int32_t* order,
                    int32_t pair_begin, int32_t pairs_local, int64_t n,
                    float* grad_sum_out, int32_t* ranks_out, int32_t* ranks2_out, void* stream);
 
-/* The same two entry points reading the EXACT 16-bit copy of the table (estk_shadow_f16):
- * 8 noise values per 128-bit load, half the bytes per pair row, bit-identical results
- * (every fp16 value converts exactly to the fp32 value the fp32 table holds).
- * estk_rank_grad_h additionally takes `world`: with world > 1, `returns` / `novelty` are
- * laid out RANK-MAJOR, [world][2][pairs/world] -- exactly what an in-place all-gather of
- * each rank's (returns_plus[pairs_local], returns_minus[pairs_local]) block produces, so
- * no re-ordering copy is needed (member j < pairs of rank r, local index i, sits at
- * ((2r + 0) * pairs_local + i), its mirror at ((2r + 1) * pairs_local + i)); ranks_out
- * stays in member order and ties are still broken by member index. */
-ESTK_API int estk_rank_grad_adam_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                          float w_rew, float w_nov, int32_t P,
-                          const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                          int64_t n, float* theta, float* m, float* v, estk_state* state,
-                          const estk_adam_desc* adam,
-                          int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream);
-ESTK_API int estk_rank_grad_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                     float w_rew, float w_nov, int32_t P, int32_t world,
-                     const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                     int32_t pair_begin, int32_t pairs_local, int64_t n,
-                     float* grad_sum_out, int32_t* ranks_out, int32_t* ranks2_out, void* stream);
-
 /* ---- the same update with the cross-GPU reduction INSIDE the kernel (NVLink peer memory) ----
- * Replaces estk_rank_grad_h -> NCCL all-reduce -> estk_clamp_adam (the reference's gather of returns
+ * Replaces estk_rank_grad -> NCCL all-reduce -> estk_clamp_adam (the reference's gather of returns
  * on the master + one optimizer step there, estorch.py:228-245) by ONE cooperative launch per GPU:
- *   rank + partial gradient over the local pairs -> own workspace            (as estk_rank_grad_h)
+ *   rank + partial gradient over the local pairs -> own workspace            (as estk_rank_grad)
  *   cross-GPU barrier (flags in peer memory, release/acquire at system scope)
  *   reduce-scatter: rank r sums slice r of all `world` workspaces in rank order (loads over NVLink),
  *   all-gather: and stores the sum into every rank's workspace (stores over NVLink)
@@ -335,6 +320,8 @@ ESTK_API int estk_rank_grad_h(estk_ctx* ctx, const float* returns, const float* 
  * The sum over ranks is taken in rank order 0..world-1 on every slice: deterministic and identical on
  * all GPUs (it differs from NCCL's order by fp32 rounding only).
  * Every rank of the job must make the same call in the same generation (like a collective).
+ * Returns rank-major, 2 <= world <= ESTK_MAX_PEERS, 0 <= rank < world; the noise comes from table16,
+ * the exact fp16 copy of the table.
  *
  * Workspaces: estk_peer_alloc gives zero-filled device memory plus a 64-byte handle that another
  * process on the same node turns into a device pointer with estk_peer_open (CUDA IPC; the bytes of the
@@ -348,13 +335,13 @@ ESTK_API int estk_peer_alloc(estk_ctx* ctx, int64_t bytes, void** ptr_out, unsig
 ESTK_API int estk_peer_open(estk_ctx* ctx, const unsigned char* handle, void** ptr_out);
 ESTK_API int estk_peer_close(estk_ctx* ctx, void* ptr);
 ESTK_API int estk_peer_free(estk_ctx* ctx, void* ptr);
-ESTK_API int estk_rank_grad_xr_adam_h(estk_ctx* ctx, const float* returns, const float* novelty,
-                             float w_rew, float w_nov, int32_t P, int32_t world, int32_t rank,
-                             const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                             int32_t pair_begin, int32_t pairs_local, int64_t n,
-                             void* const* peer_ws, float* theta, float* m, float* v,
-                             estk_state* state, const estk_adam_desc* adam,
-                             int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream);
+ESTK_API int estk_rank_grad_xr_adam(estk_ctx* ctx, const float* returns, const float* novelty,
+                           float w_rew, float w_nov, int32_t P, int32_t world, int32_t rank,
+                           const uint16_t* table16, const int64_t* offsets, const int32_t* order,
+                           int32_t pair_begin, int32_t pairs_local, int64_t n,
+                           void* const* peer_ws, float* theta, float* m, float* v,
+                           estk_state* state, const estk_adam_desc* adam,
+                           int32_t* ranks_out, int32_t* ranks2_out, float* grad_out, void* stream);
 
 /* Epilogue on an all-reduced raw sum: g = grad_sum / P, negate, clamp, Adam.
  * theta/m/v NULL with grad_out set = gradient only (for non-Adam optimizers:

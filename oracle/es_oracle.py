@@ -199,7 +199,7 @@ def round_bf16(x: np.ndarray) -> np.ndarray:
 
 
 def mlp_forward_bf16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Numerics of the wgmma evaluate path (estk_eval_mlp_bf16): weights and
+    """Numerics of the wgmma evaluate path (estk_eval_mlp, ESTK_PREC_BF16): weights and
     layer inputs rounded to bf16, products accumulated in fp32, bias / ReLU in
     fp32.  ``flat`` is the already-perturbed fp32 row."""
     h = round_bf16(np.asarray(obs, dtype=np.float32))
@@ -220,7 +220,7 @@ def round_f16(x: np.ndarray) -> np.ndarray:
 
 
 def mlp_forward_f16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Emulation of estk_eval_mlp_f16's roundings (test infrastructure for the kernel's
+    """Emulation of the roundings of estk_eval_mlp with ESTK_PREC_F16 (test infrastructure for the kernel's
     own arithmetic; parity proper is against mlp_forward): weights and hidden activations
     rounded to fp16, the observation split x_hi + x_lo, fp32 (here fp64) accumulation,
     fp32 bias."""
@@ -265,7 +265,7 @@ def sample_population(theta: np.ndarray, table: np.ndarray, offsets: np.ndarray,
 
 
 def sample_population_bf16s(theta: np.ndarray, table: np.ndarray, offsets: np.ndarray, sigma: float):
-    """Rows as the "bf16s" evaluate path forms them (estk_eval_mlp_bf16s):
+    """Rows as the "bf16s" evaluate path forms them (estk_eval_mlp, ESTK_PREC_BF16S):
     ``W = bf16(theta16 +- sigma16 * eps16)`` with theta16 = bf16(theta), eps16 =
     bf16(T[off:off+n]), sigma16 = bf16(sigma) and ONE rounding of the exact
     product-sum (PTX ``fma.rn.bf16x2``).  Biases are formed from the fp32 sources in

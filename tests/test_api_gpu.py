@@ -345,7 +345,7 @@ def test_train_n_proc_2_reexecs_under_torchrun(tmp_path):
 
 def test_peer_memory_gradient_sum_matches_nccl_on_2_gpus():
     """tools/multi_gpu_check.py under torchrun on 2 GPUs: fused ES and NSRA-ES with the gradient summed inside the
-    kernel over NVLink peer memory (estk_rank_grad_xr_adam_h) and with NCCL -- replicas bit-identical across
+    kernel over NVLink peer memory (estk_rank_grad_xr_adam) and with NCCL -- replicas bit-identical across
     ranks, CUDA-graph replay == eager launches, the two reductions equal up to the order of an fp32 sum."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")

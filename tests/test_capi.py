@@ -16,11 +16,11 @@ def _declared_symbols():
 def test_header_and_binding_agree():
     from estorch_b200 import _capi
     declared = _declared_symbols()
-    assert len(declared) >= 15
+    assert len(declared) == 25
     assert sorted(_capi.SIGNATURES) == declared
 
 
-def test_library_loads_and_exports_every_symbol():
+def test_library_loads_and_exports_the_25_symbols_of_abi_200():
     from estorch_b200 import _capi
     if not os.path.exists(_capi.LIB_PATH):
         import __graft_entry__
@@ -28,7 +28,7 @@ def test_library_loads_and_exports_every_symbol():
     lib = _capi.load()
     for name in _declared_symbols():
         assert hasattr(lib, name), f"libestk.so does not export {name}"
-    assert lib.estk_version() == 100
+    assert lib.estk_version() == 200
     assert isinstance(lib.estk_last_error(), bytes)
 
 
@@ -59,7 +59,7 @@ def test_product_never_imports_the_oracle():
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", src, flags=re.M), f
 
 
-def test_error_reporting_through_the_c_abi_without_gpu():
+def test_error_reporting_and_precision_probe_without_gpu():
     """estk_ctx_create on a box without a usable device returns a negative status and leaves a
     message in estk_last_error(); null arguments are rejected before any CUDA call."""
     import ctypes as C
@@ -73,4 +73,4 @@ def test_error_reporting_through_the_c_abi_without_gpu():
         rc = lib.estk_ctx_create(0, C.byref(ctx))
         assert rc < 0 and len(lib.estk_last_error()) > 0 and not ctx.value
     assert lib.estk_ctx_destroy(None) == 0
-    assert lib.estk_eval_mlp_bf16_supported(None, 256) == 0
+    assert lib.estk_eval_mlp_supported(None, _capi.ESTK_PREC_BF16, 256) == 0

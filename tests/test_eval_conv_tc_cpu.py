@@ -13,18 +13,19 @@ def _header_params(name):
     return [a.strip() for a in m.group(1).split(",")]
 
 
-def test_conv_f16_binding_matches_header():
+def test_conv_binding_with_precision_argument_matches_header():
     from estorch_b200 import _capi
-    for name in ("estk_eval_conv_vbn_f16", "estk_eval_conv_vbn_f16_scratch_bytes"):
+    for name in ("estk_eval_conv_vbn", "estk_eval_conv_vbn_scratch_bytes"):
         assert len(_capi.SIGNATURES[name]) == len(_header_params(name)), name
-    assert "const uint16_t* table16" in _header_params("estk_eval_conv_vbn_f16")
+        assert "int32_t precision" in _header_params(name), name
+    assert "const uint16_t* table16" in _header_params("estk_eval_conv_vbn")
 
 
-def test_conv_f16_rejects_null_arguments_before_any_cuda_call():
+def test_conv_f16_precision_rejects_null_arguments_before_any_cuda_call():
     from estorch_b200 import _capi
     lib = _capi.load()
-    rc = lib.estk_eval_conv_vbn_f16(None, 4, None, None, None, None, None, 1, 0.02, None, 128, None, None, 32,
-                                    None, None, None, 0, None)
+    rc = lib.estk_eval_conv_vbn(None, _capi.ESTK_PREC_F16, 4, None, None, None, None, None, 1, 0.02, None, 128, None,
+                                None, 32, None, None, None, 0, None)
     assert rc == -1
     assert b"null" in lib.estk_last_error()
-    assert lib.estk_eval_conv_vbn_f16_scratch_bytes(None, 128, 32) == -1
+    assert lib.estk_eval_conv_vbn_scratch_bytes(None, _capi.ESTK_PREC_F16, 128, 32) == -1

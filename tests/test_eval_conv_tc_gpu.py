@@ -1,5 +1,5 @@
 """The tensor-core ("f16") evaluate of the conv + VirtualBatchNorm policy (examples/atari.py:14-37):
-estk_eval_conv_vbn_f16 against the reference golden, the CPU oracle's fp32 forward and the fp32
+estk_eval_conv_vbn with ESTK_PREC_F16 against the reference golden, the CPU oracle's fp32 forward and the fp32
 CUDA-core kernel, through the ctypes binding and through the public ES API.
 
 Bar: every return within 1e-5 max-norm relative (SURVEY App. A.5) of the oracle's fp32 forward

@@ -1,4 +1,4 @@
-"""Tanh MLP policies on the H100: every MLP evaluate entry point with the four activation codes of
+"""Tanh MLP policies on the H100: every MLP evaluate precision with the four activation codes of
 include/estk.h (hidden ReLU / Tanh x output identity / Tanh), against the reference-generated Tanh
 goldens and the activation-aware oracle (tests/_act_oracle.py); the north-star shape in fp32 and
 f16; and the public API (ES / NSR-ES fused runs, CUDA-graph replay, an f16 fused generation)."""
@@ -73,7 +73,7 @@ def test_fp32_tanh_matches_reference_goldens(be):
     pop, _ = orc.sample_population(theta, g["table"], offs, float(g["sigma"]))
     _, want_bc = act.evaluate_population(pop, dims, g["obs"], g["target"], 64, 256, "tanh", "tanh")
     assert rel_err(bcs, want_bc) < 2e-6
-    # centre entry point: the archive's first entry is the BC of meta_theta0[0]
+    # centre evaluation: the archive's first entry is the BC of meta_theta0[0]
     one, bc1 = be.zeros(1), be.zeros(256)
     be.eval_mlp_center(dims, dev(be, g["meta_theta0"][0]), dev(be, g["obs"]), dev(be, g["target"]), one, bc1, 64, 256,
                        act=code)
@@ -153,7 +153,7 @@ def test_tensor_core_modes_vs_emulation_and_fp32(be, dims, B, pairs, bc, mode, a
         assert rel_err(got_bc, emu_bc) < t_bc
         if mode == "f16":
             assert rel_err(got_bc, exact_bc) < 2e-3
-    # the folded centre task and the *_center_* entry point evaluate theta itself
+    # the folded centre task and the centre call (offsets NULL) evaluate theta itself
     one = be.zeros(1)
     be.eval_mlp_center(dims, th, dev(be, obs), dev(be, tgt), one, precision=mode, act=act_code,
                        **({"theta16": kw["theta16"]} if mode == "bf16s" else {}))
@@ -165,20 +165,20 @@ def test_tensor_core_modes_vs_emulation_and_fp32(be, dims, B, pairs, bc, mode, a
 
 
 # ------------------------------------------------------------------ ABI: activation codes
-def test_invalid_activation_codes_are_refused(be):
+def test_invalid_activation_codes_are_refused_by_every_precision(be):
     from estorch_b200 import _capi
     from estorch_b200.backend import mlp_desc
     lib = _capi.load()
     dims, B = [64, 64, 32], 256
     for code in ALL_ACTS:
         d = mlp_desc(dims, code)
-        assert lib.estk_eval_mlp_f16_supported(C.byref(d), B) == 1
-        assert lib.estk_eval_mlp_bf16_supported(C.byref(d), B) == 1
+        assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16, B) == 1
+        assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_BF16, B) == 1
     n, table, theta, obs, tgt, offs = _tc_problem(dims, B, 2)
     for code in (2, 0x200, 0x101 | 0x10000, -1, 0xff, 1 << 9):
         d = mlp_desc(dims, code)
-        assert lib.estk_eval_mlp_f16_supported(C.byref(d), B) == 0
-        assert lib.estk_eval_mlp_bf16_supported(C.byref(d), B) == 0
+        assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16, B) == 0
+        assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_BF16, B) == 0
         ret, one = be.zeros(4), be.zeros(1)
         args = (dev(be, theta), dev(be, table), dev(be, offs), None, 2, 0.02, dev(be, obs), dev(be, tgt),
                 ret[:2], ret[2:])

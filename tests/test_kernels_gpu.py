@@ -255,10 +255,11 @@ def test_rank_ties_stable_by_index(be):
 
 @pytest.mark.parametrize("n,P,W", [(1001760, 512, 4), (6020, 256, 2), (4610, 64, 1)])
 def test_rank_grad_fp16_table_and_rank_major_layout(be, n, P, W):
-    """estk_rank_grad[_adam]_h stream the EXACT fp16 copy of the table: same ranks, and the same gradient /
-    theta as the fp32-table entry points (bit-identical when both take the column-split path, i.e. large n;
+    """estk_rank_grad[_adam] with table16, the EXACT fp16 copy of the table: same ranks, and the same gradient /
+    theta as with the fp32 table (bit-identical when both take the column-split path, i.e. large n;
     a different pair split for small n only changes the fp32 summation order).  With world = W the returns
-    arrive rank-major [W][2][pairs/W] (what the in-place all-gather produces): ranks_out stays in member order."""
+    arrive rank-major [W][2][pairs/W] (what the in-place all-gather produces), with either table: ranks_out
+    stays in member order."""
     from estorch_b200.backend import new_state, adam_desc
     rng = np.random.RandomState(5)
     table_len = (n + 31) // 32 * 32 + (1 << 16)
@@ -290,15 +291,17 @@ def test_rank_grad_fp16_table_and_rank_major_layout(be, n, P, W):
     rm = np.empty((W, 2, pl), np.float32)
     for r in range(W):
         rm[r, 0], rm[r, 1] = ret[r * pl:(r + 1) * pl], ret[pairs + r * pl: pairs + (r + 1) * pl]
-    total = be.zeros(n)
-    for r in range(W):
-        part, ranks = be.zeros(n), be.zeros(P, dtype=torch.int32)
-        so = offs[r * pl:(r + 1) * pl]
-        be.rank_grad(dev(be, rm.reshape(-1)), None, 1.0, 0.0, P, tb16, dev(be, so),
-                     dev(be, np.argsort(so, kind="stable").astype(np.int32)), r * pl, pl, n, part, ranks, None, world=W)
-        np.testing.assert_array_equal(ranks.cpu().numpy(), res["fp32"][0])
-        total += part
-    assert rel_err((total / P).cpu().numpy(), res["fp32"][1]) < 2e-6
+    for t in (tb16, tb):
+        total = be.zeros(n)
+        for r in range(W):
+            part, ranks = be.zeros(n), be.zeros(P, dtype=torch.int32)
+            so = offs[r * pl:(r + 1) * pl]
+            be.rank_grad(dev(be, rm.reshape(-1)), None, 1.0, 0.0, P, t, dev(be, so),
+                         dev(be, np.argsort(so, kind="stable").astype(np.int32)), r * pl, pl, n, part, ranks, None,
+                         world=W)
+            np.testing.assert_array_equal(ranks.cpu().numpy(), res["fp32"][0])
+            total += part
+        assert rel_err((total / P).cpu().numpy(), res["fp32"][1]) < 2e-6
 
 
 def test_rank_nan_returns_sort_last(be):

@@ -1,4 +1,4 @@
-"""Under torchrun: the in-kernel cross-GPU gradient sum (estk_rank_grad_xr_adam_h) against the same kernel +
+"""Under torchrun: the in-kernel cross-GPU gradient sum (estk_rank_grad_xr_adam) against the same kernel +
 NCCL all-reduce + clamp/Adam from identical state: theta', m, v, g compared element by element (bit-identical is
 expected at 2 GPUs: a two-term fp32 sum does not depend on its order), repeated to catch races; then timings."""
 import os, sys, traceback, torch, torch.distributed as dist
