@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ESTK_LIBRARY") or os.path.join(_HERE, "lib", "libestk.so")
 
 ESTK_MAX_LAYERS = 8
-ESTK_MAX_POPULATION = 32768
+ESTK_MAX_POPULATION = 1 << 22
 # estk_mlp_desc.activation bit fields: hidden activation in bits 0-7, output activation in bits 8-15
 ESTK_ACT_RELU = 0
 ESTK_ACT_TANH = 1

@@ -39,18 +39,39 @@ static inline bool estk_act_valid(int a) {
 }
 
 // ---------------------------------------------------------------- context
+static const int kCtxMaxRetired = 64;
+// The per-member buffers are sized for kCtxInitialMembers at estk_ctx_create and grown by
+// estk_ctx_reserve when a call needs more (a population beyond that, or a wider evaluate).
 struct estk_ctx {
   int device;
   int sm_count;
   int cc_major, cc_minor;
   int max_grid;            // sm_count * 8: upper bound on any persistent grid
-  float* cvals;            // [ESTK_MAX_POPULATION] blended centred ranks (fp32)
+  int64_t members;         // capacity of cvals / counters / sort_ws, in members
+  int64_t eval_floats;     // capacity of eval_partial, in floats
+  float* cvals;            // [members] blended centred ranks (fp32)
   float* partial;          // [max_grid * 1024] split-over-pairs partial sums
-  float* eval_partial;     // [ESTK_MAX_POPULATION * 2 * kEvalMaxChunks] loss partials
-  unsigned int* counters;  // [ESTK_MAX_POPULATION + 8] self-resetting arrival counters (+ kernel tickets)
+  float* eval_partial;     // [eval_floats] loss partials of the evaluate kernels
+  unsigned int* counters;  // [kCtxTicketSlots + members]: kernel tickets, then self-resetting arrival counters
+  void* sort_ws;           // estk_sort::workspace_bytes(members, 4, max_grid) bytes: radix-sort buffers
   double* scalars;         // [8] small fp64 scratch (||archive||_F, ...)
+  void* retired[kCtxMaxRetired];  // buffers replaced by growth, freed at estk_ctx_destroy (earlier graphs use them)
+  int n_retired;
 };
 static const int kEvalMaxChunks = 64;   // the tensor-core evaluate writes up to 2 * kEvalMaxChunks partials per member
+static const int64_t kCtxInitialMembers = 32768;
+// counters[0 .. kCtxTicketSlots): last-CTA tickets at fixed slots; the per-member counters follow
+static const int kCtxTicketSlots = 8;
+static const int kTicketClampAdam = 0;
+static const int kTicketTrackBest = 1;
+static inline unsigned int* estk_member_counters(estk_ctx* c) { return c->counters + kCtxTicketSlots; }
+
+// Grows the context workspace to at least `members` members (cvals, arrival counters, sort buffers)
+// and `eval_floats` evaluate partials; no-op when it is large enough.  Growth allocates new buffers and
+// waits on `stream` for their zero-filled counters; the old buffers stay allocated until estk_ctx_destroy
+// (graphs captured before keep working), and stay in use if the allocation fails (ESTK_ERR_NOMEM).
+// Refused with ESTK_ERR_NOMEM while `stream` is being captured into a CUDA graph.
+int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who);
 
 // ---------------------------------------------------------------- evaluate back ends
 // estk_eval_mlp and estk_eval_conv_vbn check their arguments once, then hand the call to the

@@ -255,8 +255,10 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
   p.BC = rows / 2;
   p.chunks = (p.B + p.BC - 1) / p.BC;
   ESTK_CHECK_ARG(p.chunks <= kEvalMaxChunks, "%s: B=%d needs %d chunks > %d", who, p.B, p.chunks, kEvalMaxChunks);
+  const int rc = estk_ctx_reserve(ctx, p.pairs, (int64_t)p.pairs * 2 * p.chunks, stream, who);
+  if (rc) return rc;
   p.partial = ctx->eval_partial;
-  p.counters = ctx->counters;
+  p.counters = estk_member_counters(ctx);
   const size_t smem = smem_bytes(rows, maxw);
   switch (rows) {
     case 256: return launch<256>(p, smem, stream);

@@ -611,10 +611,12 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
   p.chunks = p.B / kRows;
   ESTK_CHECK_ARG(p.chunks <= 2 * kEvalMaxChunks, "%s: batch too large", who);
   p.n_centre = p.centre_out ? p.chunks : 0;
-  ESTK_CHECK_ARG(!p.centre_out || p.pairs * 2 < ESTK_MAX_POPULATION, "%s: population too large to fold the centre task", who);
   p.n_tasks = p.n_centre + p.pairs * p.n_signs * p.chunks;
+  const int64_t cells = (int64_t)p.pairs * 2 + (p.centre_out ? 1 : 0);   // [pairs][sign], then the folded centre
+  const int rc = estk_ctx_reserve(ctx, cells, cells * p.chunks, stream, who);
+  if (rc) return rc;
   p.partial = ctx->eval_partial;
-  p.counters = ctx->counters;
+  p.counters = estk_member_counters(ctx);
 #ifdef ESTK_TC_PROFILE
   p.prof = g_prof_buf;
 #endif

@@ -37,7 +37,7 @@ extern "C" int estk_track_best(estk_ctx* ctx, estk_state* state, const float* re
   int blocks = (int)((n + 255) / 256);
   if (blocks > ctx->sm_count * 4) blocks = ctx->sm_count * 4;
   track_best_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(state, reward, theta, best_theta, n,
-                                                             ctx->counters + ESTK_MAX_POPULATION + 1);
+                                                             ctx->counters + kTicketTrackBest);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
 }

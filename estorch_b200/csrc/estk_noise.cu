@@ -4,6 +4,8 @@
 // + two `torch.cat`s (estorch/estorch.py:187-193, 96 % of its generation time)
 // by indexing a shared, device-resident unit-normal table.
 #include "estk_common.cuh"
+#include "estk_sort.cuh"
+#include <cooperative_groups.h>
 #include <cuda_fp16.h>
 
 // ------------------------------------------------------------------ Philox
@@ -71,50 +73,49 @@ extern "C" int estk_fill_noise_table(estk_ctx* ctx, float* table, int64_t len, u
 }
 
 // ------------------------------------------------------------------ offsets
-// One CTA: hash every local pair to a 128-byte-aligned table slot, optionally
-// bitonic-sort (offset, index) keys in shared memory to emit the L2-friendly
-// evaluation order.
+// Hash every local pair to a 128-byte-aligned table slot; pair i's slot depends on (seed, generation,
+// pair_begin + i) only.
+__device__ __forceinline__ uint64_t pair_slot(uint64_t base, int64_t pair_begin, int i, uint64_t nslots) {
+  return estk_mix64(base + (uint64_t)(pair_begin + i)) % nslots;
+}
+
+__device__ __forceinline__ uint64_t offsets_base(uint64_t seed, const estk_state* state, int64_t gen_host) {
+  const uint64_t gen = (uint64_t)((state ? state->generation : 0) + gen_host);
+  return estk_mix64(seed ^ (gen * ESTK_GEN_MUL));
+}
+
+// Offsets only (no evaluation order requested).
 __global__ void __launch_bounds__(1024) make_offsets_kernel(uint64_t seed, const estk_state* state,
                                                             int64_t gen_host, int64_t pair_begin,
                                                             int pairs, uint64_t nslots,
-                                                            int64_t* __restrict__ offsets_out,
-                                                            int32_t* __restrict__ order_out,
-                                                            int sort_len) {
-  extern __shared__ uint64_t keys[];
-  const uint64_t gen = (uint64_t)((state ? state->generation : 0) + gen_host);
-  const uint64_t base = estk_mix64(seed ^ (gen * ESTK_GEN_MUL));
-  for (int i = threadIdx.x; i < sort_len; i += blockDim.x) {
-    uint64_t key = ~0ull;
-    if (i < pairs) {
-      const uint64_t slot = estk_mix64(base + (uint64_t)(pair_begin + i)) % nslots;
-      const uint64_t off = slot * 32ull;
-      offsets_out[i] = (int64_t)off;
-      key = (off << 16) | (uint64_t)i;
-    }
-    if (order_out) keys[i] = key;
-  }
-  if (!order_out) return;
-  __syncthreads();
-  for (int k = 2; k <= sort_len; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < sort_len; i += blockDim.x) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const uint64_t a = keys[i], b = keys[ixj];
-          const bool up = ((i & k) == 0);
-          if ((a > b) == up) { keys[i] = b; keys[ixj] = a; }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int i = threadIdx.x; i < pairs; i += blockDim.x) order_out[i] = (int32_t)(keys[i] & 0xFFFFull);
+                                                            int64_t* __restrict__ offsets_out) {
+  const uint64_t base = offsets_base(seed, state, gen_host);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < pairs; i += gridDim.x * blockDim.x)
+    offsets_out[i] = (int64_t)(pair_slot(base, pair_begin, i, nslots) * 32ull);
 }
 
-// The same outputs for up to 4096 pairs in ~6 block-wide steps instead of the 66 passes of the bitonic network: the
-// slots are uniform hashes, so a bucket per expected key (bucket = slot * NB / nslots, monotone in the key) holds
+// More than kBucketSortMax pairs: one cooperative grid hashes the offsets and sorts (slot, local index)
+// with the grid-wide stable radix sort (estk_sort.cuh).  The input is in index order, so equal slots
+// keep index order: the unique order by (offset, index), as the bucket kernel gives below.
+constexpr int kOffsetsSortThreads = 512;
+__global__ void __launch_bounds__(kOffsetsSortThreads) make_offsets_sort_kernel(
+    uint64_t seed, const estk_state* state, int64_t gen_host, int64_t pair_begin, int pairs, uint64_t nslots,
+    int slot_bits, int64_t* __restrict__ offsets_out, int32_t* __restrict__ order_out, const estk_sort::Workspace ws) {
+  extern __shared__ __align__(16) uint32_t s_sort[];
+  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+  const uint64_t base = offsets_base(seed, state, gen_host);
+  const int gthreads = gridDim.x * kOffsetsSortThreads;
+  for (int i = blockIdx.x * kOffsetsSortThreads + threadIdx.x; i < pairs; i += gthreads)
+    offsets_out[i] = (int64_t)(pair_slot(base, pair_begin, i, nslots) * 32ull);
+  auto load = [&](int i) { return (unsigned long long)pair_slot(base, pair_begin, i, nslots); };
+  const int b = estk_sort::grid_sort<unsigned long long, kOffsetsSortThreads>(grid, ws, pairs, slot_bits, load, s_sort);
+  for (int s = blockIdx.x * kOffsetsSortThreads + threadIdx.x; s < pairs; s += gthreads)
+    order_out[s] = (int32_t)__ldcg((b ? ws.vals[1] : ws.vals[0]) + s);
+}
+
+// Up to 4096 pairs: one CTA, ~6 block-wide steps.  The slots are uniform hashes, so a bucket per expected key (bucket = slot * NB / nslots, monotone in the key) holds
 // ~1 key; count, scan, scatter, then every bucket's handful of keys is put in order by one thread.  The result
-// is the unique sorted order of the (offset << 16 | index) keys, bit-identical to the network's.
+// is the unique sorted order of the (offset << 16 | index) keys, the same order the radix sort gives above.
 constexpr int kBucketSortMax = 4096;
 __global__ void __launch_bounds__(1024) make_offsets_bucket_kernel(uint64_t seed, const estk_state* state,
                                                                    int64_t gen_host, int64_t pair_begin,
@@ -209,11 +210,12 @@ extern "C" int estk_make_offsets(estk_ctx* ctx, uint64_t seed, const estk_state*
   ESTK_CHECK_ARG(n > 0 && pair_begin >= 0, "estk_make_offsets: bad n/pair_begin");
   const int64_t n_pad = (n + 31) / 32 * 32;
   ESTK_CHECK_ARG(table_len >= n_pad, "estk_make_offsets: table_len %lld < padded row %lld", (long long)table_len, (long long)n_pad);
-  ESTK_CHECK_ARG(table_len < (1ll << 40), "estk_make_offsets: table too long for the sort key");
+  ESTK_CHECK_ARG(table_len < (1ll << 40), "estk_make_offsets: table of %lld entries is too long (< 2^40)",
+                 (long long)table_len);
   const uint64_t nslots = (uint64_t)((table_len - n_pad) / 32 + 1);
-  int sort_len = 1;
-  while (sort_len < pairs) sort_len <<= 1;
   if (order_out && pairs <= kBucketSortMax) {
+    int sort_len = 1;
+    while (sort_len < pairs) sort_len <<= 1;
     const int nb = sort_len < 32 ? 32 : sort_len;
     if ((size_t)nb * 12 > 40 * 1024)
       ESTK_CUDA(cudaFuncSetAttribute(make_offsets_bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -223,13 +225,34 @@ extern "C" int estk_make_offsets(estk_ctx* ctx, uint64_t seed, const estk_state*
     ESTK_CUDA(cudaGetLastError());
     return ESTK_OK;
   }
-  const size_t smem = order_out ? sizeof(uint64_t) * (size_t)sort_len : 0;
-  if (smem > 48 * 1024)
-    ESTK_CUDA(cudaFuncSetAttribute(make_offsets_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  make_offsets_kernel<<<1, 1024, smem, (cudaStream_t)stream>>>(
-      seed, state, gen_host, pair_begin, pairs, nslots, offsets_out, order_out,
-      order_out ? sort_len : pairs);
-  ESTK_CUDA(cudaGetLastError());
+  if (!order_out) {
+    int blocks = (pairs + 1023) / 1024;
+    if (blocks > ctx->sm_count * 4) blocks = ctx->sm_count * 4;
+    make_offsets_kernel<<<blocks, 1024, 0, (cudaStream_t)stream>>>(seed, state, gen_host, pair_begin, pairs, nslots,
+                                                                  offsets_out);
+    ESTK_CUDA(cudaGetLastError());
+    return ESTK_OK;
+  }
+  // 8-byte slot keys for `pairs` elements: the sort buffers of 2 * pairs members
+  const int rc = estk_ctx_reserve(ctx, 2 * (int64_t)pairs, 0, (cudaStream_t)stream, "estk_make_offsets");
+  if (rc) return rc;
+  int slot_bits = 0;
+  while (slot_bits < 64 && ((nslots - 1) >> slot_bits) != 0) ++slot_bits;
+  constexpr size_t kSmem = estk_sort::smem_bytes(kOffsetsSortThreads);
+  int occ = 0;
+  ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, make_offsets_sort_kernel, kOffsetsSortThreads, kSmem));
+  if (occ < 1) {
+    estk_set_error("make_offsets_sort_kernel cannot be resident");
+    return ESTK_ERR_CUDA;
+  }
+  int grid = (pairs + kOffsetsSortThreads - 1) / kOffsetsSortThreads;
+  if (grid > occ * ctx->sm_count) grid = occ * ctx->sm_count;
+  if (grid > ctx->max_grid) grid = ctx->max_grid;
+  const estk_sort::Workspace ws = estk_sort::workspace_of(ctx);
+  void* args[] = {&seed, (void*)&state, &gen_host, &pair_begin, &pairs, (void*)&nslots, &slot_bits, &offsets_out,
+                  &order_out, (void*)&ws};
+  ESTK_CUDA(cudaLaunchCooperativeKernel((void*)make_offsets_sort_kernel, dim3(grid), dim3(kOffsetsSortThreads), args,
+                                        kSmem, (cudaStream_t)stream));
   return ESTK_OK;
 }
 

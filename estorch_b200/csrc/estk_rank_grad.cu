@@ -12,9 +12,10 @@
 // reads both [eps; -eps] halves, 2x this) + 28*n (theta/m/v read+write, g) + 8*P.
 //
 // Decomposition: grid = CS column-splits x PS pair-splits, all CTAs co-resident.
-//   phase A  every warp ranks members (all-pairs count, O(P^2) compares total;
-//            bit-exact integer ranks; stable-by-index on ties), centres in
-//            fp64 -> fp32 and blends reward/novelty rows          -> grid.sync
+//   phase A  bit-exact integer ranks, stable by index on ties: P <= 8192 every warp
+//            counts over keys in shared memory (O(P^2) compares total); larger P
+//            a grid-wide radix sort (estk_sort.cuh).  Centres in fp64 -> fp32 and
+//            blends reward/novelty rows                             -> grid.sync
 //   phase B  CTA (cs, ps) owns float4 columns [c0,c1) and sorted pair slots
 //            [s0,s1): 128-bit read-only loads, fp32 FMA into registers, 16
 //            independent loads in flight per thread (128 KB per SM: the kernel is
@@ -25,6 +26,7 @@
 //            to the workspace -> grid.sync -> fixed-order sum -> epilogue
 //            (deterministic; no atomics anywhere).
 #include "estk_common.cuh"
+#include "estk_sort.cuh"
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
 #include <type_traits>
@@ -48,7 +50,7 @@ struct RankGradParams {
   const int32_t* order;    // [pairs_local] nullable
   int64_t n, n4;
   int CS, PS;
-  int keys_in_smem;  // phase A ranks from 64-bit keys staged in (dynamic) shared memory: P * 8 bytes
+  estk_sort::Workspace sort;  // phase A for P > 8192: radix-sort buffers (context workspace)
   float* cvals;    // [P] workspace
   float* partial;  // [PS * n4 * 4] workspace (PS > 1)
   int32_t* ranks_out;
@@ -77,6 +79,14 @@ __host__ __device__ inline int64_t xr_image_bytes(int64_t n) { return ((n + 3) /
 struct AdamScalars {
   float one_minus_b1, b2, one_minus_b2, bc2_sqrt, eps, neg_step, wd, clamp, inv_div;
 };
+
+// Order-preserving 32-bit image of a return: -0 maps to +0 (they compare equal), every NaN to 0xffffffff
+// (after +inf: numpy's argsort puts NaN last).  image(a) < image(b) <=> a sorts before b.
+__device__ __forceinline__ uint32_t rank_image(float v) {
+  v = __fadd_rn(v, 0.f);
+  const uint32_t b = __float_as_uint(v);
+  return v != v ? 0xffffffffu : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));
+}
 
 __device__ __forceinline__ float centre(int rank, int P) {
   // estorch.py:17-19 in float64, cast to fp32 at :176
@@ -216,7 +226,58 @@ __device__ __forceinline__ void xr_phase(const RankGradParams& p, const AdamScal
   if (blockIdx.x == 0 && tid == 0) *reinterpret_cast<volatile uint32_t*>(mine + kXrEpochOff) = epoch + 1;
 }
 
-template <int NC, int T, int LOADS = 8, bool T16 = false, bool XR = false>
+// Phase A for P > 8192, one column: a stable grid-wide radix sort of (rank_image(value), member) in member
+// order, so equal images keep index order; rank[member] = its sorted position (O(P) per pass instead of the
+// O(P^2) count).  `second`: blend into cvals (the novelty column).
+template <int T>
+__device__ __forceinline__ void sort_ranks_body(const float* vals, int32_t* ranks_out, float* cvals, float w_rew, float w_nov,
+                                        bool second, int P, int world, void* k0, void* k1, uint32_t* v0,
+                                        uint32_t* v1, uint32_t* hist, uint32_t* total, uint32_t* s_sort) {
+  cg::grid_group grid = cg::this_grid();
+  estk_sort::Workspace ws;
+  ws.keys[0] = k0; ws.keys[1] = k1; ws.vals[0] = v0; ws.vals[1] = v1; ws.hist = hist; ws.total = total;
+  const int pairs = P / 2;
+  const int pl = pairs / max(world, 1);
+  auto pos_of = [&](int m) { const int sg = m / pairs, g = m % pairs; return ((g / pl) * 2 + sg) * pl + g % pl; };
+  auto load = [&](int m) { return rank_image(__ldg(vals + (world > 1 ? pos_of(m) : m))); };
+  const int b = estk_sort::grid_sort<uint32_t, T>(grid, ws, P, 32, load, s_sort);
+  const uint32_t* member = b ? v1 : v0;
+  for (int s = blockIdx.x * T + threadIdx.x; s < P; s += gridDim.x * T) {
+    const int i = (int)__ldcg(member + s);
+    if (ranks_out) ranks_out[i] = s;
+    if (!second) {
+      cvals[i] = centre(s, P);
+    } else {
+      // estorch.py:645-646; cvals[i] was written by some thread before the sort's grid.syncs
+      cvals[i] = __fadd_rn(__fmul_rn(w_rew, __ldcg(cvals + i)), __fmul_rn(w_nov, centre(s, P)));
+    }
+  }
+}
+
+// The 512-thread kernels (up to 128 registers, phase B near the limit) call the sort out of line, with its
+// arguments by value, so that none of its state enters phase B's register allocation; the 256-thread kernels
+// (80 registers) inline it -- there the call's saved registers would spill instead.
+template <int T>
+__device__ __noinline__ void sort_ranks_call(const float* vals, int32_t* ranks_out, float* cvals, float w_rew,
+                                             float w_nov, bool second, int P, int world, void* k0, void* k1,
+                                             uint32_t* v0, uint32_t* v1, uint32_t* hist, uint32_t* total,
+                                             uint32_t* s_sort) {
+  sort_ranks_body<T>(vals, ranks_out, cvals, w_rew, w_nov, second, P, world, k0, k1, v0, v1, hist, total, s_sort);
+}
+
+template <int T>
+__device__ __forceinline__ void sort_ranks(const float* vals, int32_t* ranks_out, float* cvals, float w_rew,
+                                           float w_nov, bool second, int P, int world, void* k0, void* k1,
+                                           uint32_t* v0, uint32_t* v1, uint32_t* hist, uint32_t* total,
+                                           uint32_t* s_sort) {
+  if constexpr (T == 512)
+    sort_ranks_call<T>(vals, ranks_out, cvals, w_rew, w_nov, second, P, world, k0, k1, v0, v1, hist, total, s_sort);
+  else
+    sort_ranks_body<T>(vals, ranks_out, cvals, w_rew, w_nov, second, P, world, k0, k1, v0, v1, hist, total, s_sort);
+}
+
+// SORT: phase A by the grid-wide radix sort (P > 8192) instead of the shared-memory count (P <= 8192)
+template <int NC, int T, int LOADS = 8, bool T16 = false, bool XR = false, bool SORT = false>
 __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const RankGradParams p) {
   constexpr int kThreads = T;
   cg::grid_group grid = cg::this_grid();
@@ -225,7 +286,7 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
   __shared__ __align__(16) float s_w[kPairTile];
   __shared__ __align__(16) uint32_t s_off4[kPairTile];
   __shared__ AdamScalars s_adam;
-  extern __shared__ __align__(16) unsigned long long s_key_raw[];   // [P] when p.keys_in_smem
+  extern __shared__ __align__(16) unsigned long long s_key_raw[];   // [P] keys, or the sort's scratch (SORT)
   uint64_t* s_key = reinterpret_cast<uint64_t*>(s_key_raw);
 
   // ---- Adam scalars (read adam_step BEFORE the first grid.sync; block 0
@@ -262,19 +323,14 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
     const int pl = p.pairs / max(p.world, 1);
     auto pos_of = [&](int m) { const int sg = m / p.pairs, g = m % p.pairs; return ((g / pl) * 2 + sg) * pl + g % pl; };
     auto member_of = [&](int q) { const int r = q / (2 * pl), rem = q - r * 2 * pl; return (rem / pl) * p.pairs + r * pl + rem % pl; };
-    if (p.keys_in_smem) {
-      // Every CTA builds one 64-bit key per member in shared memory -- (order-preserving image of the
-      // fp32 value) << 32 | member index -- so that rank_i = #{j: key_j < key_i}: one shared-memory load
-      // and one 64-bit compare per (i, j), ties and the rank-major index arithmetic folded into the key.
-      auto image = [](float v) {
-        v = __fadd_rn(v, 0.f);                               // -0 -> +0 (they compare equal)
-        const uint32_t b = __float_as_uint(v);
-        return v != v ? 0xffffffffu : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));
-      };
+    if constexpr (!SORT) {
+      // P <= 8192: every CTA builds one 64-bit key per member in shared memory -- (order-preserving image
+      // of the fp32 value) << 32 | member index -- so that rank_i = #{j: key_j < key_i}: one shared-memory
+      // load and one 64-bit compare per (i, j), ties and the rank-major index arithmetic folded into the key.
       auto count = [&](const float* vals, int32_t* ranks_out, bool second) {
         __syncthreads();                                     // the previous column's keys are no longer read
         for (int q = tid; q < p.P; q += kThreads)
-          s_key[q] = ((uint64_t)image(__ldg(vals + q)) << 32) | (uint32_t)(p.world > 1 ? member_of(q) : q);
+          s_key[q] = ((uint64_t)rank_image(__ldg(vals + q)) << 32) | (uint32_t)(p.world > 1 ? member_of(q) : q);
         __syncthreads();
         for (int i = gwarp; i < p.P; i += nwarps) {
           const uint64_t ki = s_key[p.world > 1 ? pos_of(i) : i];
@@ -296,38 +352,15 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
       count(p.returns, p.ranks_out, false);
       if (p.novelty) count(p.novelty, p.ranks2_out, true);   // the same lane 0 wrote cvals[i] just above
     } else {
-      auto before = [](float a, float b) { return (a < b) || (a == a && b != b); };
-      auto same = [](float a, float b) { return (a == b) || (a != a && b != b); };
-      for (int i = gwarp; i < p.P; i += nwarps) {
-        const int pi = p.world > 1 ? pos_of(i) : i;
-        const float ri = __ldg(p.returns + pi);
-        int cnt = 0;
-        for (int j = lane; j < p.P; j += 32) {
-          const float rj = __ldg(p.returns + j);
-          cnt += before(rj, ri);
-          if (same(rj, ri)) cnt += (p.world > 1 ? member_of(j) : j) < i;   // ties are rare
-        }
-        cnt = warp_sum_i(cnt);
-        int cnt2 = 0;
-        if (p.novelty) {
-          const float qi = __ldg(p.novelty + pi);
-          for (int j = lane; j < p.P; j += 32) {
-            const float qj = __ldg(p.novelty + j);
-            cnt2 += before(qj, qi);
-            if (same(qj, qi)) cnt2 += (p.world > 1 ? member_of(j) : j) < i;
-          }
-          cnt2 = warp_sum_i(cnt2);
-        }
-        if (lane == 0) {
-          float c = centre(cnt, p.P);
-          if (p.novelty) {
-            c = __fadd_rn(__fmul_rn(p.w_rew, c), __fmul_rn(p.w_nov, centre(cnt2, p.P)));
-            if (p.ranks2_out) p.ranks2_out[i] = cnt2;
-          }
-          p.cvals[i] = c;
-          if (p.ranks_out) p.ranks_out[i] = cnt;
-        }
-      }
+      // P > 8192: a stable grid-wide radix sort (sort_ranks)
+      uint32_t* s_sort = reinterpret_cast<uint32_t*>(s_key_raw);
+      const estk_sort::Workspace& w = p.sort;
+      sort_ranks<kThreads>(p.returns, p.ranks_out, p.cvals, p.w_rew, p.w_nov, false, p.P, p.world, w.keys[0],
+                           w.keys[1], w.vals[0], w.vals[1], w.hist, w.total, s_sort);
+      if (p.novelty)
+        sort_ranks<kThreads>(p.novelty, p.ranks2_out, p.cvals, p.w_rew, p.w_nov, true, p.P, p.world, w.keys[0],
+                             w.keys[1], w.vals[0], w.vals[1], w.hist, w.total, s_sort);
+      (void)gwarp; (void)nwarps; (void)member_of;
     }
   }
   __threadfence();
@@ -588,7 +621,7 @@ template <int NC, int T, int LOADS = 8, bool T16 = false, bool XR = false>
 int launch_rank_grad(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
   constexpr int kThreads = T;
   int occ = 0;
-  constexpr size_t kKeyBytesMax = 64 * 1024;             // P <= 8192 (BASELINE config 3); larger: global-memory path
+  constexpr size_t kKeyBytesMax = 64 * 1024;             // P <= 8192 (BASELINE config 3); larger: radix sort
   static bool attr_set[64] = {};                         // per device: one process may drive several GPUs
   const int dev = ctx->device & 63;
   if (!attr_set[dev]) {
@@ -596,8 +629,9 @@ int launch_rank_grad(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
                                    (int)kKeyBytesMax));
     attr_set[dev] = true;
   }
-  const size_t key_bytes = (size_t)p.P * 8 <= kKeyBytesMax ? (size_t)p.P * 8 : 0;
-  p.keys_in_smem = key_bytes ? 1 : 0;
+  const bool sort = (size_t)p.P * 8 > kKeyBytesMax;
+  const size_t key_bytes = sort ? 0 : (size_t)p.P * 8;
+  // the geometry (hence the fp32 summation order) is the count kernel's at P > 8192 as well
   ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rank_grad_kernel<NC, T, LOADS, T16, XR>, kThreads, key_bytes));
   if (occ < 1) {
     estk_set_error("rank_grad_kernel<%d> cannot be resident", NC);
@@ -625,7 +659,23 @@ int launch_rank_grad(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
   }
   const int grid = p.CS * p.PS;
   void* args[] = {(void*)&p};
-  ESTK_CUDA(cudaLaunchCooperativeKernel((void*)rank_grad_kernel<NC, T, LOADS, T16, XR>, dim3(grid), dim3(kThreads), args, key_bytes, stream));
+  if (!sort) {
+    ESTK_CUDA(cudaLaunchCooperativeKernel((void*)rank_grad_kernel<NC, T, LOADS, T16, XR>, dim3(grid), dim3(kThreads), args,
+                                          key_bytes, stream));
+    return ESTK_OK;
+  }
+  constexpr size_t kSortBytes = estk_sort::smem_bytes(kThreads);
+  int occ_sort = 0;
+  ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_sort, rank_grad_kernel<NC, T, LOADS, T16, XR, true>,
+                                                          kThreads, kSortBytes));
+  if (occ_sort < occ) {
+    estk_set_error("rank_grad_kernel<%d> (sorting ranks): %d CTAs per SM resident, the geometry needs %d", NC,
+                   occ_sort, occ);
+    return ESTK_ERR_CUDA;
+  }
+  p.sort = estk_sort::workspace_of(ctx);
+  ESTK_CUDA(cudaLaunchCooperativeKernel((void*)rank_grad_kernel<NC, T, LOADS, T16, XR, true>, dim3(grid), dim3(kThreads),
+                                        args, kSortBytes, stream));
   return ESTK_OK;
 }
 
@@ -633,7 +683,7 @@ int launch_rank_grad(estk_ctx* ctx, RankGradParams& p, cudaStream_t stream) {
 int init_common(RankGradParams& p, estk_ctx* ctx, const float* returns, const float* novelty, float w_rew,
                 float w_nov, int P, int world, const float* table, const uint16_t* table16, const int64_t* offsets,
                 const int32_t* order, int pair_begin, int pairs_local, int64_t n, int32_t* ranks_out,
-                int32_t* ranks2_out, const char* who) {
+                int32_t* ranks2_out, cudaStream_t stream, const char* who) {
   ESTK_CHECK_ARG(ctx && returns && offsets, "%s: null argument", who);
   ESTK_CHECK_ARG((table == nullptr) != (table16 == nullptr), "%s: exactly one of table / table16 must be given", who);
   ESTK_CHECK_ARG(P >= 2 && (P % 2) == 0 && P <= ESTK_MAX_POPULATION,
@@ -644,6 +694,8 @@ int init_common(RankGradParams& p, estk_ctx* ctx, const float* returns, const fl
   ESTK_CHECK_ARG(world >= 1 && (P / 2) % world == 0, "%s: world=%d does not divide %d pairs", who, world, P / 2);
   ESTK_CHECK_ARG(pair_begin >= 0 && pairs_local > 0 && pair_begin + pairs_local <= P / 2,
                  "%s: local pairs [%d,+%d) outside %d", who, pair_begin, pairs_local, P / 2);
+  const int rc = estk_ctx_reserve(ctx, P, 0, stream, who);
+  if (rc) return rc;
   p = {};
   p.returns = returns; p.novelty = novelty; p.w_rew = w_rew; p.w_nov = w_nov;
   p.P = P; p.pairs = P / 2; p.pair_begin = pair_begin; p.pairs_local = pairs_local;
@@ -694,7 +746,7 @@ extern "C" int estk_rank_grad_adam(estk_ctx* ctx, const float* returns, const fl
   const char* who = "estk_rank_grad_adam";
   RankGradParams p;
   int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, 1, table, table16, offsets, order, 0, P / 2, n,
-                       ranks_out, ranks2_out, who);
+                       ranks_out, ranks2_out, (cudaStream_t)stream, who);
   if (!rc) rc = init_adam(p, theta, m, v, state, adam, grad_out, who);
   return rc ? rc : dispatch(ctx, p, (cudaStream_t)stream);
 }
@@ -706,7 +758,8 @@ extern "C" int estk_rank_grad(estk_ctx* ctx, const float* returns, const float* 
                               int32_t* ranks_out, int32_t* ranks2_out, void* stream) {
   RankGradParams p;
   const int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, world, table, table16, offsets, order,
-                             pair_begin, pairs_local, n, ranks_out, ranks2_out, "estk_rank_grad");
+                             pair_begin, pairs_local, n, ranks_out, ranks2_out, (cudaStream_t)stream,
+                             "estk_rank_grad");
   if (rc) return rc;
   ESTK_CHECK_ARG(grad_sum_out && ESTK_ALIGNED16(grad_sum_out), "estk_rank_grad: grad_sum_out null or unaligned");
   p.fused_adam = 0; p.grad_sum_out = grad_sum_out;
@@ -729,7 +782,7 @@ extern "C" int estk_rank_grad_xr_adam(estk_ctx* ctx, const float* returns, const
   ESTK_CHECK_ARG(peer_ws != nullptr, "%s: null peer_ws", who);
   RankGradParams p;
   int rc = init_common(p, ctx, returns, novelty, w_rew, w_nov, P, world, nullptr, table16, offsets, order,
-                       pair_begin, pairs_local, n, ranks_out, ranks2_out, who);
+                       pair_begin, pairs_local, n, ranks_out, ranks2_out, (cudaStream_t)stream, who);
   if (!rc) rc = init_adam(p, theta, m, v, state, adam, grad_out, who);
   if (rc) return rc;
   p.xr = world; p.xr_rank = rank;
@@ -755,7 +808,7 @@ extern "C" int estk_clamp_adam(estk_ctx* ctx, const float* grad_sum, int32_t P, 
   p.grad_out = grad_out; p.theta = theta; p.m = m; p.v = v; p.state = state; p.adam = *adam;
   int blocks = (int)((n + 255) / 256);
   if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-  clamp_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, ctx->counters + ESTK_MAX_POPULATION);
+  clamp_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, ctx->counters + kTicketClampAdam);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
 }

@@ -37,6 +37,7 @@ from typing import Optional
 import numpy as np
 import torch
 
+from ._capi import ESTK_MAX_POPULATION
 from .agents import DeviceAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import ConvVBNSpec, conv_vbn_spec_from_module, mlp_spec_from_module
@@ -231,6 +232,12 @@ class ES:
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
                         ``bf16s`` additionally reads bf16 shadows of theta and the table);
                         MLP policies only.
+    Population size: any even value up to ``ESTK_MAX_POPULATION`` (2**22); larger values raise
+    ``ValueError`` here.  Device memory that grows with P: the returns (4 B per member), ranks
+    (4 B), offsets and evaluation order (12 B per pair), the library workspace (about 20 B per
+    member beyond 32768, plus the evaluate partials, 4 B per member and observation chunk), and for
+    the NS family the behaviour characteristics, ``P * bc_dim`` floats (1 GB at P = 2**20,
+    bc_dim = 256).  Hooks mode (host agents) still rolls out one member at a time on the host.
     Attributes as documented at estorch.py:108-117.
     """
 
@@ -245,6 +252,9 @@ class ES:
         assert not (self.population_size % self.n_workers)           # estorch.py:130
         if self.population_size % 2 or self.population_size < 2:
             raise ValueError("population_size must be even (mirrored sampling, estorch.py:190)")
+        if self.population_size > ESTK_MAX_POPULATION:
+            raise ValueError(f"population_size {self.population_size} exceeds the engine's limit of "
+                             f"{ESTK_MAX_POPULATION} members (ESTK_MAX_POPULATION)")
         if (self.population_size // 2) % self.n_workers:
             raise ValueError("population_size/2 antithetic pairs must divide evenly over the GPUs")
         self.device = torch.device(device)

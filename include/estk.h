@@ -15,9 +15,19 @@
  *   - all buffers are CALLER-OWNED DEVICE pointers (fp32 / int32 / int64,
  *     contiguous, 16-byte aligned) unless a parameter says "host";
  *   - every launch is asynchronous on the caller's stream (`stream` is a
- *     cudaStream_t passed as void*); the library never synchronises;
+ *     cudaStream_t passed as void*); the library does not synchronise, except
+ *     that a call which grows the context workspace (below) waits on `stream`
+ *     for the new buffers' zero fill;
  *   - the library keeps no global mutable state: one estk_ctx per device
- *     holds an opaque workspace (partial sums, centred-rank scratch).
+ *     holds an opaque workspace (partial sums, centred-rank scratch, sort
+ *     buffers).  It is sized for 32768 members at estk_ctx_create; an entry
+ *     point that needs more grows it first, and returns ESTK_ERR_NOMEM instead
+ *     when its stream is being captured into a CUDA graph -- run a
+ *     configuration once before capturing it.  The buffers a growth replaces
+ *     stay allocated until estk_ctx_destroy, so graphs captured earlier replay
+ *     correctly (after 16 growths of one context the library waits for the
+ *     device and frees them: re-capture graphs after that many); if the new
+ *     allocation fails the context keeps its old buffers.
  *
  * Member / pair layout (estorch.py:190-193): population_size P = 2*pairs;
  * member j < pairs is theta + sigma*T[off_j : off_j+n], member j+pairs is
@@ -40,7 +50,7 @@ extern "C" {
 
 #define ESTK_VERSION 200          /* 0.2.0 */
 #define ESTK_MAX_LAYERS 8
-#define ESTK_MAX_POPULATION 32768 /* P; rank phase is O(P^2) */
+#define ESTK_MAX_POPULATION (1 << 22) /* P: 4,194,304 members */
 
 typedef enum {
   ESTK_OK = 0,
@@ -128,7 +138,9 @@ ESTK_API int estk_fill_noise_table(estk_ctx* ctx, float* table, int64_t len, uin
  * replayed from a CUDA graph passes a constant gen_host -- 0, or 1 while the previous
  * generation's estk_track_best is still folded into this one -- and never a host scalar).  order_out (nullable, int32
  * [pairs]) receives the local pair indices sorted by offset (ties by index):
- * evaluating / reducing pairs in that order lets overlapping table rows hit L2. */
+ * evaluating / reducing pairs in that order lets overlapping table rows hit L2.
+ * pairs <= ESTK_MAX_POPULATION/2; table_len < 2^40.  Up to 4096 pairs one CTA sorts; more
+ * take one cooperative grid-wide radix sort (workspace in the context). */
 ESTK_API int estk_make_offsets(estk_ctx* ctx, uint64_t seed, const estk_state* state, int64_t gen_host,
                       int64_t pair_begin, int32_t pairs, int64_t table_len, int64_t n,
                       int64_t* offsets_out, int32_t* order_out, void* stream);
@@ -267,7 +279,9 @@ ESTK_API int estk_track_best(estk_ctx* ctx, estk_state* state, const float* rewa
  *   returns [P] (reward column), novelty [P] or NULL.  Blend row c = w_rew*c(reward) +
  *   w_nov*c(novelty) in fp32 when novelty is given (ES: novelty NULL -> c(reward)).  Ranks are
  *   bit-exact vs _compute_ranks on tie-free input (ties: stable by member index; NaN returns sort
- *   last like numpy's argsort, among themselves by index); centring in fp64 then fp32 as
+ *   last like numpy's argsort, among themselves by index; -0 ties with +0) for any P <= ESTK_MAX_POPULATION:
+ *   P <= 8192 by an all-pairs count in shared memory, larger P by a grid-wide stable radix sort in
+ *   the same launch (one launch per call either way); centring in fp64 then fp32 as
  *   estorch.py:17-19,:176.  The gradient estimate is
  *     g = (1/P) * sum_j (c_j - c_{j+pairs}) * T[off_j : off_j+n]
  *   over pair j's offset offsets[j] (order, nullable = reduction order from estk_make_offsets).
