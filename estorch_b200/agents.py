@@ -6,7 +6,9 @@ Arbitrary Python rollouts cannot run inside a kernel, so the device path needs
 an agent that *declares* its computation:
 
 ``DeviceAgent`` -- rollout is "run the policy over a fixed observation batch
-and reduce": ``return = -mean((policy(obs) - target)**2)`` and (NS family)
+and reduce": ``return = -mean((policy(obs) - target)**2)`` (``loss="mse"``) or the
+soft-target cross-entropy ``return = mean_b sum_c target_bc * log_softmax(policy(obs))_bc``
+(``loss="cross_entropy"``: the policy's output is the logits) and (NS family)
 ``bc = policy(obs[:bc_obs]).flatten()[:bc_dim]`` (the 256-float behaviour
 characteristic shape of examples/nsra_es.py:45-49).  It still implements the
 reference protocol (``rollout``) with plain torch, so the very same object
@@ -24,14 +26,29 @@ from typing import Optional, Tuple
 import torch
 
 
-class DeviceAgent:
-    """Batch-regression agent evaluated by the fused CUDA kernel."""
+LOSSES = ("mse", "cross_entropy")
 
-    def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0):
+
+class DeviceAgent:
+    """Batch-regression or batch-classification agent evaluated by the fused CUDA kernel.
+
+    ``loss="mse"`` (default): the return is minus the mean squared error against ``target``.
+    ``loss="cross_entropy"``: ``target`` is ``[B, C]`` class weights per observation (one-hot or
+    soft labels, finite and >= 0) and the return is minus the mean over the batch of the
+    cross-entropy between those weights and the softmax of the policy's output."""
+
+    def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0, *,
+                 loss: str = "mse"):
         if obs.dim() < 2 or target.dim() != 2 or obs.shape[0] != target.shape[0]:
             raise ValueError("obs must be [B, in] (or [B, C, H, W] for conv policies) and target [B, out]")
+        if loss not in LOSSES:
+            raise ValueError(f"loss must be one of {LOSSES}, got {loss!r}")
         self.obs = obs.detach().to(torch.float32).contiguous()
         self.target = target.detach().to(torch.float32).contiguous()
+        if loss == "cross_entropy" and not (target.is_floating_point() and bool(torch.isfinite(self.target).all())
+                                            and bool((self.target >= 0).all())):
+            raise ValueError("loss='cross_entropy' needs target class weights that are finite and >= 0")
+        self.loss = loss
         self.bc_obs = int(bc_obs)
         self.bc_dim = int(bc_dim)
         if bool(self.bc_obs) != bool(self.bc_dim):
@@ -42,7 +59,11 @@ class DeviceAgent:
         with torch.no_grad():
             p = next(policy.parameters())
             out = policy(self.obs.to(p.device))
-            reward = float(-((out - self.target.to(p.device)) ** 2).mean())
+            tgt = self.target.to(p.device)
+            if self.loss == "cross_entropy":
+                reward = float((tgt * torch.log_softmax(out, 1)).sum(1).mean())
+            else:
+                reward = float(-((out - tgt) ** 2).mean())
             if self.bc_dim:
                 bc = out[:self.bc_obs].flatten()[:self.bc_dim].detach().cpu().numpy().copy()
                 return reward, bc

@@ -6,7 +6,8 @@
 //   ES._calculate_returns    estorch/estorch.py:195-202   vector_to_parameters + rollout per row
 //   Policy.forward           examples/cartpole_es.py:14-20 (Linear-ReLU-Linear-ReLU-Linear; or Tanh
 //                            hidden and / or output activations, estk.h ESTK_ACT_*)
-//   Agent.rollout            synthetic agent of SURVEY 8d: -mean((policy(obs)-y)^2)
+//   Agent.rollout            synthetic agent of SURVEY 8d: -mean((policy(obs)-y)^2), or the
+//                            soft-target cross-entropy (ESTK_LOSS_XENT)
 //                            (+ behaviour characteristic, examples/nsra_es.py:45-49)
 //
 // One CTA = one antithetic pair x one chunk of BC observations.  The pair's
@@ -16,7 +17,8 @@
 // into the + and - activation rows.  Activations stay in shared memory across
 // layers (k-major [width][ROWS], ROWS = 2*BC rows = sign-major), register tile
 // 4 rows x 4 outputs per thread.  The last layer is fused with the squared
-// error; chunk partial sums are combined in fixed order by the last-arriving
+// error; with the cross-entropy it writes the logits to shared memory like a hidden
+// layer, and one thread per row then reduces its row in column order.  Chunk partial sums are combined in fixed order by the last-arriving
 // chunk CTA (deterministic, no float atomics).
 //
 // This is the exact-fp32 path used for parity and for small policies; algorithmic
@@ -48,11 +50,12 @@ struct EvalParams {
   unsigned int* counters;  // [pairs], zero on entry, zero on exit
 };
 
-// ACT = estk_mlp_desc.activation (a compile-time constant, so the ReLU instantiations are
-// the code they were before Tanh existed)
+// ACT = estk_mlp_desc.activation (a compile-time constant, so the ReLU / squared-error
+// instantiations are the code they were before Tanh and the cross-entropy existed)
 template <int ROWS, int ACT>
 __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) {
   constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   constexpr int OT = 4096 / ROWS;  // output features per tile
   constexpr int OTP = OT + 4;      // padded row of the weight tile (keeps float4 alignment)
   constexpr int TC = OT / 4;       // thread columns
@@ -151,6 +154,16 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
 #pragma unroll
           for (int i = 0; i < 4; ++i) y[i] = HID_TANH ? tanhf(y[i]) : fmaxf(y[i], 0.f);
           *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
+        } else if constexpr (XENT) {
+          // the logits stay in shared memory for the row pass below
+          *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
+          float* bc = minus ? p.bc_minus : p.bc_plus;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int b = b0 + ((r0 + i) % BC);
+            const int64_t e = (int64_t)b * out + o;
+            if (bc && b < p.B && b < p.bc_obs && e < p.bc_dim) bc[(size_t)j * p.bc_dim + e] = y[i];
+          }
         } else {
           if constexpr (OUT_TANH) {
 #pragma unroll
@@ -176,10 +189,31 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
     pbase = bbase + out;
   }
 
-  // ---- block reduction of the squared error, per sign
+  // ---- cross-entropy: thread r < ROWS reduces row r of the logits (now in X) in column order
+  if constexpr (XENT) {
+    __syncthreads();
+    const int C = p.desc.dims[L];
+    const int b = b0 + (tid % BC);
+    if (tid < ROWS && b < p.B) {
+      const float* t = p.target + (size_t)b * C;
+      float m = -INFINITY;
+      for (int c = 0; c < C; ++c) m = fmaxf(m, X[(size_t)c * ROWS + tid]);
+      float s = 0.f, st = 0.f, sty = 0.f;
+      for (int c = 0; c < C; ++c) {
+        const float y = X[(size_t)c * ROWS + tid], tv = __ldg(t + c);
+        s += expf(y - m);
+        st += tv;
+        sty = fmaf(tv, y, sty);
+      }
+      loss = fmaf(m + logf(s), st, -sty);
+    }
+  }
+
+  // ---- block reduction of the loss, per sign
   {
-    const float lp = warp_sum_f(minus ? 0.f : loss);
-    const float lm = warp_sum_f(minus ? loss : 0.f);
+    const bool lminus = XENT ? tid >= BC : minus;   // cross-entropy: the sign of row tid
+    const float lp = warp_sum_f(lminus ? 0.f : loss);
+    const float lm = warp_sum_f(lminus ? loss : 0.f);
     if ((tid & 31) == 0) { s_red[0][tid >> 5] = lp; s_red[1][tid >> 5] = lm; }
     __syncthreads();
     if (tid == 0) {
@@ -198,7 +232,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
       const float* part = p.partial + ((size_t)slot * 2) * p.chunks;
       float sp = 0.f, sm = 0.f;
       for (int c = 0; c < p.chunks; ++c) { sp += __ldcg(part + c); sm += __ldcg(part + p.chunks + c); }
-      const float denom = (float)p.B * (float)p.desc.dims[L];
+      const float denom = XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L];
       p.ret_plus[j] = -(sp / denom);
       if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
       p.counters[slot] = 0u;  // ready for the next launch
@@ -225,6 +259,8 @@ int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
     case ESTK_ACT_TANH: return launch_act<ROWS, ESTK_ACT_TANH>(p, smem, stream);
     case ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_OUT_TANH>(p, smem, stream);
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, smem, stream);
+    case ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_LOSS_XENT>(p, smem, stream);
+    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_act<ROWS, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, smem, stream);
     default: return launch_act<ROWS, ESTK_ACT_RELU>(p, smem, stream);
   }
 }
@@ -248,6 +284,8 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
   if (smem_bytes(32, maxw) > budget) budget = 200 * 1024;
   int rows = 256;
   while (rows > 32 && (smem_bytes(rows, maxw) > budget || rows / 2 >= 2 * p.B)) rows >>= 1;
+  // 16 rows (8 observations) only where 32 do not fit: input widths up to ~1500, e.g. 784 (28 x 28 images)
+  if (smem_bytes(rows, maxw) > budget) rows = 16;
   if (smem_bytes(rows, maxw) > budget) {
     estk_set_error("%s: layer width %d does not fit the fp32 shared-memory path", who, maxw);
     return ESTK_ERR_UNSUPPORTED;
@@ -264,7 +302,8 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
     case 256: return launch<256>(p, smem, stream);
     case 128: return launch<128>(p, smem, stream);
     case 64: return launch<64>(p, smem, stream);
-    default: return launch<32>(p, smem, stream);
+    case 32: return launch<32>(p, smem, stream);
+    default: return launch<16>(p, smem, stream);
   }
 }
 

@@ -20,7 +20,10 @@
 //      consumer warpgroups take alternate N tiles); the epilogue adds the bias,
 //      applies the hidden activation (ReLU, or tanhf in fp32) and rounds to 16 bits straight into
 //      the other activation buffer.  The last layer is fused with the optional output tanhf (fp32),
-//      the squared-error reduction and the behaviour characterisation.
+//      the squared-error reduction and the behaviour characterisation; with the cross-entropy
+//      (ESTK_LOSS_XENT) each thread carries an online softmax of its two rows over its columns
+//      (running max, rescaled sum of exponentials, sum t*y, sum t) from tile to tile, and the
+//      warpgroup that drains the last tile combines the four lanes of each quad.
 // Operand modes (template MODE):
 //   kModeBF16   bf16 operands formed from fp32 theta + fp32 table (one FMA in fp32, one rounding)
 //   kModeBF16S  bf16 operands formed from bf16 shadows of theta and table (fma.rn.bf16x2)
@@ -74,6 +77,8 @@ static_assert(kProdGroups <= kStages, "parity waits need kProdGroups <= kStages"
 // 16-byte items per producer thread per stage: the CTA's quarter of the widest tile, in one batch
 constexpr int kItemsPT = kTileN / kCluster * (kBlockK / 8) / kPT;
 constexpr int kTgtBatch = 2;                       // last-layer epilogue: column blocks per target batch
+constexpr int kTgtBatchX = 1;                      // the same with the cross-entropy (its 8-float chain
+                                                   // state spills at 2 in the bf16 mode)
 constexpr int kModeBF16 = 0, kModeBF16S = 1, kModeF16 = 2;
 
 // ESTK_PREC_* -> operand mode; -1 for a precision without a tensor-core kernel
@@ -140,12 +145,14 @@ __device__ __forceinline__ TaskId decode_task(const EvalTCParams& p, int task, b
   return t;
 }
 
-// ACT = estk_mlp_desc.activation, a compile-time constant: the ReLU / identity instantiations are
-// the code they were before Tanh existed, and no epilogue carries a branch on the activation.
+// ACT = estk_mlp_desc.activation, a compile-time constant: the ReLU / identity / squared-error
+// instantiations are the code they were before Tanh and the cross-entropy existed, and no epilogue
+// carries a branch on the activation or the loss.
 template <int MODE, int ACT>
 __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTCParams p) {
   constexpr bool S16 = (MODE == kModeBF16S), F16 = (MODE == kModeF16);
   constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sH = smem;                                  // 2 activation buffers x 8 k-blocks x 8 KB
@@ -155,6 +162,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   uint64_t* bar_empty = bar_full + kStages;                             // [kStages] stage consumed
   float* s_loss = reinterpret_cast<float*>(bar_empty + kStages);        // [4]
   float* s_chain = s_loss + 4;                                          // [128] loss chain handoff
+                                                                        // ([8][128] with the cross-entropy)
   __shared__ Layer lay[ESTK_MAX_LAYERS];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -300,7 +308,96 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           fence_acc(d);
           if (lane < kCluster) mbar_arrive_cluster(mapa_shared(smem_u32(bar_empty + prev), lane));
           // ---- epilogue of the tile
-          if (last) {
+          if (XENT && last) {
+            // Cross-entropy.  Per thread and row h (r0 + 8h): first this tile's max, sum t*y and sum t
+            // over the thread's columns, with d turned into the logits; then the sum of exp(y - max).
+            float tm[2] = {-INFINITY, -INFINITY}, tsty[2] = {0.f, 0.f}, tst[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jg = 0; jg < kTileN / 8; jg += kTgtBatchX) {
+              float2 t[kTgtBatchX][2];
+#pragma unroll
+              for (int jb = jg; jb < jg + kTgtBatchX; ++jb)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                  if (jb * 8 < width)
+                    t[jb - jg][h] = __ldg(reinterpret_cast<const float2*>(
+                        p.target + (size_t)(chunk * kRows + r0 + 8 * h) * N + n0 + jb * 8 + cq));
+#pragma unroll
+              for (int jb = jg; jb < jg + kTgtBatchX; ++jb) {
+                if (jb * 8 < width) {
+                  const int col = n0 + jb * 8 + cq;
+                  const float2 bv = *reinterpret_cast<const float2*>(bias + col);
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    const int b = chunk * kRows + r0 + 8 * h;
+                    const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                    d[jb * 4 + 2 * h] = y0;
+                    d[jb * 4 + 2 * h + 1] = y1;
+                    tm[h] = fmaxf(fmaxf(tm[h], y0), y1);
+                    tsty[h] = fmaf(t[jb - jg][h].y, y1, fmaf(t[jb - jg][h].x, y0, tsty[h]));
+                    tst[h] = (tst[h] + t[jb - jg][h].x) + t[jb - jg][h].y;
+                    if (with_bc && b < p.bc_obs) {
+                      float* bc = sgn ? p.bc_minus : p.bc_plus;
+                      const int64_t idx = (int64_t)b * N + col;
+                      if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
+                      if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
+                    }
+                  }
+                }
+              }
+            }
+            float ts[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jb = 0; jb < kTileN / 8; ++jb)
+              if (jb * 8 < width)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                  ts[h] = (ts[h] + expf(d[jb * 4 + 2 * h] - tm[h])) + expf(d[jb * 4 + 2 * h + 1] - tm[h]);
+            // the chain (max, sum exp, sum t*y, sum t) continues from the previous tile, which the
+            // other warpgroup drained; thread tid of both warpgroups holds the same rows and columns
+            if (n0 > 0) {
+              ESTK_PROF(kPrDrain);
+              named_bar_sync(kBarLoss + cw, kConsThreads);
+              ESTK_PROF(kPrOther);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float cm = s_chain[(4 * h) * 128 + tid], nm = fmaxf(cm, tm[h]);
+                ts[h] = s_chain[(4 * h + 1) * 128 + tid] * expf(cm - nm) + ts[h] * expf(tm[h] - nm);
+                tm[h] = nm;
+                tsty[h] = s_chain[(4 * h + 2) * 128 + tid] + tsty[h];
+                tst[h] = s_chain[(4 * h + 3) * 128 + tid] + tst[h];
+              }
+            }
+            if (!last_tile) {                // hand the chain to the warpgroup of the next tile
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                s_chain[(4 * h) * 128 + tid] = tm[h];
+                s_chain[(4 * h + 1) * 128 + tid] = ts[h];
+                s_chain[(4 * h + 2) * 128 + tid] = tsty[h];
+                s_chain[(4 * h + 3) * 128 + tid] = tst[h];
+              }
+              named_bar_arrive(kBarLoss + (cw ^ 1), kConsThreads);
+            } else {
+              // the row's four lanes (the quad) hold disjoint columns: combine them, lane distance 1
+              // then 2, and form ce once per row on the quad's first lane
+#pragma unroll
+              for (int o = 1; o <= 2; o <<= 1)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const float om = __shfl_xor_sync(0xffffffffu, tm[h], o);
+                  const float os = __shfl_xor_sync(0xffffffffu, ts[h], o);
+                  const float osty = __shfl_xor_sync(0xffffffffu, tsty[h], o);
+                  const float ost = __shfl_xor_sync(0xffffffffu, tst[h], o);
+                  const float nm = fmaxf(tm[h], om);
+                  ts[h] = ts[h] * expf(tm[h] - nm) + os * expf(om - nm);
+                  tm[h] = nm;
+                  tsty[h] += osty;
+                  tst[h] += ost;
+                }
+              if ((lane & 3) == 0)
+                loss = fmaf(tm[0] + logf(ts[0]), tst[0], -tsty[0]) + fmaf(tm[1] + logf(ts[1]), tst[1], -tsty[1]);
+            }
+          } else if (last) {
             // the targets of kTgtBatch column blocks are loaded before any is used: the behaviour-
             // characterisation stores would otherwise hold each load until the one before returned
 #pragma unroll
@@ -387,7 +484,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           __threadfence();
           float s = 0.f;
           for (int c = 0; c < parts; ++c) s += __ldcg(part + c);
-          const float r = -(s / ((float)p.B * (float)lay[L - 1].N));
+          const float r = XENT ? -(s / (float)p.B) : -(s / ((float)p.B * (float)lay[L - 1].N));
           if (folded) p.centre_out[0] = r;
           else if (sgn) p.ret_minus[j] = r;
           else p.ret_plus[j] = r;
@@ -540,9 +637,10 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   cluster_sync();
 }
 
-size_t tc_smem_bytes() {
+// the cross-entropy's loss chain carries 8 floats per consumer thread instead of 1
+size_t tc_smem_bytes(bool xent) {
   return 1024 + 2 * (size_t)kHBytes + (size_t)kStages * kStageBytes + 2 * kMaxW * sizeof(float) +
-         2 * kStages * sizeof(uint64_t) + (4 + 128) * sizeof(float);
+         2 * kStages * sizeof(uint64_t) + (4 + (xent ? 8 : 1) * 128) * sizeof(float);
 }
 
 // Clusters of kCluster CTAs, one per SM, persistent over groups of kCluster tasks.  The number of
@@ -550,7 +648,7 @@ size_t tc_smem_bytes() {
 // kCluster, so it can be less than sm_count / kCluster.
 template <int MODE, int ACT>
 int launch_tc(const EvalTCParams& p, cudaStream_t stream) {
-  const size_t smem = tc_smem_bytes();
+  const size_t smem = tc_smem_bytes((ACT & ESTK_LOSS_XENT) != 0);
   ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -597,6 +695,8 @@ int launch_tc_act(const EvalTCParams& p, cudaStream_t stream) {
     case ESTK_ACT_TANH: return launch_tc<MODE, ESTK_ACT_TANH>(p, stream);
     case ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_OUT_TANH>(p, stream);
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, stream);
+    case ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_LOSS_XENT>(p, stream);
+    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_tc<MODE, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, stream);
     default: return launch_tc<MODE, ESTK_ACT_RELU>(p, stream);
   }
 }

@@ -37,7 +37,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from ._capi import ESTK_MAX_POPULATION
+from ._capi import ESTK_LOSS_XENT, ESTK_MAX_POPULATION
 from .agents import DeviceAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import ConvVBNSpec, conv_vbn_spec_from_module, mlp_spec_from_module
@@ -228,7 +228,9 @@ class ES:
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
             ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
-                        (ReLU and Tanh MLPs alike; always ``"fp32"`` for the conv policy);
+                        (ReLU and Tanh MLPs alike, with the squared error or the
+                        cross-entropy of ``DeviceAgent(loss=...)``; always ``"fp32"`` for
+                        the conv policy);
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
                         ``bf16s`` additionally reads bf16 shadows of theta and the table);
                         MLP policies only.
@@ -290,7 +292,7 @@ class ES:
             self._precision = "f16"
         if self._fused and not self._is_conv and eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
-            act_kw = {"act": self._spec.act} if self._spec.act else {}     # ReLU: the backends' default
+            act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
             supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
                                                                           **act_kw)
             if eval_precision != "auto" and not supported:
@@ -365,6 +367,8 @@ class ES:
             return False
         if getattr(self, "k", 0) > 32:          # estk_knn_novelty's per-lane top-k buffer; the reference accepts
             return False                        # any k (estorch.py:413) -> hooks mode (host novelty) serves it
+        if getattr(self.agent, "loss", "mse") == "cross_entropy" and (self._is_conv or self._spec.output != "identity"):
+            return False                        # the softmax is the output map: identity-output MLPs only
         if self._is_conv:
             if self._ALGORITHM_TYPE != _Algorithm.classic:      # no behaviour characteristic on the conv kernel yet
                 return False
@@ -794,12 +798,17 @@ class ES:
             kw["table16"] = self._table_h if self._precision == "f16" else self._table16
         return kw
 
+    def _act_code(self):
+        """``estk_mlp_desc.activation`` of the MLP evaluate: the policy's activations (include/estk.h
+        ESTK_ACT_*) and the agent's loss (ESTK_LOSS_XENT for ``loss="cross_entropy"``)."""
+        return self._spec.act | (ESTK_LOSS_XENT if getattr(self.agent, "loss", "mse") == "cross_entropy" else 0)
+
     def _mlp_kw(self, slot, centre=False):
-        """``_eval_kw`` plus the MLP policy's activation code (include/estk.h ESTK_ACT_*).  It is
-        left out for ReLU hidden + identity output, the default of every backend."""
+        """``_eval_kw`` plus the code of ``_act_code``.  It is left out for ReLU hidden + identity
+        output + squared error, the default of every backend."""
         kw = self._eval_kw(slot, centre)
-        if self._spec.act:
-            kw["act"] = self._spec.act
+        if self._act_code():
+            kw["act"] = self._act_code()
         return kw
 
     _streaming = False          # the agent hands a new observation batch to every generation

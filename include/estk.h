@@ -79,12 +79,24 @@ typedef struct {
  * parameter vector in torch.nn.utils.parameters_to_vector order (weight [out,in]
  * row-major, then bias, per layer) -- examples/cartpole_es.py:6-20.
  *
- * `activation` is two bit fields:
+ * `activation` is three bit fields:
  *   bits 0-7   hidden activation, applied after every Linear but the last:
  *              ESTK_ACT_RELU (0) max(y, 0), ESTK_ACT_TANH (1) tanh(y);
  *   bits 8-15  output activation, applied after the last Linear, before the squared
- *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y).
- * 0 is ReLU hidden + identity output.  Any other value is ESTK_ERR_INVALID in
+ *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y);
+ *   bits 16-23 the loss, i.e. what a member's return is:
+ *              0 the squared error, return = -sum_bc (y_bc - t_bc)^2 / (B*C);
+ *              ESTK_LOSS_XENT soft-target cross-entropy on the logits y (the last Linear's
+ *              output, acc + bias), target rows t_b = class weights (one-hot or soft labels):
+ *                m_b = max_c y_bc,  lse_b = m_b + logf(sum_c expf(y_bc - m_b)),
+ *                ce_b = lse_b * sum_c t_bc - sum_c t_bc * y_bc,  return = -sum_b ce_b / B.
+ *              All of it fp32 with IEEE expf / logf, reductions in a fixed order (the same
+ *              bits from run to run); the max shift keeps it finite for finite logits and a
+ *              NaN logit gives a NaN return.  The behaviour characteristic stays the logits.
+ *              Valid with the identity output only (the softmax is the output map).
+ * The defined codes are 0, ESTK_ACT_TANH, ESTK_ACT_OUT_TANH, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH,
+ * ESTK_LOSS_XENT and ESTK_LOSS_XENT | ESTK_ACT_TANH.
+ * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
  * and makes estk_eval_mlp_supported return 0.
  * Arithmetic of tanh: IEEE tanhf (libdevice, ~1-2 ulp, no tanh.approx) on the fp32
@@ -94,6 +106,7 @@ typedef struct {
 #define ESTK_ACT_RELU 0
 #define ESTK_ACT_TANH 1
 #define ESTK_ACT_OUT_TANH (1 << 8)
+#define ESTK_LOSS_XENT (1 << 16)
 
 /* Arithmetic of the evaluate kernels (estk_eval_mlp, estk_eval_conv_vbn); what each one
  * computes is stated at those functions. */
