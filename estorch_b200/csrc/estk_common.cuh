@@ -41,7 +41,7 @@ static inline bool estk_act_valid(int a) {
 }
 
 // ---------------------------------------------------------------- context
-static const int kCtxMaxRetired = 64;
+static const int kCtxMaxRetired = 80;   // 16 growths of the 5 workspace buffers
 // The per-member buffers are sized for kCtxInitialMembers at estk_ctx_create and grown by
 // estk_ctx_reserve when a call needs more (a population beyond that, or a wider evaluate).
 struct estk_ctx {
@@ -51,9 +51,11 @@ struct estk_ctx {
   int max_grid;            // sm_count * 8: upper bound on any persistent grid
   int64_t members;         // capacity of cvals / counters / sort_ws, in members
   int64_t eval_floats;     // capacity of eval_partial, in floats
+  int64_t slab_floats;     // capacity of eval_slab, in floats (0 until a streamed evaluate needs it)
   float* cvals;            // [members] blended centred ranks (fp32)
   float* partial;          // [max_grid * 1024] split-over-pairs partial sums
   float* eval_partial;     // [eval_floats] loss partials of the evaluate kernels
+  float* eval_slab;        // [slab_floats] per-CTA activations of the streamed fp32 evaluate
   unsigned int* counters;  // [kCtxTicketSlots + members]: kernel tickets, then self-resetting arrival counters
   void* sort_ws;           // estk_sort::workspace_bytes(members, 4, max_grid) bytes: radix-sort buffers
   double* scalars;         // [8] small fp64 scratch (||archive||_F, ...)
@@ -68,12 +70,14 @@ static const int kTicketClampAdam = 0;
 static const int kTicketTrackBest = 1;
 static inline unsigned int* estk_member_counters(estk_ctx* c) { return c->counters + kCtxTicketSlots; }
 
-// Grows the context workspace to at least `members` members (cvals, arrival counters, sort buffers)
-// and `eval_floats` evaluate partials; no-op when it is large enough.  Growth allocates new buffers and
-// waits on `stream` for their zero-filled counters; the old buffers stay allocated until estk_ctx_destroy
-// (graphs captured before keep working), and stay in use if the allocation fails (ESTK_ERR_NOMEM).
+// Grows the context workspace to at least `members` members (cvals, arrival counters, sort buffers),
+// `eval_floats` evaluate partials and `slab_floats` activation-slab floats; no-op when it is large
+// enough.  Growth allocates new buffers and waits on `stream` for their zero-filled counters; the old
+// buffers stay allocated until estk_ctx_destroy (graphs captured before keep working), and stay in use
+// if the allocation fails (ESTK_ERR_NOMEM).
 // Refused with ESTK_ERR_NOMEM while `stream` is being captured into a CUDA graph.
-int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who);
+int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who,
+                     int64_t slab_floats = 0);
 
 // ---------------------------------------------------------------- evaluate back ends
 // estk_eval_mlp and estk_eval_conv_vbn check their arguments once, then hand the call to the

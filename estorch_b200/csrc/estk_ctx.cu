@@ -21,24 +21,27 @@ static void free_workspace(estk_ctx* c) {
   cudaFree(c->eval_partial);
   cudaFree(c->counters);
   cudaFree(c->sort_ws);
-  c->cvals = c->eval_partial = nullptr;
+  cudaFree(c->eval_slab);
+  c->cvals = c->eval_partial = c->eval_slab = nullptr;
   c->counters = nullptr;
   c->sort_ws = nullptr;
-  c->members = c->eval_floats = 0;
+  c->members = c->eval_floats = c->slab_floats = 0;
 }
 
-// The per-member buffers for `members` members and `eval_floats` evaluate partials, into `c`; the arrival
-// counters are zero-filled on `stream` (every kernel that takes one leaves it at zero again).  On failure
-// whatever was allocated is freed again and `c`'s buffers are null.
-static cudaError_t alloc_workspace(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream) {
+// The per-member buffers for `members` members, `eval_floats` evaluate partials and `slab_floats` slab
+// floats (none when 0), into `c`; the arrival counters are zero-filled on `stream` (every kernel that takes
+// one leaves it at zero again).  On failure whatever was allocated is freed again and `c`'s buffers are null.
+static cudaError_t alloc_workspace(estk_ctx* c, int64_t members, int64_t eval_floats, int64_t slab_floats,
+                                   cudaStream_t stream) {
   const size_t counters = sizeof(unsigned int) * (size_t)(kCtxTicketSlots + members);
-  c->cvals = c->eval_partial = nullptr;
+  c->cvals = c->eval_partial = c->eval_slab = nullptr;
   c->counters = nullptr;
   c->sort_ws = nullptr;
   cudaError_t e = cudaMalloc(&c->cvals, sizeof(float) * (size_t)members);
   if (e == cudaSuccess) e = cudaMalloc(&c->eval_partial, sizeof(float) * (size_t)eval_floats);
   if (e == cudaSuccess) e = cudaMalloc(&c->counters, counters);
   if (e == cudaSuccess) e = cudaMalloc(&c->sort_ws, estk_sort::workspace_bytes(members, 4, c->max_grid));
+  if (e == cudaSuccess && slab_floats > 0) e = cudaMalloc(&c->eval_slab, sizeof(float) * (size_t)slab_floats);
   if (e == cudaSuccess) e = cudaMemsetAsync(c->counters, 0, counters, stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);   // zero before any launch on any stream
   if (e != cudaSuccess) {
@@ -47,12 +50,14 @@ static cudaError_t alloc_workspace(estk_ctx* c, int64_t members, int64_t eval_fl
   }
   c->members = members;
   c->eval_floats = eval_floats;
+  c->slab_floats = slab_floats;
   return e;
 }
 
 // Buffers replaced by a growth stay allocated until estk_ctx_destroy: a CUDA graph captured before the
 // growth still points at them, and replaying it must not touch freed memory.
 static void retire(estk_ctx* c, void* ptr) {
+  if (!ptr) return;
   if (c->n_retired == kCtxMaxRetired) {
     // (only after kCtxMaxRetired / 4 growths of one context) nothing in flight may still use them
     cudaDeviceSynchronize();
@@ -86,7 +91,7 @@ extern "C" int estk_ctx_create(int device, estk_ctx** out) {
   c->max_grid = c->sm_count * 8;
   cudaError_t e = cudaMalloc(&c->partial, sizeof(float) * (size_t)c->max_grid * 1024);
   if (e == cudaSuccess) e = cudaMalloc(&c->scalars, sizeof(double) * 8);
-  if (e == cudaSuccess) e = alloc_workspace(c, kCtxInitialMembers, kCtxInitialMembers * 2 * kEvalMaxChunks, 0);
+  if (e == cudaSuccess) e = alloc_workspace(c, kCtxInitialMembers, kCtxInitialMembers * 2 * kEvalMaxChunks, 0, 0);
   if (e != cudaSuccess) {
     estk_set_error("estk_ctx_create: workspace allocation failed: %s", cudaGetErrorString(e));
     estk_ctx_destroy(c);
@@ -106,43 +111,50 @@ extern "C" int estk_ctx_destroy(estk_ctx* c) {
   return ESTK_OK;
 }
 
-int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who) {
-  if (members <= c->members && eval_floats <= c->eval_floats) return ESTK_OK;
+int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who,
+                     int64_t slab_floats) {
+  if (members <= c->members && eval_floats <= c->eval_floats && slab_floats <= c->slab_floats) return ESTK_OK;
   cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
   ESTK_CUDA(cudaStreamIsCapturing(stream, &capture));
   if (capture != cudaStreamCaptureStatusNone) {
-    estk_set_error("%s: the context workspace must grow (%lld members, %lld evaluate partials; it holds %lld, %lld), "
-                   "which is not possible while the stream is captured into a CUDA graph: run the same call once "
-                   "before capturing it", who, (long long)members, (long long)eval_floats, (long long)c->members,
-                   (long long)c->eval_floats);
+    estk_set_error("%s: the context workspace must grow (%lld members, %lld evaluate partials, %lld slab floats; it "
+                   "holds %lld, %lld, %lld), which is not possible while the stream is captured into a CUDA graph: "
+                   "run the same call once before capturing it", who, (long long)members, (long long)eval_floats,
+                   (long long)slab_floats, (long long)c->members, (long long)c->eval_floats,
+                   (long long)c->slab_floats);
     return ESTK_ERR_NOMEM;
   }
   if (members < c->members) members = c->members;
   if (eval_floats < c->eval_floats) eval_floats = c->eval_floats;
+  if (slab_floats < c->slab_floats) slab_floats = c->slab_floats;
   members = (members + 1023) / 1024 * 1024;
   int prev = 0;
   ESTK_CUDA(cudaGetDevice(&prev));
   ESTK_CUDA(cudaSetDevice(c->device));
   // the new buffers first: on failure the context keeps the ones it has
   estk_ctx grown = *c;
-  const cudaError_t e = alloc_workspace(&grown, members, eval_floats, stream);
+  const cudaError_t e = alloc_workspace(&grown, members, eval_floats, slab_floats, stream);
   cudaSetDevice(prev);
   if (e != cudaSuccess) {
     cudaGetLastError();   // an allocation failure is not sticky: clear it for the caller's next launch
-    estk_set_error("%s: growing the context workspace to %lld members, %lld evaluate partials failed: %s", who,
-                   (long long)members, (long long)eval_floats, cudaGetErrorString(e));
+    estk_set_error("%s: growing the context workspace to %lld members, %lld evaluate partials, %lld slab floats "
+                   "failed: %s", who, (long long)members, (long long)eval_floats, (long long)slab_floats,
+                   cudaGetErrorString(e));
     return ESTK_ERR_NOMEM;
   }
   retire(c, c->cvals);
   retire(c, c->eval_partial);
   retire(c, c->counters);
   retire(c, c->sort_ws);
+  retire(c, c->eval_slab);
   c->cvals = grown.cvals;
   c->eval_partial = grown.eval_partial;
   c->counters = grown.counters;
   c->sort_ws = grown.sort_ws;
+  c->eval_slab = grown.eval_slab;
   c->members = grown.members;
   c->eval_floats = grown.eval_floats;
+  c->slab_floats = grown.slab_floats;
   return ESTK_OK;
 }
 

@@ -24,6 +24,7 @@
 // This is the exact-fp32 path used for parity and for small policies; algorithmic
 // bytes per launch = 4*n*pairs (noise rows) + 4*n (theta) + 4*B*(in+out) + 4*P.
 #include "estk_common.cuh"
+#include <algorithm>
 
 namespace {
 
@@ -265,6 +266,268 @@ int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
   }
 }
 
+// ---------------------------------------------------------------- streamed kernel
+// eval_mlp_wide_kernel: the shapes eval_mlp_kernel cannot hold -- a layer too wide for 16 rows of
+// activations in shared memory, or a batch of more than kEvalMaxChunks chunks.  Persistent CTAs loop
+// over work items (pair slot, chunk of kWideBC observations); both signs share one read of the noise row.
+// Hidden activations (and the logits of the cross-entropy) live in a per-CTA slab in global memory,
+// [width][kWideRows] per buffer, two buffers that alternate by layer; layer 0 reads obs directly.  Each
+// layer is an N-tiled (kWideOT outputs), K-chunked (kWideKT) product: the X chunk is copied into shared
+// memory with cp.async, W+ / W- are formed in shared memory from theta and the table (loaded into
+// registers one chunk ahead), both double-buffered so one barrier per chunk separates the stages.
+// Thread tile: 4 rows x 8 outputs.  The per-element arithmetic is eval_mlp_kernel's.
+constexpr int kWideRows = 128;                               // 64 observations x 2 signs
+constexpr int kWideBC = kWideRows / 2;
+constexpr int kWideOT = 64;
+constexpr int kWideOTP = kWideOT + 4;
+constexpr int kWideKT = 32;
+constexpr int kWideWPer = kWideOT * kWideKT / kThreads;      // weights each thread forms per chunk
+constexpr size_t kWideSmem = sizeof(float) * (2 * kWideKT * kWideRows + 2 * 2 * kWideKT * kWideOTP);
+
+__device__ __forceinline__ void cp_async4(float* dst, const float* src, bool full) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"((unsigned)__cvta_generic_to_shared(dst)),
+               "l"(src), "r"(full ? 4 : 0) : "memory");
+}
+// L2 only: the slab is written by this CTA's threads, never through the read-only path
+__device__ __forceinline__ void cp_async16(float* dst, const float* src, bool full) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"((unsigned)__cvta_generic_to_shared(dst)),
+               "l"(src), "r"(full ? 16 : 0) : "memory");
+}
+
+// slab: [gridDim.x][2][slab_w][kWideRows]; p.partial [pairs][2][chunks]
+template <int ACT>
+__global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalParams p, float* const slab,
+                                                                    const int slab_w) {
+  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
+  constexpr int ROWS = kWideRows, BC = kWideBC, OT = kWideOT, OTP = kWideOTP, KT = kWideKT;
+  extern __shared__ __align__(16) float smem[];
+  float* const Xs = smem;                     // [2][KT][ROWS]; layer 0 fills the first BC rows only
+  float* const Ws = Xs + 2 * KT * ROWS;       // [2][sign][KT][OTP]
+  __shared__ float s_red[2][kThreads / 32];
+
+  const int tid = threadIdx.x;
+  const int tc = tid % 8, r0 = (tid / 8) * 4;    // outputs tc*4 + {0..3} and 32 + tc*4 + {0..3}
+  const bool minus = r0 >= BC;                   // all 4 rows share the sign
+  const bool centre = (p.offsets == nullptr);
+  const float sigma = centre ? 0.f : p.sigma;
+  const int L = p.desc.n_layers;
+  float* const act0 = slab + (size_t)blockIdx.x * 2 * slab_w * ROWS;
+  float* const act1 = act0 + (size_t)slab_w * ROWS;
+  const int64_t items = (int64_t)p.pairs * p.chunks;
+
+  for (int64_t item = blockIdx.x; item < items; item += gridDim.x) {
+    const int slot = (int)(item / p.chunks);
+    const int chunk = (int)(item % p.chunks);
+    const int j = p.order ? p.order[slot] : slot;
+    const float* trow = centre ? p.theta : p.table + p.offsets[j];
+    const int b0 = chunk * BC;
+    float loss = 0.f;
+    int64_t pbase = 0;
+
+    for (int l = 0; l < L; ++l) {
+      const int in = p.desc.dims[l], out = p.desc.dims[l + 1];
+      const int64_t wbase = pbase, bbase = pbase + (int64_t)in * out;
+      const bool last = (l == L - 1);
+      const float* xin = (l & 1) ? act0 : act1;     // layer l-1's output
+      float* const yout = (l & 1) ? act1 : act0;
+      const int xr = (l == 0 && minus) ? r0 - BC : r0;   // layer 0: one copy of the observations serves both signs
+      const int nk = (in + KT - 1) / KT;
+      for (int o0 = 0; o0 < out; o0 += OT) {
+        float th[kWideWPer], tv[kWideWPer];
+        // chunk kc of X -> Xs[kc & 1] (zero past `in` and past B), of theta / noise -> th, tv (zero outside)
+        auto stage = [&](int kc) {
+          const int k0 = kc * KT;
+          float* dst = Xs + (kc & 1) * KT * ROWS;
+          if (l == 0) {
+            for (int e = tid; e < KT * BC; e += kThreads) {
+              const int b = e % BC, k = e / BC;
+              const bool ok = b0 + b < p.B && k0 + k < in;
+              cp_async4(dst + k * ROWS + b, ok ? p.obs + (size_t)(b0 + b) * in + k0 + k : p.obs, ok);
+            }
+          } else {
+            for (int e = tid; e < KT * ROWS / 4; e += kThreads) {
+              const int k = e / (ROWS / 4), r = (e % (ROWS / 4)) * 4;
+              const bool ok = k0 + k < in;
+              cp_async16(dst + k * ROWS + r, ok ? xin + (size_t)(k0 + k) * ROWS + r : xin, ok);
+            }
+          }
+          asm volatile("cp.async.commit_group;" ::: "memory");
+#pragma unroll
+          for (int i = 0; i < kWideWPer; ++i) {
+            const int e = tid + i * kThreads, k = e % KT, o = e / KT;
+            th[i] = tv[i] = 0.f;
+            if (o0 + o < out && k0 + k < in) {
+              const int64_t idx = wbase + (int64_t)(o0 + o) * in + k0 + k;
+              th[i] = __ldg(p.theta + idx);
+              tv[i] = ld_noise1(trow + idx);
+            }
+          }
+        };
+        float acc[4][8];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int c = 0; c < 8; ++c) acc[i][c] = 0.f;
+        __syncthreads();   // the previous tile's readers of Xs / Ws are done, the previous layer's slab written
+        stage(0);
+        for (int kc = 0; kc < nk; ++kc) {
+          float* const Wb = Ws + (kc & 1) * 2 * KT * OTP;
+#pragma unroll
+          for (int i = 0; i < kWideWPer; ++i) {
+            const int e = tid + i * kThreads, k = e % KT, o = e / KT;
+            const float ep = __fmul_rn(sigma, tv[i]);
+            Wb[k * OTP + o] = __fadd_rn(th[i], ep);
+            Wb[KT * OTP + k * OTP + o] = __fsub_rn(th[i], ep);
+          }
+          asm volatile("cp.async.wait_all;" ::: "memory");
+          __syncthreads();   // chunk kc staged and formed; chunk kc-1 consumed by every thread
+          if (kc + 1 < nk) stage(kc + 1);
+          const float* X = Xs + (kc & 1) * KT * ROWS + xr;
+          const float* W = Wb + (minus ? KT * OTP : 0) + tc * 4;
+#pragma unroll 8
+          for (int k = 0; k < KT; ++k) {
+            const float4 x = *reinterpret_cast<const float4*>(X + k * ROWS);
+            const float4 wa = *reinterpret_cast<const float4*>(W + k * OTP);
+            const float4 wb = *reinterpret_cast<const float4*>(W + k * OTP + 32);
+            const float xv[4] = {x.x, x.y, x.z, x.w};
+            const float wv[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+              for (int c = 0; c < 8; ++c) acc[i][c] = fmaf(xv[i], wv[c], acc[i][c]);
+          }
+        }
+        // ---- tile epilogue: as eval_mlp_kernel's, into the slab
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          const int o = o0 + (c >> 2) * 32 + tc * 4 + (c & 3);
+          if (o >= out) continue;
+          const float th0 = __ldg(p.theta + bbase + o);
+          const float ep = __fmul_rn(sigma, ld_noise1(trow + bbase + o));
+          const float bias = minus ? __fsub_rn(th0, ep) : __fadd_rn(th0, ep);
+          float y[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
+          if (!last) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) y[i] = HID_TANH ? tanhf(y[i]) : fmaxf(y[i], 0.f);
+            *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
+          } else if constexpr (XENT) {
+            *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
+            float* bc = minus ? p.bc_minus : p.bc_plus;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int b = b0 + ((r0 + i) % BC);
+              const int64_t e = (int64_t)b * out + o;
+              if (bc && b < p.B && b < p.bc_obs && e < p.bc_dim) bc[(size_t)j * p.bc_dim + e] = y[i];
+            }
+          } else {
+            if constexpr (OUT_TANH) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) y[i] = tanhf(y[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int b = b0 + ((r0 + i) % BC);
+              if (b < p.B) {
+                const float d = y[i] - __ldg(p.target + (size_t)b * out + o);
+                loss = fmaf(d, d, loss);
+                float* bc = minus ? p.bc_minus : p.bc_plus;
+                const int64_t e = (int64_t)b * out + o;
+                if (bc && b < p.bc_obs && e < p.bc_dim) bc[(size_t)j * p.bc_dim + e] = y[i];
+              }
+            }
+          }
+        }
+      }
+      pbase = bbase + out;
+    }
+
+    // ---- cross-entropy: thread r < ROWS reduces row r of the logits (in the slab) in column order
+    if constexpr (XENT) {
+      __syncthreads();
+      const float* Y = ((L - 1) & 1) ? act1 : act0;
+      const int C = p.desc.dims[L];
+      const int b = b0 + (tid % BC);
+      if (tid < ROWS && b < p.B) {
+        const float* t = p.target + (size_t)b * C;
+        float m = -INFINITY;
+        for (int c = 0; c < C; ++c) m = fmaxf(m, __ldcg(Y + (size_t)c * ROWS + tid));
+        float s = 0.f, st = 0.f, sty = 0.f;
+        for (int c = 0; c < C; ++c) {
+          const float y = __ldcg(Y + (size_t)c * ROWS + tid), tv = __ldg(t + c);
+          s += expf(y - m);
+          st += tv;
+          sty = fmaf(tv, y, sty);
+        }
+        loss = fmaf(m + logf(s), st, -sty);
+      }
+    }
+
+    // ---- block reduction of the loss per sign, chunk partials combined in chunk order by the last arrival
+    const bool lminus = XENT ? tid >= BC : minus;
+    const float lp = warp_sum_f(lminus ? 0.f : loss);
+    const float lm = warp_sum_f(lminus ? loss : 0.f);
+    if ((tid & 31) == 0) { s_red[0][tid >> 5] = lp; s_red[1][tid >> 5] = lm; }
+    __syncthreads();
+    if (tid == 0) {   // s_red is written again only after the next item's first barrier
+      float sp = 0.f, sm = 0.f;
+      for (int w = 0; w < kThreads / 32; ++w) { sp += s_red[0][w]; sm += s_red[1][w]; }
+      float* part = p.partial + (size_t)slot * 2 * p.chunks;
+      part[chunk] = sp;
+      part[p.chunks + chunk] = sm;
+      __threadfence();
+      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
+      if (arrived == (unsigned int)p.chunks - 1) {
+        __threadfence();
+        sp = sm = 0.f;
+        for (int c = 0; c < p.chunks; ++c) { sp += __ldcg(part + c); sm += __ldcg(part + p.chunks + c); }
+        const float denom = XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L];
+        p.ret_plus[j] = -(sp / denom);
+        if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
+        p.counters[slot] = 0u;  // ready for the next launch
+      }
+    }
+  }
+}
+
+using WideKernel = void (*)(const EvalParams, float*, int);
+
+WideKernel wide_kernel(int act) {
+  switch (act) {
+    case ESTK_ACT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_TANH>;
+    case ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>;
+    case ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_LOSS_XENT>;
+    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return eval_mlp_wide_kernel<ESTK_LOSS_XENT | ESTK_ACT_TANH>;
+    default: return eval_mlp_wide_kernel<ESTK_ACT_RELU>;
+  }
+}
+
+// The streamed kernel for a checked call: a persistent grid of at most (resident CTAs per SM) x SMs,
+// each with its slab of 2 x (widest hidden layer, or the logits of the cross-entropy) x kWideRows floats.
+int run_wide(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who) {
+  const estk_mlp_desc& d = p.desc;
+  int slab_w = (d.activation & ESTK_LOSS_XENT) ? d.dims[d.n_layers] : 0;
+  for (int l = 1; l < d.n_layers; ++l) slab_w = max(slab_w, d.dims[l]);
+  p.BC = kWideBC;
+  p.chunks = (p.B + kWideBC - 1) / kWideBC;
+  const int64_t items = (int64_t)p.pairs * p.chunks;
+  const WideKernel kern = wide_kernel(d.activation);
+  ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWideSmem));
+  int per_sm = 0;
+  ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kWideSmem));
+  const int grid = (int)std::min<int64_t>(items, (int64_t)ctx->sm_count * std::max(per_sm, 1));
+  const int rc = estk_ctx_reserve(ctx, p.pairs, items * 2, stream, who, (int64_t)grid * 2 * slab_w * kWideRows);
+  if (rc) return rc;
+  p.partial = ctx->eval_partial;
+  p.counters = estk_member_counters(ctx);
+  kern<<<grid, kThreads, kWideSmem, stream>>>(p, ctx->eval_slab, slab_w);
+  ESTK_CUDA(cudaGetLastError());
+  return ESTK_OK;
+}
+
 int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who) {
   const estk_mlp_desc& d = p.desc;
   ESTK_CHECK_ARG(d.n_layers >= 1 && d.n_layers <= ESTK_MAX_LAYERS, "%s: n_layers=%d", who, d.n_layers);
@@ -286,13 +549,11 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
   while (rows > 32 && (smem_bytes(rows, maxw) > budget || rows / 2 >= 2 * p.B)) rows >>= 1;
   // 16 rows (8 observations) only where 32 do not fit: input widths up to ~1500, e.g. 784 (28 x 28 images)
   if (smem_bytes(rows, maxw) > budget) rows = 16;
-  if (smem_bytes(rows, maxw) > budget) {
-    estk_set_error("%s: layer width %d does not fit the fp32 shared-memory path", who, maxw);
-    return ESTK_ERR_UNSUPPORTED;
-  }
+  // what does not fit in shared memory at 16 rows, or needs more than kEvalMaxChunks chunks, streams
+  if (smem_bytes(rows, maxw) > budget) return run_wide(ctx, p, stream, who);
   p.BC = rows / 2;
   p.chunks = (p.B + p.BC - 1) / p.BC;
-  ESTK_CHECK_ARG(p.chunks <= kEvalMaxChunks, "%s: B=%d needs %d chunks > %d", who, p.B, p.chunks, kEvalMaxChunks);
+  if (p.chunks > kEvalMaxChunks) return run_wide(ctx, p, stream, who);
   const int rc = estk_ctx_reserve(ctx, p.pairs, (int64_t)p.pairs * 2 * p.chunks, stream, who);
   if (rc) return rc;
   p.partial = ctx->eval_partial;

@@ -20,7 +20,7 @@
  *     for the new buffers' zero fill;
  *   - the library keeps no global mutable state: one estk_ctx per device
  *     holds an opaque workspace (partial sums, centred-rank scratch, sort
- *     buffers).  It is sized for 32768 members at estk_ctx_create; an entry
+ *     buffers, activation slabs of the wide fp32 evaluate).  It is sized for 32768 members at estk_ctx_create; an entry
  *     point that needs more grows it first, and returns ESTK_ERR_NOMEM instead
  *     when its stream is being captured into a CUDA graph -- run a
  *     configuration once before capturing it.  The buffers a growth replaces
@@ -202,7 +202,11 @@ ESTK_API int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, in
  *
  * precision -- the arithmetic, and the buffers it needs besides theta / obs / target / returns:
  *   ESTK_PREC_FP32   CUDA cores, exact fp32 with the reference's two roundings (eps = sigma*t,
- *                    then theta +- eps).  Population: table.  Any widths that fit in shared memory.
+ *                    then theta +- eps).  Population: table.  Any widths and any B, limited only by
+ *                    device memory: shapes whose activations do not fit in shared memory, or whose
+ *                    batch needs more than 64 observation chunks, stream their hidden activations
+ *                    through a slab in the context workspace (grown like the other buffers above),
+ *                    with the same arithmetic per element and the same bits from run to run.
  *   ESTK_PREC_F16    the default: wgmma with fp16 operands (11-bit significand, the TF32 class)
  *                    and fp32 accumulation.  Every weight is formed in fp32 from the fp32 theta
  *                    and the noise value and rounded ONCE: W16 = rn_f16(theta + s*sigma*T[off+i])
