@@ -26,6 +26,7 @@ ESTK_PREC_FP32 = 0
 ESTK_PREC_F16 = 1
 ESTK_PREC_BF16 = 2
 ESTK_PREC_BF16S = 3
+ESTK_PREC_F16_ANY = 4
 
 
 class EstkState(C.Structure):

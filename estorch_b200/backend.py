@@ -62,7 +62,8 @@ def adam_desc(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, clamp=1.0
 
 # eval_precision -> (ESTK_PREC_* code, dtype of its 16-bit theta16 / table16 buffers)
 _PRECISIONS = {"fp32": (_capi.ESTK_PREC_FP32, None), "f16": (_capi.ESTK_PREC_F16, torch.float16),
-               "bf16": (_capi.ESTK_PREC_BF16, None), "bf16s": (_capi.ESTK_PREC_BF16S, torch.bfloat16)}
+               "bf16": (_capi.ESTK_PREC_BF16, None), "bf16s": (_capi.ESTK_PREC_BF16S, torch.bfloat16),
+               "f16_any": (_capi.ESTK_PREC_F16_ANY, torch.float16)}
 
 
 class CudaBackend:
@@ -165,6 +166,11 @@ class CudaBackend:
         d = mlp_desc(dims, act)
         return bool(self.lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16, int(B)))
 
+    def eval_supports_f16_any(self, dims, B, act=0) -> bool:
+        """``"f16_any"``: the F16 arithmetic for every MLP shape (False only for an invalid code or B < 1)."""
+        d = mlp_desc(dims, act)
+        return bool(self.lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16_ANY, int(B)))
+
     def shadow_f16(self, src, dst, check=True) -> int:
         """dst (float16, same numel) = src; returns how many entries were NOT exactly
         representable (0 for tables made by fill_noise_table).  ``check`` reads the
@@ -202,7 +208,8 @@ class CudaBackend:
             self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
             int(bc_obs), int(bc_dim), self._ptr(centre_out, torch.float32, "centre_out"), self._stream()),
             f"estk_eval_mlp[{precision}]")
-        self.launches += 1
+        # "f16_any" off the cluster kernel's shapes: the observation split, then the streamed kernel
+        self.launches += 2 if precision == "f16_any" and not self.eval_supports_f16(dims, obs.shape[0], act) else 1
 
     def eval_mlp_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
                         precision="fp32", theta16=None, act=0):

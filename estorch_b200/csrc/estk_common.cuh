@@ -105,6 +105,10 @@ struct EvalMlpCall {
   float* centre_out;
 };
 int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);     // estk_eval_mlp_tc.cu
+// ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
+// shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
+int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
+int eval_mlp_tc_stream_supported(const estk_mlp_desc& d, int B, const char** why);
 
 struct EvalConvCall {
   int A, R, B;  // n_actions, ref_batch, batch

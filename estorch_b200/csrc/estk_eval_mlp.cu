@@ -578,9 +578,10 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
                              const float* obs, const float* target, int32_t B, float* returns_plus,
                              float* returns_minus, float* bc_plus, float* bc_minus, int32_t bc_obs, int32_t bc_dim,
                              float* centre_return_out, void* stream) {
-  const bool tc = precision == ESTK_PREC_F16 || precision == ESTK_PREC_BF16 || precision == ESTK_PREC_BF16S;
+  const bool f16 = precision == ESTK_PREC_F16 || precision == ESTK_PREC_F16_ANY;
+  const bool tc = f16 || precision == ESTK_PREC_BF16 || precision == ESTK_PREC_BF16S;
   const bool shadows = precision == ESTK_PREC_BF16S;                 // reads theta16, and table16 as a bf16 shadow
-  const bool t16 = shadows || precision == ESTK_PREC_F16;            // a population reads table16
+  const bool t16 = shadows || f16;                                   // a population reads table16
   const bool centre = offsets == nullptr;
   ESTK_CHECK_ARG(tc || precision == ESTK_PREC_FP32, "estk_eval_mlp: unknown precision %d", precision);
   ESTK_CHECK_ARG(ctx && desc && theta && obs && target && returns_plus && (theta16 || !shadows) &&

@@ -727,15 +727,22 @@ int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who)
 
 }  // namespace
 
-// estk_eval_mlp with a tensor-core precision (estk_eval_mlp.cu has checked the arguments)
+// estk_eval_mlp with a tensor-core precision (estk_eval_mlp.cu has checked the arguments).
+// ESTK_PREC_F16_ANY: this file's kernel in fp16 mode where its shape rule holds, else the streamed kernel.
 int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
+  int precision = c.precision;
+  if (precision == ESTK_PREC_F16_ANY) {
+    const char* why = "";
+    if (!tc_supported(c.desc, c.B, &why, kModeF16)) return eval_mlp_tc_stream(ctx, c, stream);
+    precision = ESTK_PREC_F16;
+  }
   EvalTCParams p = {};
   p.desc = c.desc; p.theta = c.theta; p.table = c.table; p.theta16 = c.theta16; p.table16 = c.table16;
   p.offsets = c.offsets; p.order = c.order;
   p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.target = c.target; p.B = c.B;
   p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
-  p.n_signs = c.offsets ? 2 : 1; p.centre_out = c.centre_out; p.mode = mode_of(c.precision);
+  p.n_signs = c.offsets ? 2 : 1; p.centre_out = c.centre_out; p.mode = mode_of(precision);
   return run_tc(ctx, p, stream, "estk_eval_mlp");
 }
 
@@ -805,6 +812,7 @@ extern "C" ESTK_API int estk_tc_profile(void* buf, int32_t* warps, int32_t* cons
 
 extern "C" int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B) {
   const char* why = "";
+  if (desc && precision == ESTK_PREC_F16_ANY) return eval_mlp_tc_stream_supported(*desc, B, &why);
   const int mode = mode_of(precision);
   return desc && mode >= 0 ? tc_supported(*desc, B, &why, mode) : 0;
 }

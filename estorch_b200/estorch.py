@@ -223,7 +223,12 @@ class ES:
             ``"f16"``   wgmma tensor cores with fp16 operands (11-bit significand, the
                         TF32 class) and fp32 accumulation; every weight is formed in fp32
                         from the fp32 theta and the (exactly 16-bit representable) noise
-                        value and rounded once; observations enter as hi + lo halves;
+                        value and rounded once; observations enter as hi + lo halves.
+                        On an MLP shape outside the cluster kernel's rule (widths not
+                        multiples of 64 / 32 or above 512, B not a multiple of 256, e.g. a
+                        10-class head or a 784-wide input) it selects ``"f16_any"``: the same
+                        arithmetic per element on a streamed wgmma kernel, for any widths and
+                        any batch (no folded post-update rollout there).
                         For the conv + VirtualBatchNorm policy (examples/atari.py) ``"f16"``
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
@@ -295,11 +300,16 @@ class ES:
             act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
             supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
                                                                           **act_kw)
-            if eval_precision != "auto" and not supported:
+            # "f16" where the cluster kernel's shape rule fails: the same arithmetic on the streamed kernel
+            any_shape = (eval_precision == "f16" and not supported and
+                         getattr(self._be, "eval_supports_f16_any", lambda d, b, **_: False)(
+                             self._spec.dims, self.agent.obs.shape[0], **act_kw))
+            if eval_precision != "auto" and not supported and not any_shape:
                 raise ValueError(f"eval_precision={eval_precision!r} needs layer widths that are multiples of 64 "
                                  "(in) / 32 (out), at most 512 (f16: input width at most 256), and a batch that "
                                  "is a multiple of 256")
-            self._precision = ("f16" if eval_precision == "auto" else eval_precision) if supported else "fp32"
+            self._precision = ("f16_any" if any_shape else
+                               ("f16" if eval_precision == "auto" else eval_precision) if supported else "fp32")
 
         # ---- noise table (replicated on every GPU, identical by construction)
         n_pad = (self.n_parameters + 31) // 32 * 32
@@ -771,9 +781,9 @@ class ES:
         return self._table if t is None else t
 
     def _ensure_table16(self):
-        """16-bit table copies of the tensor-core evaluate modes: ``"f16"`` needs the exact
-        fp16 copy, ``"bf16s"`` a rounded bf16 shadow."""
-        if self._precision == "f16":
+        """16-bit table copies of the tensor-core evaluate modes: ``"f16"`` / ``"f16_any"`` need the
+        exact fp16 copy, ``"bf16s"`` a rounded bf16 shadow."""
+        if self._precision in ("f16", "f16_any"):
             if self._exact_table16() is None:
                 raise ValueError("eval_precision='f16' needs a noise table whose entries are exactly "
                                  "fp16-representable; use the engine's own table or eval_precision='fp32'")
@@ -793,9 +803,9 @@ class ES:
                 slot.theta16 = self._be.alloc(slot.n, dtype=torch.bfloat16)
             self._be.shadow_bf16(slot.theta, slot.theta16)
             kw["theta16"] = slot.theta16
-        if self._precision in ("f16", "bf16s") and not centre:
+        if self._precision in ("f16", "f16_any", "bf16s") and not centre:
             self._ensure_table16()
-            kw["table16"] = self._table_h if self._precision == "f16" else self._table16
+            kw["table16"] = self._table16 if self._precision == "bf16s" else self._table_h
         return kw
 
     def _act_code(self):

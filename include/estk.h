@@ -20,7 +20,7 @@
  *     for the new buffers' zero fill;
  *   - the library keeps no global mutable state: one estk_ctx per device
  *     holds an opaque workspace (partial sums, centred-rank scratch, sort
- *     buffers, activation slabs of the wide fp32 evaluate).  It is sized for 32768 members at estk_ctx_create; an entry
+ *     buffers, activation slabs of the streamed fp32 and F16_ANY evaluates).  It is sized for 32768 members at estk_ctx_create; an entry
  *     point that needs more grows it first, and returns ESTK_ERR_NOMEM instead
  *     when its stream is being captured into a CUDA graph -- run a
  *     configuration once before capturing it.  The buffers a growth replaces
@@ -114,6 +114,7 @@ typedef struct {
 #define ESTK_PREC_F16 1    /* tensor cores, fp16 operands formed from fp32 sums (the default) */
 #define ESTK_PREC_BF16 2   /* tensor cores, bf16 operands (opt-in, lower precision) */
 #define ESTK_PREC_BF16S 3  /* tensor cores, bf16 operands from bf16 shadows (opt-in, lower precision) */
+#define ESTK_PREC_F16_ANY 4 /* tensor cores, the F16 arithmetic for every MLP shape (opt-in) */
 typedef struct {
   int32_t n_layers;                  /* number of Linear layers, 1..ESTK_MAX_LAYERS */
   int32_t dims[ESTK_MAX_LAYERS + 1]; /* dims[0] = obs dim, dims[n_layers] = out dim */
@@ -227,11 +228,23 @@ ESTK_API int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, in
  *                    not exactly the one that produced it (estorch.py:177-178 uses the same eps on
  *                    both sides); F16 has no such departure.  Always: theta16.  Population: table,
  *                    table16 (the bf16 shadow of the table).
+ *   ESTK_PREC_F16_ANY  opt-in: the F16 arithmetic above, per element, for every MLP shape FP32 takes
+ *                    (any widths, any B >= 1, limited only by device memory).  Where F16's shape rule
+ *                    below holds it runs F16's kernel, the same launch and the same bits.  Elsewhere a
+ *                    streamed wgmma kernel runs: K is padded with zero weights and activations, rows
+ *                    past B are masked out, hidden activations stream through a slab in the context
+ *                    workspace, and the k-order per accumulator is F16's, so a pre-activation is the
+ *                    same bits as F16's for the same member, row and column.  The streamed kernel
+ *                    takes two launches (the observations' hi / lo split, then the evaluate), has no
+ *                    folded centre (centre_return_out is ESTK_ERR_UNSUPPORTED there, before any
+ *                    launch) and gives the same bits from run to run.  The kernel follows from the
+ *                    shape, never from the caller.  Population: table, table16.
  *   Buffers a precision does not list are not read.
- * Tensor-core precisions (F16, BF16, BF16S): theta, obs, target and the listed table / table16 /
- * theta16 must be 16-byte aligned.  Every layer input width a multiple of 64 in [64,512], every
- * output width a multiple of 32 in [32,512], B a multiple of 256, and for F16 dims[0] <= 256;
- * other shapes are ESTK_ERR_UNSUPPORTED (estk_eval_mlp_supported tells in advance).
+ * Tensor-core precisions (F16, F16_ANY, BF16, BF16S): theta, obs, target and the listed table / table16 /
+ * theta16 must be 16-byte aligned.  F16, BF16 and BF16S: every layer input width a multiple of 64 in
+ * [64,512], every output width a multiple of 32 in [32,512], B a multiple of 256, and for F16
+ * dims[0] <= 256; other shapes are ESTK_ERR_UNSUPPORTED (estk_eval_mlp_supported tells in advance).
+ * F16_ANY: an undefined activation code is ESTK_ERR_UNSUPPORTED.
  * Agreement with FP32 is asserted in tests/test_kernels_gpu.py and tests/test_eval_mlp_act_gpu.py. */
 ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t precision,
                   const float* theta, const uint16_t* theta16,
@@ -244,7 +257,8 @@ ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t pre
 
 /* 1 when the tensor-core `precision` (F16, BF16 or BF16S) can evaluate `desc` at batch B (the
  * shape rules above, and a defined activation code), else 0 -- also for a null desc and for any
- * other precision code. */
+ * other precision code.  F16_ANY: 1 for every desc with 1..ESTK_MAX_LAYERS layers, positive widths
+ * and a defined activation code, at every B >= 1. */
 ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B);
 
 /* ---- conv + VirtualBatchNorm policy of examples/atari.py:14-37 (BASELINE config 5):
