@@ -19,6 +19,9 @@ ESTK_MAX_POPULATION = 1 << 22
 # the loss in bits 16-23 (0: squared error)
 ESTK_ACT_RELU = 0
 ESTK_ACT_TANH = 1
+ESTK_ACT_ELU = 3
+ESTK_ACT_SILU = 4
+ESTK_ACT_LEAKY_RELU = 5
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
 # evaluate precision codes (estk_eval_mlp, estk_eval_conv_vbn)

@@ -33,12 +33,49 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
-// estk_mlp_desc.activation: the six defined codes (hidden ReLU / Tanh x output identity / Tanh with
-// the squared error, and hidden ReLU / Tanh x identity output with the cross-entropy)
+// estk_mlp_desc.activation: the fifteen defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
+// LeakyReLU x output identity / Tanh with the squared error, and x identity output with the cross-entropy)
 static inline bool estk_act_valid(int a) {
-  return a == ESTK_ACT_RELU || a == ESTK_ACT_TANH || a == ESTK_ACT_OUT_TANH || a == (ESTK_ACT_TANH | ESTK_ACT_OUT_TANH) ||
-         a == ESTK_LOSS_XENT || a == (ESTK_LOSS_XENT | ESTK_ACT_TANH);
+  const int h = a & 0xff, rest = a & ~0xff;
+  const bool hidden = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
+                      h == ESTK_ACT_LEAKY_RELU;
+  return hidden && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT);
 }
+
+#ifdef __CUDACC__
+// y / d rounded to nearest-even in fp32 -- the bits of the IEEE divide y / d -- for d >= 1 or d = +inf,
+// without the out-of-line slow path of div.rn.f32 (its calls in the unrolled 64-element epilogue cost
+// the cluster kernel's bf16 consumer spills; the streamed wgmma kernel, at 255 registers, spills with
+// this form instead and keeps div.rn).  r = 1/d to ~2^-52 by two fp64 Newton steps from rcp.approx, then
+// q = y * r in fp64 (relative error < 2^-51) rounded once to fp32.  That rounding is exact: a quotient of
+// two 24-bit floats that is not a float is at least 2^-49 (relative) from every fp32 rounding boundary,
+// and never on one.  d = +inf (y < -88.7 in SiLU) gives y * 0, the IEEE y / inf; NaNs propagate.
+__device__ __forceinline__ float estk_div_rn_ge1(float y, float d) {
+  const double dd = d;
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(dd));
+  r = fma(r, fma(-dd, r, 1.0), r);
+  r = fma(r, fma(-dd, r, 1.0), r);
+  return d == INFINITY ? y * 0.f : __double2float_rn((double)y * r);
+}
+
+// The hidden activation H = activation & 0xff on the fp32 value y = acc + bias (estk.h states the
+// arithmetic).  H is a compile-time constant, so an epilogue carries no branch on it.  CALL_FREE_DIV:
+// SiLU divides with estk_div_rn_ge1 instead of div.rn -- the same bits, another register footprint.
+template <int H, bool CALL_FREE_DIV = false>
+__device__ __forceinline__ float estk_hidden_act(float y) {
+  static_assert(H == ESTK_ACT_RELU || H == ESTK_ACT_TANH || H == ESTK_ACT_ELU || H == ESTK_ACT_SILU ||
+                H == ESTK_ACT_LEAKY_RELU, "undefined hidden activation");
+  if constexpr (H == ESTK_ACT_TANH) return tanhf(y);
+  else if constexpr (H == ESTK_ACT_ELU) return y > 0.f ? y : expm1f(y);
+  else if constexpr (H == ESTK_ACT_SILU) {
+    const float d = 1.0f + expf(-y);
+    return CALL_FREE_DIV ? estk_div_rn_ge1(y, d) : __fdiv_rn(y, d);
+  }
+  else if constexpr (H == ESTK_ACT_LEAKY_RELU) return y > 0.f ? y : y * 0.01f;
+  else return fmaxf(y, 0.f);
+}
+#endif
 
 // ---------------------------------------------------------------- context
 static const int kCtxMaxRetired = 80;   // 16 growths of the 5 workspace buffers

@@ -55,7 +55,8 @@ struct EvalParams {
 // instantiations are the code they were before Tanh and the cross-entropy existed)
 template <int ROWS, int ACT>
 __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) {
-  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr int HID = ACT & 0xff;
+  constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   constexpr int OT = 4096 / ROWS;  // output features per tile
   constexpr int OTP = OT + 4;      // padded row of the weight tile (keeps float4 alignment)
@@ -153,7 +154,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
         for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
         if (!last) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) y[i] = HID_TANH ? tanhf(y[i]) : fmaxf(y[i], 0.f);
+          for (int i = 0; i < 4; ++i) y[i] = estk_hidden_act<HID>(y[i]);
           *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
         } else if constexpr (XENT) {
           // the logits stay in shared memory for the row pass below
@@ -262,6 +263,15 @@ int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, smem, stream);
     case ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_LOSS_XENT>(p, smem, stream);
     case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_act<ROWS, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, smem, stream);
+    case ESTK_ACT_ELU: return launch_act<ROWS, ESTK_ACT_ELU>(p, smem, stream);
+    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>(p, smem, stream);
+    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_LOSS_XENT>(p, smem, stream);
+    case ESTK_ACT_SILU: return launch_act<ROWS, ESTK_ACT_SILU>(p, smem, stream);
+    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>(p, smem, stream);
+    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_LOSS_XENT>(p, smem, stream);
+    case ESTK_ACT_LEAKY_RELU: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU>(p, smem, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, smem, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, smem, stream);
     default: return launch_act<ROWS, ESTK_ACT_RELU>(p, smem, stream);
   }
 }
@@ -298,7 +308,8 @@ __device__ __forceinline__ void cp_async16(float* dst, const float* src, bool fu
 template <int ACT>
 __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalParams p, float* const slab,
                                                                     const int slab_w) {
-  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr int HID = ACT & 0xff;
+  constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   constexpr int ROWS = kWideRows, BC = kWideBC, OT = kWideOT, OTP = kWideOTP, KT = kWideKT;
   extern __shared__ __align__(16) float smem[];
@@ -411,7 +422,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
           for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
           if (!last) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) y[i] = HID_TANH ? tanhf(y[i]) : fmaxf(y[i], 0.f);
+            for (int i = 0; i < 4; ++i) y[i] = estk_hidden_act<HID>(y[i]);
             *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
           } else if constexpr (XENT) {
             *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
@@ -501,6 +512,15 @@ WideKernel wide_kernel(int act) {
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>;
     case ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_LOSS_XENT>;
     case ESTK_LOSS_XENT | ESTK_ACT_TANH: return eval_mlp_wide_kernel<ESTK_LOSS_XENT | ESTK_ACT_TANH>;
+    case ESTK_ACT_ELU: return eval_mlp_wide_kernel<ESTK_ACT_ELU>;
+    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_LOSS_XENT>;
+    case ESTK_ACT_SILU: return eval_mlp_wide_kernel<ESTK_ACT_SILU>;
+    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_LOSS_XENT>;
+    case ESTK_ACT_LEAKY_RELU: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
     default: return eval_mlp_wide_kernel<ESTK_ACT_RELU>;
   }
 }

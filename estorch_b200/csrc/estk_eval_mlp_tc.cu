@@ -151,7 +151,8 @@ __device__ __forceinline__ TaskId decode_task(const EvalTCParams& p, int task, b
 template <int MODE, int ACT>
 __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTCParams p) {
   constexpr bool S16 = (MODE == kModeBF16S), F16 = (MODE == kModeF16);
-  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr int HID = ACT & 0xff;
+  constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -455,9 +456,13 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
                 for (int h = 0; h < 2; ++h) {
                   const int r = r0 + 8 * h;
                   const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
-                  // Tanh: fp32 tanhf, then the one rounding to 16 bits (|tanh| <= 1: satfinite never fires)
+                  // ReLU fused into the conversion; any other kind: fp32 activation, then the one rounding
+                  // to 16 bits (saturating in fp16; |tanh| <= 1, so for Tanh it never fires).  SiLU divides
+                  // without div.rn's out-of-line call, which spills the bf16 consumer.
                   st_shared_u32(h_out + (col >> 6) * kHBlockBytes + sw128_offset(r, (col & 63) >> 3) + (col & 7) * 2,
-                                HID_TANH ? pack16<F16>(tanhf(y0), tanhf(y1)) : pack16_relu<F16>(y0, y1));
+                                HID == ESTK_ACT_RELU ? pack16_relu<F16>(y0, y1)
+                                                     : pack16<F16>(estk_hidden_act<HID, true>(y0),
+                                                                   estk_hidden_act<HID, true>(y1)));
                 }
               }
             }
@@ -697,6 +702,15 @@ int launch_tc_act(const EvalTCParams& p, cudaStream_t stream) {
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, stream);
     case ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_LOSS_XENT>(p, stream);
     case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_tc<MODE, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, stream);
+    case ESTK_ACT_ELU: return launch_tc<MODE, ESTK_ACT_ELU>(p, stream);
+    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>(p, stream);
+    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_LOSS_XENT>(p, stream);
+    case ESTK_ACT_SILU: return launch_tc<MODE, ESTK_ACT_SILU>(p, stream);
+    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>(p, stream);
+    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_LOSS_XENT>(p, stream);
+    case ESTK_ACT_LEAKY_RELU: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU>(p, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, stream);
     default: return launch_tc<MODE, ESTK_ACT_RELU>(p, stream);
   }
 }

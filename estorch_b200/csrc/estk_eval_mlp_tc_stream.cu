@@ -109,7 +109,8 @@ __device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os
 
 template <int ACT>
 __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const StreamParams p) {
-  constexpr bool HID_TANH = (ACT & 0xff) == ESTK_ACT_TANH, OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
+  constexpr int HID = ACT & 0xff;
+  constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -245,7 +246,8 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
               const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
               *reinterpret_cast<uint32_t*>(aout + (size_t)(col >> 6) * kABytes + sw128_offset(r, (col & 63) >> 3) +
                                            (col & 7) * 2) =
-                  HID_TANH ? pack_f16(tanhf(y0), tanhf(y1)) : pack_f16_relu(y0, y1);
+                  HID == ESTK_ACT_RELU ? pack_f16_relu(y0, y1)
+                                       : pack_f16(estk_hidden_act<HID>(y0), estk_hidden_act<HID>(y1));
             }
           }
         } else if constexpr (XENT) {
@@ -359,6 +361,15 @@ StreamKernel stream_kernel(int act) {
     case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>;
     case ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_LOSS_XENT>;
     case ESTK_LOSS_XENT | ESTK_ACT_TANH: return eval_mlp_tc_stream_kernel<ESTK_LOSS_XENT | ESTK_ACT_TANH>;
+    case ESTK_ACT_ELU: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU>;
+    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_LOSS_XENT>;
+    case ESTK_ACT_SILU: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU>;
+    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_LOSS_XENT>;
+    case ESTK_ACT_LEAKY_RELU: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
     default: return eval_mlp_tc_stream_kernel<ESTK_ACT_RELU>;
   }
 }

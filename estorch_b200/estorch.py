@@ -233,7 +233,7 @@ class ES:
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
             ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
-                        (ReLU and Tanh MLPs alike, with the squared error or the
+                        (ReLU, Tanh, ELU, SiLU and LeakyReLU MLPs alike, with the squared error or the
                         cross-entropy of ``DeviceAgent(loss=...)``; always ``"fp32"`` for
                         the conv policy);
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;

@@ -3,8 +3,8 @@
 The reference accepts any ``nn.Module`` class as ``policy`` and runs it on the
 host (estorch.py:136,142,195-202).  The fused evaluate kernel needs the
 architecture, so the module is inspected once: a chain
-``Linear -> act -> ... -> Linear [-> Tanh]`` with ``act`` ReLU or Tanh (the same on
-every hidden layer) whose parameters are registered in forward order
+``Linear -> act -> ... -> Linear [-> Tanh]`` with ``act`` ReLU, Tanh, ELU (alpha 1),
+SiLU or LeakyReLU (slope 0.01), the same on every hidden layer, whose parameters are registered in forward order
 (examples/cartpole_es.py:6-20, examples/nsra_es.py:52-67) becomes an ``MLPSpec``.
 Anything else returns ``None`` and the engine uses the materialising path (rows
 built on the device, rollout on the host).
@@ -18,14 +18,15 @@ import torch
 from torch import nn
 
 
-_HIDDEN_CODES = {"relu": 0, "tanh": 1}          # estk.h ESTK_ACT_RELU / ESTK_ACT_TANH
+# estk.h ESTK_ACT_RELU / _TANH / _ELU / _SILU / _LEAKY_RELU
+_HIDDEN_CODES = {"relu": 0, "tanh": 1, "elu": 3, "silu": 4, "leaky_relu": 5}
 _OUTPUT_CODES = {"identity": 0, "tanh": 1 << 8}  # 0 / ESTK_ACT_OUT_TANH
 
 
 @dataclass(frozen=True)
 class MLPSpec:
     dims: tuple  # (in, h1, ..., out)
-    hidden: str = "relu"        # activation after every Linear but the last: "relu" or "tanh"
+    hidden: str = "relu"        # activation after every Linear but the last: a key of _HIDDEN_CODES
     output: str = "identity"    # after the last Linear: "identity" or "tanh"
 
     @property
@@ -43,12 +44,27 @@ def _leaf_modules(module: nn.Module) -> List[nn.Module]:
     return [m for m in module.modules() if len(list(m.children())) == 0]
 
 
+# the hidden kinds, their module types and the forms the kernels compute (default parameters only:
+# estk_mlp_desc has no field for ELU's alpha or LeakyReLU's slope)
+_F = torch.nn.functional
+_HIDDEN = {"relu": (nn.ReLU, torch.relu), "tanh": (nn.Tanh, torch.tanh), "elu": (nn.ELU, _F.elu),
+           "silu": (nn.SiLU, _F.silu), "leaky_relu": (nn.LeakyReLU, _F.leaky_relu)}
+
+
+def _default_params(m: nn.Module) -> bool:
+    if isinstance(m, nn.ELU):
+        return float(m.alpha) == 1.0
+    if isinstance(m, nn.LeakyReLU):
+        return float(m.negative_slope) == 0.01
+    return True
+
+
 def _chain(x, linears, weights, hidden, output):
     h = x
     for i, (l, (w, b)) in enumerate(zip(linears, weights)):
         h = torch.nn.functional.linear(h, w, b)
         if i + 1 < len(linears):
-            h = torch.relu(h) if hidden == "relu" else torch.tanh(h)
+            h = _HIDDEN[hidden][1](h)
     return torch.tanh(h) if output == "tanh" else h
 
 
@@ -59,15 +75,17 @@ def _matches(y, h) -> bool:
 def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPSpec]:
     """Return the MLPSpec of ``module`` or None.
 
-    Structural test: the leaf modules are only Linear / ReLU / Tanh; every Linear
-    has a bias; widths chain; parameters are registered in layer order.
+    Structural test: the leaf modules are only Linear / ReLU / Tanh / ELU / SiLU /
+    LeakyReLU, ELU with ``alpha == 1`` and LeakyReLU with ``negative_slope == 0.01``;
+    every Linear has a bias; widths chain; parameters are registered in layer order.
     Behavioural test (``probe``): a random batch through the module equals the
     chain evaluated from its flat parameters -- this rejects modules whose
     ``forward`` does something else with the same layers.
 
-    The activations are found by the probe.  A kind (ReLU / Tanh) is a candidate if
-    a leaf module of that type is registered, or if no activation module is (a
-    ``forward`` calling ``torch.relu`` / ``torch.tanh``); the output is identity or,
+    The activations are found by the probe.  A hidden kind is a candidate if a leaf
+    module of its type is registered, or if no activation module is (a ``forward``
+    calling ``torch.relu`` / ``torch.tanh`` / ``F.elu`` / ``F.silu`` / ``F.leaky_relu``,
+    every kind a candidate); the output is identity or,
     when Tanh is a candidate, Tanh.  Every (hidden, output) candidate pair is
     compared with the module's forward under parameters redrawn at a scale that
     keeps each layer's output O(1) (weights N(0, 1/fan_in), biases N(0, 1); the
@@ -78,7 +96,8 @@ def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPS
     """
     leaves = _leaf_modules(module)
     linears = [m for m in leaves if isinstance(m, nn.Linear)]
-    others = [m for m in leaves if not isinstance(m, (nn.Linear, nn.ReLU, nn.Tanh))]
+    acts = tuple(t for t, _ in _HIDDEN.values())
+    others = [m for m in leaves if not isinstance(m, (nn.Linear,) + acts) or not _default_params(m)]
     if not linears or others or len(linears) > 8:
         return None
     if any(l.bias is None for l in linears):
@@ -92,13 +111,13 @@ def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPS
     expect = [p for l in linears for p in (l.weight, l.bias)]
     if len(params) != len(expect) or any(a is not b for a, b in zip(params, expect)):
         return None
-    kinds = [k for k, t in (("relu", nn.ReLU), ("tanh", nn.Tanh)) if any(isinstance(m, t) for m in leaves)]
-    kinds = kinds or ["relu", "tanh"]
+    kinds = [k for k, (t, _) in _HIDDEN.items() if any(isinstance(m, t) for m in leaves)]
+    kinds = kinds or list(_HIDDEN)
     hiddens = kinds if len(linears) > 1 else ["relu"]
     outputs = ["identity"] + (["tanh"] if "tanh" in kinds else [])
     cands = [(h, o) for h in hiddens for o in outputs]
-    if not probe:                       # structure only: a Tanh needs the probe to be placed
-        return None if any(isinstance(m, nn.Tanh) for m in leaves) else MLPSpec(tuple(dims))
+    if not probe:                       # structure only: any activation but ReLU needs the probe to be placed
+        return None if any(isinstance(m, acts) and not isinstance(m, nn.ReLU) for m in leaves) else MLPSpec(tuple(dims))
     with torch.no_grad():
         dev, dt = params[0].device, params[0].dtype
         # the same global-RNG draw as before Tanh was recognised: module initialisations that

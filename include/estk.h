@@ -81,7 +81,12 @@ typedef struct {
  *
  * `activation` is three bit fields:
  *   bits 0-7   hidden activation, applied after every Linear but the last:
- *              ESTK_ACT_RELU (0) max(y, 0), ESTK_ACT_TANH (1) tanh(y);
+ *              ESTK_ACT_RELU (0) max(y, 0), ESTK_ACT_TANH (1) tanh(y),
+ *              ESTK_ACT_ELU (3) y > 0 ? y : expm1(y)             (torch.nn.ELU(), alpha = 1),
+ *              ESTK_ACT_SILU (4) y / (1 + exp(-y))               (torch.nn.SiLU()),
+ *              ESTK_ACT_LEAKY_RELU (5) y > 0 ? y : y * 0.01      (torch.nn.LeakyReLU(), slope 0.01);
+ *              2 and every value above 5 are undefined (2 is kept unassigned: callers have used
+ *              it as the example of a refused code);
  *   bits 8-15  output activation, applied after the last Linear, before the squared
  *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y);
  *   bits 16-23 the loss, i.e. what a member's return is:
@@ -94,17 +99,26 @@ typedef struct {
  *              bits from run to run); the max shift keeps it finite for finite logits and a
  *              NaN logit gives a NaN return.  The behaviour characteristic stays the logits.
  *              Valid with the identity output only (the softmax is the output map).
- * The defined codes are 0, ESTK_ACT_TANH, ESTK_ACT_OUT_TANH, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH,
- * ESTK_LOSS_XENT and ESTK_LOSS_XENT | ESTK_ACT_TANH.
+ * The defined codes are, for each hidden kind h in {ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU,
+ * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH and h | ESTK_LOSS_XENT (15 codes).
  * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
  * and makes estk_eval_mlp_supported return 0.
  * Arithmetic of tanh: IEEE tanhf (libdevice, ~1-2 ulp, no tanh.approx) on the fp32
  * value acc + bias.  fp32 path: the result stays fp32.  Tensor-core paths: a hidden
  * tanh is rounded ONCE to the 16-bit operand type when the activation is written back
- * (|tanh| <= 1, so the fp16 saturation never applies); the output tanh stays fp32. */
+ * (|tanh| <= 1, so the fp16 saturation never applies); the output tanh stays fp32.
+ * Arithmetic of ELU / SiLU / LeakyReLU, on the fp32 value y = acc + bias: ELU y > 0 ? y :
+ * expm1f(y); SiLU y / (1.0f + expf(-y)) with an IEEE divide; LeakyReLU y > 0 ? y : y * 0.01f.
+ * IEEE expf / expm1f only (no __expf): SiLU(-100) = -0, ELU(-100) = -1.  fp32 path: the result
+ * stays fp32.  Tensor-core paths: rounded ONCE to the 16-bit operand type when the activation
+ * is written back, saturating in fp16 as ReLU does (ELU >= -1 and SiLU >= -0.28, so only their
+ * positive side can saturate; LeakyReLU can saturate on both sides). */
 #define ESTK_ACT_RELU 0
 #define ESTK_ACT_TANH 1
+#define ESTK_ACT_ELU 3
+#define ESTK_ACT_SILU 4
+#define ESTK_ACT_LEAKY_RELU 5
 #define ESTK_ACT_OUT_TANH (1 << 8)
 #define ESTK_LOSS_XENT (1 << 16)
 
