@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("ESTK_LIBRARY") or os.path.join(_HERE, "lib", "libestk
 ESTK_MAX_LAYERS = 8
 ESTK_MAX_POPULATION = 1 << 22
 # estk_mlp_desc.activation bit fields: hidden activation in bits 0-7, output activation in bits 8-15,
-# the loss in bits 16-23 (0: squared error)
+# the loss in bits 16-23 (0: squared error; ESTK_ACTIONS: no return, the outputs on each member's own observations)
 ESTK_ACT_RELU = 0
 ESTK_ACT_TANH = 1
 ESTK_ACT_ELU = 3
@@ -24,6 +24,7 @@ ESTK_ACT_SILU = 4
 ESTK_ACT_LEAKY_RELU = 5
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
+ESTK_ACTIONS = 3 << 16
 # evaluate precision codes (estk_eval_mlp, estk_eval_conv_vbn)
 ESTK_PREC_FP32 = 0
 ESTK_PREC_F16 = 1

@@ -77,4 +77,40 @@ class DeviceAgent:
         return None
 
 
+class PopulationAgent:
+    """An environment agent that steps one environment per population member, all members at once.
+
+    Subclasses implement ``rollout_population(act, members)``, which runs ``members`` episodes side by
+    side (environment state, done masks and termination are the agent's own) and returns
+    ``returns[members]``; for the NS family it returns ``(returns[members], bc[members, bc_dim])`` and the
+    subclass declares ``bc_dim`` (a positive int) as an attribute.
+
+    ``act(obs)`` takes a float32 tensor on ``self.device``, shaped ``[members, in]`` or
+    ``[members, B, in]``, and returns the policy outputs, ``[members, out]`` or ``[members, B, out]``.
+    Under ``ES`` in population mode, rows ``< members/2`` are the + members of the local antithetic pairs
+    in pair order and the rest are their mirrors, and every row is evaluated by one fused CUDA launch of
+    every perturbed policy; ``members == 1`` is the unperturbed policy.  ``act`` never synchronises with
+    the device, so an episode loop that keeps its state on the device runs without host round trips.
+
+    ``rollout(policy)`` -- the reference protocol -- is ``rollout_population`` with ``members == 1`` and
+    ``act = policy``, so the same object also runs in hooks mode and under the reference itself.
+    ``device`` is where the agent creates its tensors; ``ES`` sets it to the engine's device in
+    population mode and to the policy's device otherwise."""
+
+    device = torch.device("cpu")
+    bc_dim = 0
+
+    def rollout_population(self, act, members: int):
+        raise NotImplementedError
+
+    def rollout(self, policy):
+        p = next(policy.parameters())
+        with torch.no_grad():
+            res = self.rollout_population(lambda o: policy(o.to(p.device)).to(o.device), 1)
+        if isinstance(res, tuple):
+            ret, bc = res
+            return float(torch.as_tensor(ret).reshape(-1)[0]), torch.as_tensor(bc).reshape(1, -1)[0].cpu().numpy().copy()
+        return float(torch.as_tensor(res).reshape(-1)[0])
+
+
 SyntheticAgent = DeviceAgent

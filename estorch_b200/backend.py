@@ -217,6 +217,30 @@ class CudaBackend:
         self.eval_mlp(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs, bc_dim,
                       precision=precision, theta16=theta16, act=act)
 
+    def act_mlp(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act=0, table16=None):
+        """Every perturbed policy's outputs on its own observations (estk_eval_mlp with ESTK_ACTIONS, fp32).
+        Population: ``obs`` ``[2*pairs, B, in]`` -> ``out`` ``[2*pairs, B, out]``, rows ``< pairs`` the + members
+        of the local pairs, the rest their mirrors.  ``offsets`` None = the centre: ``obs`` / ``out``
+        ``[1, B, ...]`` for theta.  ``act``: the policy's hidden / output code (ESTK_ACTIONS is added here);
+        ``table16``: the exact fp16 copy of ``table``, read instead of it."""
+        M = 1 if offsets is None else 2 * int(pairs)
+        if obs.dim() != 3 or tuple(obs.shape) != (M, obs.shape[1], dims[0]) or \
+                tuple(out.shape) != (M, obs.shape[1], dims[-1]):
+            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match dims {list(dims)} for "
+                             f"{M} members")
+        d = mlp_desc(dims, (int(act) & 0xffff) | _capi.ESTK_ACTIONS)
+        B, per = int(obs.shape[1]), int(obs.shape[1]) * int(dims[-1])
+        t32 = None if table16 is not None else table
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), _capi.ESTK_PREC_FP32, self._ptr(theta, torch.float32, "theta"), None,
+            self._ptr(t32, torch.float32, "table"), self._ptr(table16, torch.float16, "table16"),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+            float(sigma), self._ptr(obs, torch.float32, "obs"), None, B, None, None,
+            self._ptr(out, torch.float32, "out"),
+            None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size()),
+            B, per, None, self._stream()), "estk_eval_mlp[actions]")
+        self.launches += 1
+
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),
                                                              int(B)))

@@ -13,11 +13,16 @@ the body of a generation runs on the GPU through the C ABI in include/estk.h:
     grad scatter/clamp :236-244, Adam.step :245  fused Adam epilogue (or torch optimizer.step)
     _after_optimize :181-185                     estk_eval_mlp (centre, offsets NULL) + estk_track_best
 
-Two execution modes, chosen per instance:
+Three execution modes, chosen per instance:
 
 * fused  -- DeviceAgent + recognised MLP policy + torch.optim.Adam + no hook
             overridden: a generation is a handful of kernel launches, nothing
             touches the host unless the user reads an attribute.
+* population -- PopulationAgent (environments stepped by user code, one per
+            member) + recognised MLP policy + Adam + no hook overridden, on one
+            GPU: every environment step is one launch that evaluates every
+            perturbed policy on its member's own observation (estk_eval_mlp with
+            ESTK_ACTIONS); ranks, gradient and Adam as in fused mode.
 * hooks  -- anything else (host agents such as gym loops, custom subclasses
             overriding ``_sample_policy`` / ``_calculate_grad`` / ..., other
             optimizers): the reference's own control flow through its hooks,
@@ -38,7 +43,7 @@ import numpy as np
 import torch
 
 from ._capi import ESTK_LOSS_XENT, ESTK_MAX_POPULATION
-from .agents import DeviceAgent
+from .agents import DeviceAgent, PopulationAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import ConvVBNSpec, conv_vbn_spec_from_module, mlp_spec_from_module
 from .population import LazyPopulation, NoiseHandle
@@ -287,15 +292,21 @@ class ES:
         self._spec = mlp_spec_from_module(self.target) or conv_vbn_spec_from_module(self.target)
         self._is_conv = isinstance(self._spec, ConvVBNSpec)
         self._fused = self._decide_fused(optimizer)
+        self._population = self._fused and isinstance(self.agent, PopulationAgent)
+        if isinstance(self.agent, PopulationAgent):
+            self.agent.device = self._dev if self._population else self.device
         self._host_cache = {}
         if eval_precision not in ("auto", "fp32", "f16", "bf16", "bf16s"):
             raise ValueError("eval_precision must be 'auto', 'fp32', 'f16', 'bf16' or 'bf16s'")
+        if self._population and eval_precision not in ("auto", "fp32"):
+            raise ValueError("population mode (a PopulationAgent) computes every member's actions in fp32 only: "
+                             "eval_precision must be 'auto' or 'fp32'")
         self._precision = "fp32"
         if self._fused and self._is_conv and eval_precision in ("bf16", "bf16s"):
             raise ValueError("the conv + VirtualBatchNorm evaluate kernel has 'fp32' and 'f16' modes only")
         if self._fused and self._is_conv and eval_precision == "f16":
             self._precision = "f16"
-        if self._fused and not self._is_conv and eval_precision != "fp32":
+        if self._fused and not self._is_conv and not self._population and eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
             act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
             supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
@@ -368,7 +379,12 @@ class ES:
         return not getattr(getattr(type(self), name), "_estk_builtin", False)
 
     def _decide_fused(self, optimizer_cls):
-        if not self._device_agent or self._spec is None:
+        """Fused mode for a DeviceAgent, population mode for a PopulationAgent (an MLP policy on one GPU:
+        the multi-GPU population generation is not implemented, hooks mode serves it)."""
+        population = isinstance(self.agent, PopulationAgent)
+        if not (self._device_agent or population) or self._spec is None:
+            return False
+        if population and (self._is_conv or self.n_workers > 1):
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -377,9 +393,11 @@ class ES:
             return False
         if getattr(self, "k", 0) > 32:          # estk_knn_novelty's per-lane top-k buffer; the reference accepts
             return False                        # any k (estorch.py:413) -> hooks mode (host novelty) serves it
-        if getattr(self.agent, "loss", "mse") == "cross_entropy" and (self._is_conv or self._spec.output != "identity"):
+        if population:
+            pass                                # its episodes are user code: no shape of the agent to check
+        elif getattr(self.agent, "loss", "mse") == "cross_entropy" and (self._is_conv or self._spec.output != "identity"):
             return False                        # the softmax is the output map: identity-output MLPs only
-        if self._is_conv:
+        elif self._is_conv:
             if self._ALGORITHM_TYPE != _Algorithm.classic:      # no behaviour characteristic on the conv kernel yet
                 return False
             if tuple(self.agent.obs.shape[1:]) != (4, 84, 84) or \
@@ -952,6 +970,8 @@ class ES:
         """Run one fused generation: eagerly the first two times a configuration is seen, then
         captured into a CUDA graph and replayed (one launch instead of ~10 + 2 collectives;
         at 8 GPUs the host-side launch cost was 40 % of a generation)."""
+        if self._population:        # the episode loop is host code: nothing to capture
+            return self._population_generation(slot)
         self._peek_batch()
         key = self._graph_key(slot)
         if key is None:
@@ -998,6 +1018,74 @@ class ES:
         self._offsets_gen = self._generation
         self._offsets_all_gen = self._generation if self.n_workers == 1 else None
         self._best_slot = slot
+
+    # ------------------------------------------------------------------ population generation (PopulationAgent)
+    def _population_act(self, slot, centre=False):
+        """The ``act`` handed to ``rollout_population``: observations ``[M, in]`` or ``[M, B, in]`` -> outputs of
+        every member in ONE launch (estk_eval_mlp with ESTK_ACTIONS).  Population: M = P members of the last
+        drawn offsets around ``slot.theta_prev`` (+ members first, then their mirrors); centre: M = 1, theta."""
+        be, dims, dev, code = self._be, self._spec.dims, self._dev, self._spec.act
+        M = 1 if centre else self.population_size
+        t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
+
+        def act(obs):
+            x = torch.as_tensor(obs).to(device=dev, dtype=torch.float32).contiguous()
+            single = x.dim() == 2
+            x3 = x.unsqueeze(1) if single else x
+            if x3.dim() != 3 or x3.shape[0] != M or x3.shape[2] != dims[0]:
+                raise ValueError(f"act: observations {tuple(x.shape)}, expected [{M}, {dims[0]}] or "
+                                 f"[{M}, B, {dims[0]}]")
+            out = torch.empty(M, x3.shape[1], dims[-1], dtype=torch.float32, device=dev)
+            if centre:
+                be.act_mlp(dims, slot.theta, None, None, None, 1, 0.0, x3, out, act=code)
+            else:
+                be.act_mlp(dims, slot.theta_prev, self._table, self._offsets, self._order, self._pairs_local,
+                           self.sigma, x3, out, act=code, table16=t16)
+            return out[:, 0] if single else out
+        return act
+
+    def _population_rollout(self, slot, centre=False):
+        """``rollout_population`` of the agent -> (returns ``[M]``, bc ``[M, bc_dim]`` or None) on the device."""
+        M = 1 if centre else self.population_size
+        res = self.agent.rollout_population(self._population_act(slot, centre), M)
+        ret, bc = res if self._ALGORITHM_TYPE == _Algorithm.novelty else (res, None)
+        ret = torch.as_tensor(ret).to(device=self._dev, dtype=torch.float32).reshape(M)
+        if bc is not None:
+            bc = torch.as_tensor(bc).to(device=self._dev, dtype=torch.float32).reshape(M, -1)
+        return ret, bc
+
+    def _population_centre(self, slot):
+        """theta's rollout into ``self._episode`` (NS family: and its behaviour characteristic into
+        ``self._bc_center[0]``) -- what eval_mlp_center writes in fused mode."""
+        ret, bc = self._population_rollout(slot, centre=True)
+        self._episode.copy_(ret)
+        if bc is not None:
+            self._bc_center.copy_(bc)
+
+    def _population_generation(self, slot):
+        """One generation with a PopulationAgent (one GPU): offsets, the agent's episodes of all P members
+        (every step one fused launch), returns (and novelty) into the member-order buffers, the fused
+        rank + gradient + Adam step, then theta's rollout and the best tracking."""
+        be, pl = self._be, self._pairs_local
+        slot.theta_prev.copy_(slot.theta)
+        self._draw_offsets()
+        self._rm_live = False
+        ret, bc = self._population_rollout(slot)
+        self._returns.copy_(ret)
+        novelty = self._ALGORITHM_TYPE == _Algorithm.novelty
+        if novelty:
+            self._bc.copy_(bc)
+            be.knn_novelty(self._bc[:pl], self._arch_dev, self.k, self._novelty[:pl])
+            be.knn_novelty(self._bc[pl:], self._arch_dev, self.k, self._novelty[pl:])
+            self._update_step(slot, self._returns, self._novelty, np.float32(self._w_rew()),
+                              np.float32(self._w_nov()), False)
+            self._population_centre(slot)
+            self._after_update(slot)
+            return
+        self._update_step(slot, self._returns, None, 1.0, 0.0, False)
+        self._best_slot = slot
+        self._population_centre(slot)
+        be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
 
     def _graph_stream(self):
         if getattr(self, "_gstream", None) is None:
@@ -1324,10 +1412,7 @@ class NS_ES(ES):
     def _rollout_bc(self, policy):
         """Initial archive entry of a meta-population member (estorch.py:405)."""
         if self._fused:
-            slot = self._slots[-1]
-            self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
-                                     self._bc_center[0], self.agent.bc_obs, self.agent.bc_dim,
-                                     **self._mlp_kw(slot, True))
+            self._centre_bc(self._slots[-1])
             return float(self._episode.item()), self._bc_center[0].cpu().numpy().copy()
         with torch.no_grad():
             return self.agent.rollout(policy)
@@ -1381,18 +1466,26 @@ class NS_ES(ES):
         return self.meta_population[self.idx]
 
     # ------------------------------------------------------------------ fused NS generation
+    def _centre_bc(self, slot):
+        """Rollout of ``slot``'s theta: its return into ``self._episode``, its behaviour characteristic into
+        ``self._bc_center[0]`` (the device kernel in fused mode, the agent's episodes in population mode)."""
+        if self._population:
+            return self._population_centre(slot)
+        ag = self.agent
+        self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
+                                 self._bc_center[0], ag.bc_obs, ag.bc_dim, **self._mlp_kw(slot, True))
+
     def _archive_tensor(self):
         return torch.from_numpy(np.ascontiguousarray(np.stack(self._archive), dtype=np.float32)).to(self._dev)
 
     def _select_slot(self):
         """Device version of ``_get_policy``: M centre rollouts + kNN novelty,
         then the reference's ``np.random.choice`` on the host (estorch.py:451-454)."""
-        be, dims = self._be, self._spec.dims
+        be = self._be
         arch = self._archive_tensor()
         nov = []
         for s in self._slots:
-            be.eval_mlp_center(dims, s.theta, self._obs, self._tgt, self._episode, self._bc_center[0],
-                               self.agent.bc_obs, self.agent.bc_dim, **self._mlp_kw(s, True))
+            self._centre_bc(s)
             be.knn_novelty(self._bc_center, arch, self.k, self._nov_center)
             nov.append(self._nov_center.clone())
         total = torch.cat(nov).double().cpu().numpy()
@@ -1431,8 +1524,12 @@ class NS_ES(ES):
         self._update_step(slot, R, N, np.float32(self._w_rew()), np.float32(self._w_nov()), rm)
         # _after_optimize (estorch.py:427-432 / :650-662): rollout of the updated
         # policy, archive append, best tracking, NSRA schedule (host scalars)
-        be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, self._bc_center[0],
-                           ag.bc_obs, ag.bc_dim, **self._mlp_kw(slot, True))
+        self._centre_bc(slot)
+        self._after_update(slot)
+
+    def _after_update(self, slot):
+        """The host side of ``_after_optimize`` once theta's rollout is in ``self._episode`` /
+        ``self._bc_center[0]``: archive append, best tracking, NSRA schedule."""
         episode = float(self._episode.item())
         self._archive.append(self._bc_center[0].cpu().numpy().copy())
         self.episode_reward = episode

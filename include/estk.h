@@ -99,8 +99,29 @@ typedef struct {
  *              bits from run to run); the max shift keeps it finite for finite logits and a
  *              NaN logit gives a NaN return.  The behaviour characteristic stays the logits.
  *              Valid with the identity output only (the softmax is the output map).
+ *              ESTK_ACTIONS: no return at all -- the outputs themselves, on each member's OWN
+ *              observations (one forward of every perturbed policy per environment step):
+ *                population (offsets != NULL): obs is [2*pairs][B][dims[0]]; block j holds the
+ *                observations of the + member of local pair j, block pairs + j those of its - member;
+ *                bc_plus[j] / bc_minus[j] receive policy_m(obs_m[:bc_obs]).flatten()[:bc_dim] (the
+ *                behaviour-characteristic definition above, on the member's own observations);
+ *                centre (offsets == NULL): obs is [B][dims[0]] and bc_plus receives theta's outputs.
+ *              target, returns_plus, returns_minus and centre_return_out are not read (NULL is fine;
+ *              centre_return_out must be NULL); bc_plus (and bc_minus for a population) must be set.
+ *              order keeps its meaning (scheduling only).  table16, when non-null, is read INSTEAD
+ *              of table: it must be the exact fp16 copy (estk_shadow_f16 with inexact_count 0), so
+ *              the values and the bits are the same at half the noise bytes.
+ *              ESTK_PREC_FP32 only (tensor-core precisions are ESTK_ERR_UNSUPPORTED before any
+ *              launch).  Arithmetic: that of the fp32 evaluate -- W = theta +- (sigma*t) with two
+ *              roundings, one fmaf chain per output from 0 in ascending k, + bias, the hidden
+ *              activation, tanhf for ESTK_ACT_OUT_TANH -- so a member's outputs are bit-identical to
+ *              the behaviour characteristic the squared-error fp32 evaluate writes for that member
+ *              when every member is given the same observations.  A member's outputs never depend on
+ *              another member's observations; no float atomics (the same bits from run to run, with
+ *              or without order, from table or table16).  Any widths, any B >= 1.
  * The defined codes are, for each hidden kind h in {ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU,
- * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH and h | ESTK_LOSS_XENT (15 codes).
+ * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH, h | ESTK_LOSS_XENT, h | ESTK_ACTIONS
+ * and h | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (25 codes).  Loss value 2 (0x20000) is undefined.
  * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
  * and makes estk_eval_mlp_supported return 0.
@@ -121,6 +142,7 @@ typedef struct {
 #define ESTK_ACT_LEAKY_RELU 5
 #define ESTK_ACT_OUT_TANH (1 << 8)
 #define ESTK_LOSS_XENT (1 << 16)
+#define ESTK_ACTIONS (3 << 16)
 
 /* Arithmetic of the evaluate kernels (estk_eval_mlp, estk_eval_conv_vbn); what each one
  * computes is stated at those functions. */
@@ -270,9 +292,10 @@ ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t pre
                   float* centre_return_out, void* stream);
 
 /* 1 when the tensor-core `precision` (F16, BF16 or BF16S) can evaluate `desc` at batch B (the
- * shape rules above, and a defined activation code), else 0 -- also for a null desc and for any
- * other precision code.  F16_ANY: 1 for every desc with 1..ESTK_MAX_LAYERS layers, positive widths
- * and a defined activation code, at every B >= 1. */
+ * shape rules above, and a defined activation code that computes a return, i.e. not ESTK_ACTIONS),
+ * else 0 -- also for a null desc and for any other precision code.  F16_ANY: 1 for every desc with
+ * 1..ESTK_MAX_LAYERS layers, positive widths and a defined activation code other than the
+ * ESTK_ACTIONS ones, at every B >= 1. */
 ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B);
 
 /* ---- conv + VirtualBatchNorm policy of examples/atari.py:14-37 (BASELINE config 5):
