@@ -25,6 +25,8 @@ ESTK_ACT_LEAKY_RELU = 5
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
 ESTK_ACTIONS = 3 << 16
+# estk_eval_conv_vbn with n_actions | ESTK_ACTIONS: VBN statistics per member, in floats
+ESTK_CONV_VBN_STATS_FLOATS = 17984
 # evaluate precision codes (estk_eval_mlp, estk_eval_conv_vbn)
 ESTK_PREC_FP32 = 0
 ESTK_PREC_F16 = 1

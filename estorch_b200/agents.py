@@ -87,6 +87,10 @@ class PopulationAgent:
 
     ``act(obs)`` takes a float32 tensor on ``self.device``, shaped ``[members, in]`` or
     ``[members, B, in]``, and returns the policy outputs, ``[members, out]`` or ``[members, B, out]``.
+    For the conv + VirtualBatchNorm policy of the reference's Atari example the observations are stacks of
+    frames, ``[members, 4, 84, 84]`` or ``[members, B, 4, 84, 84]``, and the outputs ``[members, A]`` or
+    ``[members, B, A]``; the members' VBN statistics over the policy's ``xref`` are computed once when
+    ``act`` is built (they depend only on the weights), not on every call as the reference's forward does.
     Under ``ES`` in population mode, rows ``< members/2`` are the + members of the local antithetic pairs
     in pair order and the rest are their mirrors, and every row is evaluated by one fused CUDA launch of
     every perturbed policy; ``members == 1`` is the unperturbed policy.  ``act`` never synchronises with

@@ -262,6 +262,39 @@ class CudaBackend:
             f"estk_eval_conv_vbn[{precision}]")
         self.launches += 1
 
+    def act_conv_vbn(self, n_actions, theta, table, offsets, order, pairs, sigma, xref, obs, out, stats,
+                     table16=None):
+        """The conv + VirtualBatchNorm policy's action mode (estk_eval_conv_vbn with ESTK_ACTIONS, fp32).
+        ``xref`` ``[R, 4, 84, 84]`` (or None): compute every member's VBN statistics into ``stats`` (float32,
+        ``[members, ESTK_CONV_VBN_STATS_FLOATS]``).  ``obs`` (or None): every member's outputs on its own frames
+        from the statistics in ``stats``; population ``obs`` ``[2*pairs, B, 4, 84, 84]`` -> ``out``
+        ``[2*pairs, B, A]`` (rows ``< pairs`` the + members of the local pairs, the rest their mirrors);
+        ``offsets`` None = the centre, ``obs`` / ``out`` ``[1, B, ...]`` for theta.  ``table16``: the exact fp16
+        copy of ``table``, read instead of it."""
+        M = 1 if offsets is None else 2 * int(pairs)
+        A = int(n_actions)
+        if tuple(stats.shape) != (M, _capi.ESTK_CONV_VBN_STATS_FLOATS):
+            raise ValueError(f"stats {tuple(stats.shape)}, expected [{M}, {_capi.ESTK_CONV_VBN_STATS_FLOATS}]")
+        B, per = 1, 0
+        if obs is not None:
+            B = int(obs.shape[1]) if obs.dim() == 5 else -1
+            if obs.dim() != 5 or tuple(obs.shape) != (M, B, 4, 84, 84) or tuple(out.shape) != (M, B, A):
+                raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)}, expected [{M}, B, 4, 84, 84] / "
+                                 f"[{M}, B, {A}]")
+            per = B * A
+        t32 = None if table16 is not None else table
+        _capi.check(self.lib.estk_eval_conv_vbn(
+            self._ctx, _capi.ESTK_PREC_FP32, A | _capi.ESTK_ACTIONS, self._ptr(theta, torch.float32, "theta"),
+            self._ptr(t32, torch.float32, "table"), self._ptr(table16, torch.float16, "table16"),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+            float(sigma), self._ptr(xref, torch.float32, "xref"), 0 if xref is None else int(xref.shape[0]),
+            self._ptr(obs, torch.float32, "obs"), None, B,
+            None if obs is None else self._ptr(out, torch.float32, "out"),
+            None if obs is None or offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * 4),
+            self._ptr(stats, torch.float32, "stats"), stats.numel() * 4, self._stream()),
+            "estk_eval_conv_vbn[actions]")
+        self.launches += (xref is not None) + (obs is not None)
+
     def track_best(self, state, reward, theta, best_theta):
         _capi.check(self.lib.estk_track_best(
             self._ctx, self._ptr(state, torch.uint8, "state"), self._ptr(reward, torch.float32, "reward"),

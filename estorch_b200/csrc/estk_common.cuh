@@ -175,6 +175,12 @@ struct EvalConvCall {
 };
 int64_t eval_conv_tc_scratch_per_cta(int R, int B);                              // estk_eval_conv_tc.cu
 int eval_conv_tc(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream);
+// estk_eval_conv_vbn with n_actions | ESTK_ACTIONS: its own argument checks, then the stats and / or act
+// kernels (estk_act_conv.cu); target is not part of the call, scratch holds the per-member VBN stats
+int eval_conv_actions(estk_ctx* ctx, int precision, int32_t code, const float* theta, const float* table,
+                      const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
+                      const float* xref, int ref_batch, const float* obs, int B, float* returns_plus,
+                      float* returns_minus, void* scratch, int64_t scratch_bytes, cudaStream_t stream);
 
 // ---------------------------------------------------------------- hashing
 // splitmix64 finaliser; must stay in lock-step with oracle/es_oracle.py:mix64

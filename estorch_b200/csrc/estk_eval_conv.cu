@@ -316,6 +316,10 @@ extern "C" int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_ac
                                   int32_t B, float* returns_plus, float* returns_minus, void* scratch,
                                   int64_t scratch_bytes, void* stream) {
   const bool f16 = precision == ESTK_PREC_F16;
+  if (((n_actions >> 16) & 0xff) == (ESTK_ACTIONS >> 16))
+    return eval_conv_actions(ctx, precision, n_actions, theta, table, table16, offsets, order, pairs, sigma, xref,
+                             ref_batch, obs, B, returns_plus, returns_minus, scratch, scratch_bytes,
+                             (cudaStream_t)stream);
   ESTK_CHECK_ARG(ctx && theta && xref && obs && target && returns_plus && scratch, "estk_eval_conv_vbn: null argument");
   ESTK_CHECK_ARG(offsets == nullptr || (table && (table16 || !f16) && returns_minus),
                  "estk_eval_conv_vbn: table%s/returns_minus required with offsets", f16 ? "/table16" : "");

@@ -19,10 +19,12 @@ Three execution modes, chosen per instance:
             overridden: a generation is a handful of kernel launches, nothing
             touches the host unless the user reads an attribute.
 * population -- PopulationAgent (environments stepped by user code, one per
-            member) + recognised MLP policy + Adam + no hook overridden, on one
-            GPU: every environment step is one launch that evaluates every
-            perturbed policy on its member's own observation (estk_eval_mlp with
-            ESTK_ACTIONS); ranks, gradient and Adam as in fused mode.
+            member) + recognised MLP or conv + VirtualBatchNorm policy + Adam +
+            no hook overridden, on one GPU: every environment step is one launch
+            that evaluates every perturbed policy on its member's own observation
+            (estk_eval_mlp / estk_eval_conv_vbn with ESTK_ACTIONS; the conv
+            policy's VBN statistics are one more launch per generation); ranks,
+            gradient and Adam as in fused mode.
 * hooks  -- anything else (host agents such as gym loops, custom subclasses
             overriding ``_sample_policy`` / ``_calculate_grad`` / ..., other
             optimizers): the reference's own control flow through its hooks,
@@ -42,7 +44,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from ._capi import ESTK_LOSS_XENT, ESTK_MAX_POPULATION
+from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
 from .agents import DeviceAgent, PopulationAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import ConvVBNSpec, conv_vbn_spec_from_module, mlp_spec_from_module
@@ -354,9 +356,13 @@ class ES:
             self._obs = self.agent.obs.to(self._dev).contiguous()
             self._tgt = self.agent.target.to(self._dev).contiguous()
 
-        self._xref = self._conv_scratch = None
+        self._xref = self._conv_scratch = self._conv_stats = None
         if self._fused and self._is_conv:
             self._xref = self.target.xref.detach().to(self._dev, torch.float32).contiguous()
+        if self._fused and self._is_conv and self._population:
+            # VBN statistics of every member, computed once per generation (population mode's conv act)
+            self._conv_stats = torch.empty(P, ESTK_CONV_VBN_STATS_FLOATS, dtype=torch.float32, device=self._dev)
+        elif self._fused and self._is_conv:
             nbytes = be.conv_scratch_bytes(self._xref.shape[0], self._obs.shape[0], self._precision)
             self._conv_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self._dev)
 
@@ -379,12 +385,13 @@ class ES:
         return not getattr(getattr(type(self), name), "_estk_builtin", False)
 
     def _decide_fused(self, optimizer_cls):
-        """Fused mode for a DeviceAgent, population mode for a PopulationAgent (an MLP policy on one GPU:
-        the multi-GPU population generation is not implemented, hooks mode serves it)."""
+        """Fused mode for a DeviceAgent, population mode for a PopulationAgent (a recognised MLP or conv +
+        VirtualBatchNorm policy on one GPU: the multi-GPU population generation is not implemented, hooks
+        mode serves it)."""
         population = isinstance(self.agent, PopulationAgent)
         if not (self._device_agent or population) or self._spec is None:
             return False
-        if population and (self._is_conv or self.n_workers > 1):
+        if population and self.n_workers > 1:
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -1024,6 +1031,8 @@ class ES:
         """The ``act`` handed to ``rollout_population``: observations ``[M, in]`` or ``[M, B, in]`` -> outputs of
         every member in ONE launch (estk_eval_mlp with ESTK_ACTIONS).  Population: M = P members of the last
         drawn offsets around ``slot.theta_prev`` (+ members first, then their mirrors); centre: M = 1, theta."""
+        if self._is_conv:
+            return self._population_act_conv(slot, centre)
         be, dims, dev, code = self._be, self._spec.dims, self._dev, self._spec.act
         M = 1 if centre else self.population_size
         t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
@@ -1041,6 +1050,35 @@ class ES:
             else:
                 be.act_mlp(dims, slot.theta_prev, self._table, self._offsets, self._order, self._pairs_local,
                            self.sigma, x3, out, act=code, table16=t16)
+            return out[:, 0] if single else out
+        return act
+
+    def _population_act_conv(self, slot, centre):
+        """``act`` for the conv + VirtualBatchNorm policy: frames ``[M, 4, 84, 84]`` or ``[M, B, 4, 84, 84]`` ->
+        outputs ``[M, A]`` or ``[M, B, A]``.  The members' VBN statistics over ``xref`` depend only on their
+        weights, so they are computed by ONE launch here, when the ``act`` is built, and every call is one
+        launch that reuses them (the reference recomputes them on every forward, examples/atari.py:25-37).
+        The centre form keeps them in a one-member buffer of its slot."""
+        be, dev, A = self._be, self._dev, self._spec.n_actions
+        M = 1 if centre else self.population_size
+        t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
+        if centre:
+            if getattr(slot, "conv_stats", None) is None:
+                slot.conv_stats = torch.empty(1, ESTK_CONV_VBN_STATS_FLOATS, dtype=torch.float32, device=dev)
+            theta, stats, args = slot.theta, slot.conv_stats, (None, None, None, 1, 0.0)
+        else:
+            theta, stats = slot.theta_prev, self._conv_stats
+            args = (self._table, self._offsets, self._order, self._pairs_local, self.sigma)
+        be.act_conv_vbn(A, theta, *args, self._xref, None, None, stats, table16=t16)
+
+        def act(obs):
+            x = torch.as_tensor(obs).to(device=dev, dtype=torch.float32).contiguous()
+            single = x.dim() == 4
+            x5 = x.unsqueeze(1) if single else x
+            if x5.dim() != 5 or x5.shape[0] != M or tuple(x5.shape[2:]) != (4, 84, 84):
+                raise ValueError(f"act: frames {tuple(x.shape)}, expected [{M}, 4, 84, 84] or [{M}, B, 4, 84, 84]")
+            out = torch.empty(M, x5.shape[1], A, dtype=torch.float32, device=dev)
+            be.act_conv_vbn(A, theta, *args, None, x5, out, stats, table16=t16)
             return out[:, 0] if single else out
         return act
 

@@ -323,7 +323,40 @@ ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precisio
  *                   relative) of the fp32 forward.  VBN statistics, normalisation, biases, fc2 and
  *                   the loss are fp32; no atomics, so the returns are the same bits run to run.
  *                   Population: table, table16.  theta, scratch and table16 16-byte aligned.
- *   any other       ESTK_ERR_UNSUPPORTED. */
+ *   any other       ESTK_ERR_UNSUPPORTED.
+ *
+ * Action mode (an environment population's per-step forward).  n_actions is three bit fields:
+ *   bits 0-7   A, the number of actions, 1..64;
+ *   bits 8-15  must be 0;
+ *   bits 16-23 0 (the evaluate above) or ESTK_ACTIONS (the same macro and meaning as the loss field of
+ *              estk_mlp_desc.activation): no return, each member's outputs on its OWN frames.
+ * Every value refused before this mode existed is still refused.  With ESTK_ACTIONS only ESTK_PREC_FP32
+ * serves (ESTK_PREC_F16 and any other precision are ESTK_ERR_UNSUPPORTED before any launch), target is not
+ * read, order keeps its meaning (scheduling only), and table16, when non-null, is read INSTEAD of table (the
+ * exact fp16 copy: the same values and bits at half the noise bytes).  estk_eval_conv_vbn_scratch_bytes keeps
+ * its meaning (the evaluate's scratch); here scratch holds the VBN statistics of every member,
+ * [members][ESTK_CONV_VBN_STATS_FLOATS] fp32 in member order (the + members of the local pairs, then their
+ * mirrors; the centre has one member), so scratch_bytes >= members * ESTK_CONV_VBN_STATS_FLOATS * 4, and
+ * scratch is 16-byte aligned.  A member's entry is VBN1's scale and shift [16*20*20] each, then VBN2's
+ * [32*9*9] each, folded as a = gamma / sqrtf(var + 1e-5f), c = beta - mean * a (gamma, beta the member's
+ * perturbed parameters; mean, unbiased var over xref in the fp32 evaluate's accumulation order).  A call
+ * runs one or both phases, the stats phase first:
+ *   stats phase (xref != NULL): writes every member's statistics into scratch; ref_batch >= 2.  The raw
+ *              conv1 outputs of the reference batch go through a per-CTA slab of the context workspace
+ *              (grown like the buffers above: ESTK_ERR_NOMEM under capture).
+ *   act phase (obs != NULL): reads the statistics from scratch.  Population: obs [2*pairs][B][4][84][84]
+ *              (block j the frames of the + member of local pair j, block pairs + j those of its mirror),
+ *              returns_plus [pairs][B][A] receives the + members' outputs, returns_minus [pairs][B][A] the
+ *              mirrors'.  Centre (offsets == NULL): obs [B][4][84][84], returns_plus [B][A] for theta.
+ * A call with xref == NULL uses what an earlier stats call left in scratch; the caller must have made that
+ * call for the same theta, offsets, pairs and sigma.  xref and obs both NULL is ESTK_ERR_INVALID.
+ * Arithmetic, element by element that of the fp32 evaluate: W = theta +- (sigma*t) with two roundings,
+ * conv1 / conv2 as fmaf chains from the bias in (ci, kh, kw) order, normalisation fmaxf(fmaf(y, a, c), 0),
+ * fc1 one chain from 0 in ascending k then + bias and ReLU, fc2 one chain from the bias -- a member's
+ * outputs are the bits of the outputs its ESTK_PREC_FP32 evaluate computes on the same frames.  A member's
+ * outputs never depend on another member's frames; no float atomics (the same bits from run to run, with
+ * or without order, from table or table16). */
+#define ESTK_CONV_VBN_STATS_FLOATS 17984  /* per member: 2 * 16*20*20 + 2 * 32*9*9 */
 ESTK_API int64_t estk_eval_conv_vbn_scratch_bytes(estk_ctx* ctx, int32_t precision, int32_t ref_batch, int32_t B);
 ESTK_API int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_actions, const float* theta,
                        const float* table, const uint16_t* table16,
