@@ -77,8 +77,31 @@ constexpr int64_t kXrDataOff = 4096;      // float gsum[nq * 4]  (this rank's pa
 __host__ __device__ inline int64_t xr_image_bytes(int64_t n) { return ((n + 3) / 4 * 16 + 255) / 256 * 256; }
 
 struct AdamScalars {
-  float one_minus_b1, b2, one_minus_b2, bc2_sqrt, eps, neg_step, wd, clamp, inv_div;
+  float lerp_coef, b2, one_minus_b2, bc2_sqrt, eps, neg_step, wd, clamp, inv_div;
+  int lerp_big;      // lerp_coef = w = 1 - beta1 (0), or w - 1 with the new gradient as the fma's addend (1)
 };
+
+// The launch-wide scalars of adam_elem for Adam step t (t = 0: gradient only, no bias corrections).
+// torch.optim.Adam takes 1 - beta1 / 1 - beta2 / -lr/bc1 in fp64 and rounds them to fp32 when they meet
+// the fp32 tensors; lerp_ picks its form once from the fp32 weight (ATen lerp: small while |w| < 0.5).
+__device__ __forceinline__ AdamScalars adam_scalars(const estk_adam_desc& d, int P, int64_t t) {
+  AdamScalars a;
+  a.inv_div = (float)P;
+  a.clamp = d.clamp;
+  const float w = (float)(1.0 - d.beta1);
+  a.lerp_big = fabsf(w) >= 0.5f;
+  a.lerp_coef = a.lerp_big ? __fsub_rn(w, 1.f) : w;
+  a.b2 = (float)d.beta2;
+  a.one_minus_b2 = (float)(1.0 - d.beta2);
+  a.eps = (float)d.eps;
+  a.wd = (float)d.weight_decay;
+  a.bc2_sqrt = 1.f; a.neg_step = 0.f;
+  if (t > 0) {
+    a.bc2_sqrt = (float)sqrt(1.0 - pow(d.beta2, (double)t));
+    a.neg_step = (float)(-(d.lr / (1.0 - pow(d.beta1, (double)t))));
+  }
+  return a;
+}
 
 // Order-preserving 32-bit image of a return: -0 maps to +0 (they compare equal), every NaN to 0xffffffff
 // (after +inf: numpy's argsort puts NaN last).  image(a) < image(b) <=> a sorts before b.
@@ -94,18 +117,22 @@ __device__ __forceinline__ float centre(int rank, int P) {
 }
 
 // torch.optim.Adam single-tensor update on one element (torch/optim/adam.py:
-// lerp_ :457, mul_/addcmul_ :476, sqrt/div/add_ :529-545, addcdiv_ :546), with
-// IEEE-rounded individual operations (no FMA contraction) like the CPU kernels.
+// add :429, lerp_ :457, mul_/addcmul_ :476, sqrt/div/add_ :543, addcdiv_ :545), operation for
+// operation as ATen's vectorised CPU kernels round it: three of them are single fmas there
+// (add with alpha: fma(wd, theta, g); lerp_: fma(w, g - m, m), or fma(w - 1, g - m, g) for
+// |w| >= 0.5; addcmul_: fma((1 - beta2) g, g, beta2 v)), every other operation is rounded on its
+// own (explicit intrinsics: no contraction).  m and v are therefore torch's bits; theta is too
+// wherever torch's own sqrt is correctly rounded (__fsqrt_rn always is; torch's CPU sqrt is
+// occasionally one ulp off).
 __device__ __forceinline__ void adam_elem(float sum, const AdamScalars& a, float& th, float& m,
                                           float& v, float* g_out) {
   const float g = __fdiv_rn(sum, a.inv_div);  // inv_div holds (float)P
   if (g_out) *g_out = g;
   float gp = -g;                               // estorch.py:239
   if (a.clamp > 0.f) gp = fminf(fmaxf(gp, -a.clamp), a.clamp);  // :243
-  if (a.wd != 0.f) gp = __fadd_rn(gp, __fmul_rn(a.wd, th));
-  m = __fadd_rn(m, __fmul_rn(__fsub_rn(gp, m), a.one_minus_b1));
-  v = __fmul_rn(v, a.b2);
-  v = __fadd_rn(v, __fmul_rn(__fmul_rn(a.one_minus_b2, gp), gp));
+  if (a.wd != 0.f) gp = __fmaf_rn(a.wd, th, gp);
+  m = __fmaf_rn(a.lerp_coef, __fsub_rn(gp, m), a.lerp_big ? gp : m);
+  v = __fmaf_rn(__fmul_rn(a.one_minus_b2, gp), gp, __fmul_rn(v, a.b2));
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), a.bc2_sqrt), a.eps);
   th = __fadd_rn(th, __fdiv_rn(__fmul_rn(a.neg_step, m), denom));
 }
@@ -293,25 +320,7 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
   //      publishes the increment after the last one, so there is no race)
   int64_t adam_t = 0;
   if (p.fused_adam) adam_t = p.state->adam_step + 1;
-  if (tid == 0) {
-    AdamScalars a;
-    a.inv_div = (float)p.P;
-    a.clamp = p.adam.clamp;
-    a.one_minus_b1 = (float)(1.0 - p.adam.beta1);
-    a.b2 = (float)p.adam.beta2;
-    a.one_minus_b2 = (float)(1.0 - p.adam.beta2);
-    a.eps = (float)p.adam.eps;
-    a.wd = (float)p.adam.weight_decay;
-    if (p.fused_adam) {
-      const double bc1 = 1.0 - pow(p.adam.beta1, (double)adam_t);
-      const double bc2 = 1.0 - pow(p.adam.beta2, (double)adam_t);
-      a.bc2_sqrt = (float)sqrt(bc2);
-      a.neg_step = (float)(-(p.adam.lr / bc1));
-    } else {
-      a.bc2_sqrt = 1.f; a.neg_step = 0.f;
-    }
-    s_adam = a;
-  }
+  if (tid == 0) s_adam = adam_scalars(p.adam, p.P, adam_t);
 
   // ---- phase A: ranks.  rank_i = #{j: r_j < r_i} + #{j < i: r_j == r_i}
   //      numpy's argsort order (estorch.py:25): NaN sorts last, NaNs among themselves by index.
@@ -373,7 +382,9 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
   const int64_t c1 = (int64_t)(cs + 1) * p.n4 / p.CS;
   const int s0 = (int)((int64_t)ps * p.pairs_local / p.PS);
   const int s1 = (int)((int64_t)(ps + 1) * p.pairs_local / p.PS);
-  const AdamScalars adam = s_adam;  // valid: written before the __syncthreads in grid.sync
+  // valid: written before the __syncthreads in grid.sync; read from shared memory where the epilogue
+  // needs it, so that none of it is held in registers through phase B
+  const AdamScalars& adam = s_adam;
   const bool raw_out = !p.fused_adam || XR;   // phases B / C leave the raw sum in grad_sum_out
   if constexpr (T16) {
     // fp16 table: a 128-bit load carries 8 noise values; same 16 loads in flight per thread, half the
@@ -571,22 +582,7 @@ __global__ void __launch_bounds__(256) clamp_adam_kernel(const RankGradParams p,
   const bool do_adam = p.theta != nullptr;
   int64_t adam_t = 0;
   if (do_adam) adam_t = p.state->adam_step + 1;
-  if (threadIdx.x == 0) {
-    AdamScalars a;
-    a.inv_div = (float)p.P;
-    a.clamp = p.adam.clamp;
-    a.one_minus_b1 = (float)(1.0 - p.adam.beta1);
-    a.b2 = (float)p.adam.beta2;
-    a.one_minus_b2 = (float)(1.0 - p.adam.beta2);
-    a.eps = (float)p.adam.eps;
-    a.wd = (float)p.adam.weight_decay;
-    a.bc2_sqrt = 1.f; a.neg_step = 0.f;
-    if (do_adam) {
-      a.bc2_sqrt = (float)sqrt(1.0 - pow(p.adam.beta2, (double)adam_t));
-      a.neg_step = (float)(-(p.adam.lr / (1.0 - pow(p.adam.beta1, (double)adam_t))));
-    }
-    s_adam = a;
-  }
+  if (threadIdx.x == 0) s_adam = adam_scalars(p.adam, p.P, adam_t);
   __syncthreads();
   const AdamScalars a = s_adam;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;

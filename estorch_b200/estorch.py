@@ -53,6 +53,17 @@ from .population import LazyPopulation, NoiseHandle
 __all__ = ["ES", "NS_ES", "NSR_ES", "NSRA_ES", "rank_transformation"]
 
 DEFAULT_NOISE_TABLE_SIZE = 1 << 28   # fp32 unit normals = 1 GiB per GPU (SURVEY 8d)
+_UNFUSED_ADAM_FLAGS = ("amsgrad", "maximize", "differentiable", "decoupled_weight_decay")
+
+
+def _refuse_unfused_adam_flags(group):
+    """The fused epilogue is torch's Adam with L2 weight decay only.  Constructor keywords that ask for
+    something else select hooks mode (ES._decide_fused); switched on in ``param_groups`` after
+    construction, they would silently give a different optimizer."""
+    on = [k for k in _UNFUSED_ADAM_FLAGS if group.get(k)]
+    if on:
+        raise ValueError(f"the fused Adam step does not implement {', '.join(on)}; pass it to the optimizer's "
+                         "constructor instead (hooks mode runs torch's own optimizer)")
 
 
 # ----------------------------------------------------------------------------
@@ -396,8 +407,8 @@ class ES:
         if optimizer_cls is not torch.optim.Adam:
             return False
         kw = self._optimizer_kwargs
-        if kw.get("amsgrad") or kw.get("maximize") or kw.get("differentiable"):
-            return False
+        if any(kw.get(k) for k in _UNFUSED_ADAM_FLAGS):
+            return False                        # the fused epilogue is Adam with L2 weight decay only
         if getattr(self, "k", 0) > 32:          # estk_knn_novelty's per-lane top-k buffer; the reference accepts
             return False                        # any k (estorch.py:413) -> hooks mode (host novelty) serves it
         if population:
@@ -784,6 +795,7 @@ class ES:
     # ------------------------------------------------------------------ fused generation
     def _adam_desc(self, optimizer):
         g = optimizer.param_groups[0]
+        _refuse_unfused_adam_flags(g)
         return adam_desc(lr=g["lr"], betas=g["betas"], eps=g["eps"], weight_decay=g["weight_decay"], clamp=1.0)
 
     def _exact_table16(self):
@@ -968,6 +980,7 @@ class ES:
                 or getattr(self, "_graph_broken", False) or type(self)._fused_generation is not ES._fused_generation):
             return None
         g = slot.optimizer.param_groups[0]
+        _refuse_unfused_adam_flags(g)           # a replay does not go through _adam_desc
         nb = self._next_batch_ptrs
         return (id(slot), bool(self._pending_centre), self._defers_centre(), float(g["lr"]), tuple(g["betas"]), float(g["eps"]),
                 float(g["weight_decay"]), float(self.sigma), self._table._version, nb,

@@ -157,8 +157,14 @@ typedef struct {
   int32_t activation;                /* ESTK_ACT_* bit fields above; 0 = ReLU between layers, none after the last */
 } estk_mlp_desc;
 
-/* torch.optim.Adam hyper-parameters (torch/optim/adam.py:457-546; the
- * optimizer every reference example uses, examples/cartpole_es.py:48-50). */
+/* torch.optim.Adam hyper-parameters (torch/optim/adam.py:429-545; the
+ * optimizer every reference example uses, examples/cartpole_es.py:48-50).
+ * The step is torch's single-tensor CPU Adam rounded as ATen rounds it: the weight-decay add,
+ * lerp_ (both of its forms) and addcmul_ are one fma each, every other operation is rounded on
+ * its own.  m and v are bit-exact to torch; theta is bit-exact to that form, and to torch wherever
+ * torch's CPU sqrt is correctly rounded (the kernels' sqrt always is).  weight_decay is torch's L2
+ * decay through the gradient; AdamW's decoupled decay (decoupled_weight_decay=True), amsgrad and
+ * maximize are not implemented (the Python engine refuses them and runs torch's own optimizer). */
 typedef struct {
   double lr, beta1, beta2, eps, weight_decay;
   float clamp; /* estorch.py:243 clamps the negated gradient to +-1.0; <=0 disables */

@@ -35,7 +35,7 @@ __all__ = [
     "round_f16", "mlp_forward_f16",
     "sample_population", "sample_population_bf16s", "evaluate_population",
     "blend_weights", "calculate_grad", "calculate_grad_pairs", "negate_clamp",
-    "adam_step", "novelty", "nsra_weight_update", "vbn_stats", "vbn_normalize",
+    "fma32", "adam_step", "novelty", "nsra_weight_update", "vbn_stats", "vbn_normalize",
     "conv2d_nchw", "atari_param_layout", "atari_forward",
     "es_generation",
 ]
@@ -350,23 +350,54 @@ def negate_clamp(grad: np.ndarray) -> np.ndarray:
 # optimizer -- estorch.py:245 -> torch/optim/adam.py:457,476,529-546
 # --------------------------------------------------------------------------
 
+def fma32(a, b, c) -> np.ndarray:
+    """fp32 ``fma(a, b, c)``, rounded once.  The fp64 product of two fp32 values is exact; the fp64
+    sum is rounded to odd (its TwoSum error term decides the last bit), and a round-to-odd value with
+    53 >= 24 + 2 bits rounds to the correctly rounded fp32 result -- a plain fp64 sum would round twice
+    when it lands on an fp32 midpoint."""
+    a, b, c = np.broadcast_arrays(*(np.asarray(x, dtype=np.float32).astype(np.float64) for x in (a, b, c)))
+    with np.errstate(over="ignore", invalid="ignore"):
+        p = a * b
+        s = p + c
+        bv = s - p
+        err = (p - (s - bv)) + (c - bv)
+        inexact = (err != 0) & np.isfinite(err) & ((np.atleast_1d(s).view(np.int64) & 1) == 0).reshape(s.shape)
+        s = np.where(inexact, np.nextafter(s, np.where(err > 0, np.inf, -np.inf)), s)
+        return s.astype(np.float32)
+
+
 def adam_step(theta, m, v, grad, step: int, lr=0.01, beta1=0.9, beta2=0.999,
               eps=1e-8, weight_decay=0.0):
-    """torch.optim.Adam single-tensor CPU path, defaults as in
+    """torch.optim.Adam single-tensor CPU path (``foreach=False``), defaults as in
     examples/cartpole_es.py:48-50.  ``step`` is the 1-based step count *after*
-    the increment.  Returns new (theta, m, v), fp32."""
+    the increment.  Returns new (theta, m, v), fp32.
+
+    Rounded as ATen's vectorised CPU kernels round it: ``grad.add(param, alpha=wd)`` is
+    ``fma(wd, theta, g)``, ``lerp_`` is ``fma(w, g - m, m)`` for ``|w| < 0.5`` and
+    ``fma(w - 1, g - m, g)`` otherwise (w = 1 - beta1 in fp32), ``addcmul_`` is
+    ``fma((1 - beta2) g, g, beta2 v)``; every other operation is rounded on its own.
+    ``np.sqrt`` is correctly rounded; torch's CPU ``sqrt`` is sometimes one ulp off, so theta
+    equals torch's exactly wherever torch's ``sqrt(v)`` is the correctly rounded value."""
     f = np.float32
-    g = grad.astype(np.float32)
-    if weight_decay:
-        g = (g + f(weight_decay) * theta).astype(np.float32)
-    m = (m + (g - m) * f(1.0 - beta1)).astype(np.float32)          # lerp_
-    v = (v * f(beta2)).astype(np.float32)
-    v = (v + (f(1.0 - beta2) * g) * g).astype(np.float32)          # addcmul_
-    bc1 = 1.0 - beta1 ** step
-    bc2 = 1.0 - beta2 ** step
-    step_size = lr / bc1
-    denom = (np.sqrt(v).astype(np.float32) / f(math.sqrt(bc2)) + f(eps)).astype(np.float32)
-    theta = (theta + (f(-step_size) * m) / denom).astype(np.float32)  # addcdiv_
+    theta = np.asarray(theta, dtype=f)
+    m = np.asarray(m, dtype=f)
+    v = np.asarray(v, dtype=f)
+    g = np.asarray(grad, dtype=f)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        if weight_decay:
+            g = fma32(f(weight_decay), theta, g)                   # adam.py:429
+        w = f(1.0 - beta1)
+        d = (g - m).astype(f)
+        if abs(w) < 0.5:                                           # lerp_, adam.py:457
+            m = fma32(w, d, m)
+        else:
+            m = fma32(w - f(1.0), d, g)
+        v = fma32((f(1.0 - beta2) * g).astype(f), g, (v * f(beta2)).astype(f))   # mul_ / addcmul_, :476
+        bc1 = 1.0 - beta1 ** step
+        bc2 = 1.0 - beta2 ** step
+        step_size = lr / bc1
+        denom = ((np.sqrt(v) / f(math.sqrt(bc2))).astype(f) + f(eps)).astype(f)   # :543
+        theta = (theta + ((f(-step_size) * m).astype(f) / denom).astype(f)).astype(f)   # addcdiv_, :545
     return theta, m, v
 
 

@@ -191,15 +191,21 @@ def test_rank_grad_adam_matches_reference_golden(be, name):
         ok = np.abs(g["grad"][gen]) > 1e-4 * np.abs(g["grad"][gen]).max()      # see DESIGN.md (Adam at g~0)
         assert rel_err(out["theta"][ok], g["theta_after"][gen][ok]) < 1e-5
         assert np.abs(out["theta"] - g["theta_after"][gen]).max() <= 0.02
-        # Adam alone (identical gradient bits through clamp_adam) is exact to 1e-6
+        # Adam alone (identical gradient bits through clamp_adam; P is a power of two, so sum / P is
+        # the golden's g exactly): bit-exact to the oracle's restatement of torch's Adam, and within
+        # 1e-6 of the reference (whose CPU sqrt is sometimes one ulp off; the kernel's is correctly rounded)
         from estorch_b200.backend import new_state, write_state, adam_desc
         st = new_state(be.device); write_state(st, adam_step=gen)
         th, mm, vv = dev(be, theta), dev(be, m), dev(be, v)
         be.clamp_adam(dev(be, g["grad"][gen] * np.float32(len(ret))), len(ret), th, mm, vv, st,
                       adam_desc(lr=0.01))
-        assert rel_err(th.cpu().numpy(), g["theta_after"][gen]) < 1e-6
+        want = orc.adam_step(theta, m, v, orc.negate_clamp(g["grad"][gen]), gen + 1)
         theta, m, v = th.cpu().numpy(), mm.cpu().numpy(), vv.cpu().numpy()
-    assert rel_err(m, g["m_final"]) < 1e-5 and rel_err(v, g["v_final"]) < 1e-5
+        for got, w in zip((theta, m, v), want):
+            np.testing.assert_array_equal(got.view(np.int32), w.view(np.int32))
+        assert rel_err(theta, g["theta_after"][gen]) < 1e-6
+    np.testing.assert_array_equal(m.view(np.int32), g["m_final"].view(np.int32))     # torch's bits
+    np.testing.assert_array_equal(v.view(np.int32), g["v_final"].view(np.int32))
 
 
 @pytest.mark.parametrize("algo,w", [("ns", (0.0, 1.0)), ("nsr", (0.5, 0.5)), ("nsra", None)])
