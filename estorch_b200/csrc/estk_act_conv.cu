@@ -11,8 +11,8 @@
 //
 // conv_stats_kernel: phases B-C of eval_conv_vbn_kernel (estk_eval_conv.cu) with the same arithmetic in
 // the same order -- one persistent CTA per member, the R raw conv1 outputs in a per-CTA slab of the
-// context workspace -- writing the folded VBN scale a = gamma / sqrtf(var + 1e-5f) and shift
-// c = beta - mean * a to stats[member][ESTK_CONV_VBN_STATS_FLOATS] instead of shared memory.
+// context workspace -- writing the VBN scale a = gamma / sqrtf(var + 1e-5f) and the mean (Welford's update) to
+// stats[member][ESTK_CONV_VBN_STATS_FLOATS] instead of shared memory.
 //
 // conv_act_kernel: one CTA per antithetic pair x chunk of NB frames per member.  The pair's noise is read
 // once and serves both signs: conv1 / conv2 weights are formed as W+ = theta + sigma*t and
@@ -20,7 +20,7 @@
 // member's stats, coalesced loads), ReLU, conv2, VBN2, ReLU into features [2][NB][2592] (shared memory
 // for NB <= 4, a workspace slab for NB = 8); fc1 is tiled over k (each W+/W- tile from one noise read,
 // aliasing the dead conv weights); fc2 last.  Per element the arithmetic of eval_conv_vbn_kernel: fmaf
-// chains from the bias in (ci, kh, kw) order, fmaxf(fmaf(y, a, c), 0), fc1 one chain from 0 in
+// chains from the bias in (ci, kh, kw) order, fmaxf(fmaf(y - mean, a, beta), 0), fc1 one chain from 0 in
 // ascending k then + bias and ReLU, fc2 one chain from the bias -- so a member's outputs are the bits
 // of the y its fp32 evaluate computes.  No atomics: the same bits from run to run.
 //
@@ -42,7 +42,7 @@ constexpr int FC1 = 256;
 constexpr int KT = 32;                                         // k-tile of fc1 (2592 = 81 tiles)
 constexpr int FC2_AT = 32;                                     // fc2 outputs per formed weight tile
 constexpr int kStats = 2 * P1 + 2 * P2;
-static_assert(kStats == ESTK_CONV_VBN_STATS_FLOATS, "stats layout: a1, c1 [6400], a2, c2 [2592]");
+static_assert(kStats == ESTK_CONV_VBN_STATS_FLOATS, "stats layout: a1, mean1 [6400], a2, mean2 [2592]");
 
 // parameter offsets, registration order of examples/atari.py:17-23
 constexpr int64_t oC1W = 0, oC1B = 4096, oG1 = 4112, oB1 = 4128, oC2W = 4144, oC2B = 12336, oG2 = 12368,
@@ -87,10 +87,10 @@ __global__ void __launch_bounds__(kT, 1) conv_stats_kernel(const StatsParams p) 
   extern __shared__ __align__(16) float sm[];
   float* sW1 = sm;                    // [16][256]
   float* sW2 = sW1 + C1 * 256;        // [32][256]
-  float* sSmall = sW2 + C2 * 256;     // conv1.b 16, conv2.b 32
+  float* sSmall = sW2 + C2 * 256;     // conv1.b 16, conv2.b 32, bn1.b 16  (64)
   float* sA1 = sSmall + 64;           // [6400]
-  float* sC1 = sA1 + P1;              // [6400]
-  float* sX1 = sC1 + P1;              // [6400] normalised layer-1 activations of one reference frame
+  float* sM1 = sA1 + P1;              // [6400]
+  float* sX1 = sM1 + P1;              // [6400] normalised layer-1 activations of one reference frame
 
   const int tid = threadIdx.x;
   const bool centre = (p.offsets == nullptr);
@@ -112,6 +112,7 @@ __global__ void __launch_bounds__(kT, 1) conv_stats_kernel(const StatsParams p) 
     for (int i = tid; i < C2 * 256; i += kT) sW2[i] = par(oC2W + i);
     if (tid < 16) sSmall[tid] = par(oC1B + tid);
     if (tid < 32) sSmall[16 + tid] = par(oC2B + tid);
+    if (tid < 16) sSmall[48 + tid] = par(oB1 + tid);
     __syncthreads();
 
     auto conv1_image = [&](const float* img, float (&out)[2][C1]) {
@@ -142,14 +143,15 @@ __global__ void __launch_bounds__(kT, 1) conv_stats_kernel(const StatsParams p) 
 
     // ---------------- reference batch through conv1, per-position statistics of layer 1
     {
-      float sum[2][C1], ssq[2][C1];
+      float mean[2][C1], m2[2][C1];
 #pragma unroll
       for (int q = 0; q < 2; ++q)
 #pragma unroll
-        for (int co = 0; co < C1; ++co) { sum[q][co] = 0.f; ssq[q][co] = 0.f; }
+        for (int co = 0; co < C1; ++co) { mean[q][co] = 0.f; m2[q][co] = 0.f; }
       for (int r = 0; r < p.R; ++r) {
         float out[2][C1];
         conv1_image(p.xref + (size_t)r * IMG, out);
+        const float inv = 1.f / (float)(r + 1);
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const int hw = tid + q * kT;
@@ -158,27 +160,24 @@ __global__ void __launch_bounds__(kT, 1) conv_stats_kernel(const StatsParams p) 
           for (int co = 0; co < C1; ++co) {
             const float y = out[q][co];
             R1[(size_t)r * P1 + co * (H1 * W1) + hw] = y;
-            sum[q][co] += y;
-            ssq[q][co] = fmaf(y, y, ssq[q][co]);
+            welford_add(y, inv, mean[q][co], m2[q][co]);
           }
         }
       }
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int hw = tid + q * kT;
         if (hw >= H1 * W1) continue;
 #pragma unroll
         for (int co = 0; co < C1; ++co) {
-          const float mean = sum[q][co] * invR;
-          const float var = fmaxf((ssq[q][co] - sum[q][co] * mean) * invR1, 0.f);   // unbiased (modules.py:52)
+          const float var = m2[q][co] * invR1;   // unbiased (modules.py:52)
           const float a = par(oG1 + co) / sqrtf(var + 1e-5f);
-          const float c = par(oB1 + co) - mean * a;
           const int i = co * (H1 * W1) + hw;
           sA1[i] = a;
-          sC1[i] = c;
+          sM1[i] = mean[q][co];
           st[i] = a;
-          st[P1 + i] = c;
+          st[P1 + i] = mean[q][co];
         }
       }
     }
@@ -206,29 +205,29 @@ __global__ void __launch_bounds__(kT, 1) conv_stats_kernel(const StatsParams p) 
 
     // ---------------- reference batch through VBN1 / ReLU / conv2, statistics of layer 2
     {
-      float sum[11], ssq[11];
+      float mean[11], m2[11];
 #pragma unroll
-      for (int i = 0; i < 11; ++i) { sum[i] = 0.f; ssq[i] = 0.f; }
+      for (int i = 0; i < 11; ++i) { mean[i] = 0.f; m2[i] = 0.f; }
       for (int r = 0; r < p.R; ++r) {
         __syncthreads();
-        for (int i = tid; i < P1; i += kT) sX1[i] = fmaxf(fmaf(R1[(size_t)r * P1 + i], sA1[i], sC1[i]), 0.f);
+        for (int i = tid; i < P1; i += kT)
+          sX1[i] = fmaxf(fmaf(R1[(size_t)r * P1 + i] - sM1[i], sA1[i], sSmall[48 + i / (H1 * W1)]), 0.f);
         __syncthreads();
         float out[11];
         conv2_image(out);
+        const float inv = 1.f / (float)(r + 1);
 #pragma unroll
-        for (int i = 0; i < 11; ++i) { sum[i] += out[i]; ssq[i] = fmaf(out[i], out[i], ssq[i]); }
+        for (int i = 0; i < 11; ++i) welford_add(out[i], inv, mean[i], m2[i]);
       }
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
 #pragma unroll
       for (int i = 0; i < 11; ++i) {
         const int o = tid + i * kT;
         if (o >= P2) continue;
         const int co = o / (H2 * W2);
-        const float mean = sum[i] * invR;
-        const float var = fmaxf((ssq[i] - sum[i] * mean) * invR1, 0.f);
-        const float a = par(oG2 + co) / sqrtf(var + 1e-5f);
+        const float a = par(oG2 + co) / sqrtf(m2[i] * invR1 + 1e-5f);
         st[2 * P1 + o] = a;
-        st[2 * P1 + P2 + o] = par(oB2 + co) - mean * a;
+        st[2 * P1 + P2 + o] = mean[i];
       }
     }
   }
@@ -254,7 +253,7 @@ struct ActParams {
 
 // shared memory: conv weights of both signs, biases, one layer-1 frame, then the features unless SLAB
 constexpr int kActW = 2 * C1 * 256 + 2 * C2 * 256;   // 24576 floats; fc1 / fc2 tiles alias it later
-constexpr int kActHead = kActW + 128 + P1;
+constexpr int kActHead = kActW + 224 + P1;
 static_assert(2 * KT * (FC1 + 1) + 2 * 8 * FC1 <= kActW, "fc1 tiles + hidden rows fit in the conv-weight region");
 static_assert(2 * FC2_AT * FC1 + 2 * 8 * FC1 <= kActW, "fc2 tiles + hidden rows fit in the conv-weight region");
 
@@ -263,8 +262,8 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
   extern __shared__ __align__(16) float sm[];
   float* const sW1 = sm;                   // [2][16][256]  (+, -)
   float* const sW2 = sW1 + 2 * C1 * 256;   // [2][32][256]
-  float* const sB = sm + kActW;            // conv1.b [2][16], conv2.b [2][32]
-  float* const sX1 = sB + 128;             // [6400]
+  float* const sB = sm + kActW;            // conv1.b [2][16], conv2.b [2][32], bn1.b [2][16], bn2.b [2][32]
+  float* const sX1 = sB + 224;             // [6400]
   float* const sWtp = sm;                  // fc1: [KT][FC1+1] W+, then W-  (aliases sW1 / sW2)
   float* const sWtm = sWtp + KT * (FC1 + 1);
   float* const sH = sm + 2 * KT * (FC1 + 1);    // [2][NB][FC1] hidden rows (+ rows, then - rows)
@@ -297,6 +296,8 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
     for (int i = tid; i < C2 * 256; i += kT) form(oC2W + i, sW2[i], sW2[C2 * 256 + i]);
     if (tid < 16) form(oC1B + tid, sB[tid], sB[16 + tid]);
     if (tid < 32) form(oC2B + tid, sB[32 + tid], sB[64 + tid]);
+    if (tid < 16) form(oB1 + tid, sB[96 + tid], sB[112 + tid]);
+    if (tid < 32) form(oB2 + tid, sB[128 + tid], sB[160 + tid]);
     __syncthreads();
 
     // ---------------- each sign's frames: conv1, VBN1, ReLU, conv2, VBN2, ReLU -> F[s][b]
@@ -307,6 +308,8 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
       const float* const W2s = sW2 + s * C2 * 256;
       const float* const b1s = sB + s * 16;
       const float* const b2s = sB + 32 + s * 32;
+      const float* const be1s = sB + 96 + s * 16;
+      const float* const be2s = sB + 128 + s * 32;
       for (int bl = 0; bl < nb; ++bl) {
         const float* const img = p.obs + ((size_t)member * p.B + b0 + bl) * IMG;
         float out1[2][C1];
@@ -341,7 +344,7 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
 #pragma unroll
           for (int co = 0; co < C1; ++co) {
             const int i = co * (H1 * W1) + hw;
-            sX1[i] = fmaxf(fmaf(out1[q][co], __ldg(st + i), __ldg(st + P1 + i)), 0.f);
+            sX1[i] = fmaxf(fmaf(out1[q][co] - __ldg(st + P1 + i), __ldg(st + i), be1s[co]), 0.f);
           }
         }
         __syncthreads();
@@ -360,7 +363,7 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
 #pragma unroll
               for (int kw = 0; kw < 4; ++kw) acc = fmaf(x[kh * W1 + kw], w[ci * 16 + kh * 4 + kw], acc);
           }
-          Fr[o] = fmaxf(fmaf(acc, __ldg(st + 2 * P1 + o), __ldg(st + 2 * P1 + P2 + o)), 0.f);
+          Fr[o] = fmaxf(fmaf(acc - __ldg(st + 2 * P1 + P2 + o), __ldg(st + 2 * P1 + o), be2s[co]), 0.f);
         }
       }
     }

@@ -227,6 +227,14 @@ __device__ __forceinline__ int warp_sum_i(int v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// One step of Welford's mean / variance update for the n-th sample y (inv = 1.f / n, correctly rounded):
+// d = y - mean, mean += d * inv, m2 += d * (y - mean); the unbiased variance is m2 / (n - 1).  Where every y
+// is the same, d is 0 from the second sample on and the variance is exactly 0.
+__device__ __forceinline__ void welford_add(float y, float inv, float& mean, float& m2) {
+  const float d = y - mean;
+  mean = fmaf(d, inv, mean);
+  m2 = fmaf(d, y - mean, m2);
+}
 __device__ __forceinline__ float warp_sum_f(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

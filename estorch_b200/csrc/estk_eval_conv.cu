@@ -63,12 +63,12 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
   extern __shared__ __align__(16) float sm[];
   float* sW1 = sm;                    // [16][256]
   float* sW2 = sW1 + C1 * 256;        // [32][256]
-  float* sSmall = sW2 + C2 * 256;     // conv1.b 16, conv2.b 32  (48)
-  float* sA1 = sSmall + 64;           // [6400] scale of VBN1 per position
-  float* sC1 = sA1 + P1;              // [6400] shift
-  float* sA2 = sC1 + P1;              // [2592]
-  float* sC2 = sA2 + P2;              // [2592]
-  float* sX1 = sC2 + P2;              // [6400] normalised layer-1 activations of one image
+  float* sSmall = sW2 + C2 * 256;     // conv1.b 16, conv2.b 32, bn1.b 16, bn2.b 32  (96 of 128)
+  float* sA1 = sSmall + 128;          // [6400] scale of VBN1 per position
+  float* sM1 = sA1 + P1;              // [6400] mean
+  float* sA2 = sM1 + P1;              // [2592]
+  float* sM2 = sA2 + P2;              // [2592]
+  float* sX1 = sM2 + P2;              // [6400] normalised layer-1 activations of one image
   // fc phase aliases sX1.. : Wt [KT][FC1+1], Xt [TB][KT], Hs [TB][FC1]
   float* sWt = sX1;
   float* sXt = sWt + KT * (FC1 + 1);
@@ -96,6 +96,8 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
     for (int i = tid; i < C2 * 256; i += kT) sW2[i] = par(L.c2w + i);
     if (tid < 16) sSmall[tid] = par(L.c1b + tid);
     if (tid < 32) sSmall[16 + tid] = par(L.c2b + tid);
+    if (tid < 16) sSmall[48 + tid] = par(L.b1 + tid);
+    if (tid < 32) sSmall[64 + tid] = par(L.b2 + tid);
     __syncthreads();
 
     // conv1 of one image for this thread's spatial positions -> out[q][co]
@@ -126,15 +128,18 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
     };
 
     // ---------------- phase B: reference batch through conv1, per-position statistics
+    // Welford's update in frame order (welford_add): a sum of squares minus sum * mean cancels
+    // catastrophically where the mean is large and the variance small, e.g. 0..255 pixels that never change.
     {
-      float sum[2][C1], ssq[2][C1];
+      float mean[2][C1], m2[2][C1];
 #pragma unroll
       for (int q = 0; q < 2; ++q)
 #pragma unroll
-        for (int co = 0; co < C1; ++co) { sum[q][co] = 0.f; ssq[q][co] = 0.f; }
+        for (int co = 0; co < C1; ++co) { mean[q][co] = 0.f; m2[q][co] = 0.f; }
       for (int r = 0; r < p.R; ++r) {
         float out[2][C1];
         conv1_image(p.xref + (size_t)r * IMG, out);
+        const float inv = 1.f / (float)(r + 1);
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const int hw = tid + q * kT;
@@ -143,23 +148,21 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
           for (int co = 0; co < C1; ++co) {
             const float y = out[q][co];
             R1[(size_t)r * P1 + co * (H1 * W1) + hw] = y;
-            sum[q][co] += y;
-            ssq[q][co] = fmaf(y, y, ssq[q][co]);
+            welford_add(y, inv, mean[q][co], m2[q][co]);
           }
         }
       }
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int hw = tid + q * kT;
         if (hw >= H1 * W1) continue;
 #pragma unroll
         for (int co = 0; co < C1; ++co) {
-          const float mean = sum[q][co] * invR;
-          const float var = fmaxf((ssq[q][co] - sum[q][co] * mean) * invR1, 0.f);   // unbiased (modules.py:52)
+          const float var = m2[q][co] * invR1;   // unbiased (modules.py:52)
           const float a = par(L.g1 + co) / sqrtf(var + 1e-5f);
           sA1[co * (H1 * W1) + hw] = a;
-          sC1[co * (H1 * W1) + hw] = par(L.b1 + co) - mean * a;
+          sM1[co * (H1 * W1) + hw] = mean[q][co];
         }
       }
     }
@@ -188,29 +191,29 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
 
     // ---------------- phase C: reference batch through VBN1/ReLU/conv2, statistics of layer 2
     {
-      float sum[11], ssq[11];
+      float mean[11], m2[11];
 #pragma unroll
-      for (int i = 0; i < 11; ++i) { sum[i] = 0.f; ssq[i] = 0.f; }
+      for (int i = 0; i < 11; ++i) { mean[i] = 0.f; m2[i] = 0.f; }
       for (int r = 0; r < p.R; ++r) {
         __syncthreads();
-        for (int i = tid; i < P1; i += kT) sX1[i] = fmaxf(fmaf(R1[(size_t)r * P1 + i], sA1[i], sC1[i]), 0.f);
+        for (int i = tid; i < P1; i += kT)
+          sX1[i] = fmaxf(fmaf(R1[(size_t)r * P1 + i] - sM1[i], sA1[i], sSmall[48 + i / (H1 * W1)]), 0.f);
         __syncthreads();
         float out[11];
         conv2_image(out);
+        const float inv = 1.f / (float)(r + 1);
 #pragma unroll
-        for (int i = 0; i < 11; ++i) { sum[i] += out[i]; ssq[i] = fmaf(out[i], out[i], ssq[i]); }
+        for (int i = 0; i < 11; ++i) welford_add(out[i], inv, mean[i], m2[i]);
       }
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
 #pragma unroll
       for (int i = 0; i < 11; ++i) {
         const int o = tid + i * kT;
         if (o >= P2) continue;
         const int co = o / (H2 * W2);
-        const float mean = sum[i] * invR;
-        const float var = fmaxf((ssq[i] - sum[i] * mean) * invR1, 0.f);
-        const float a = par(L.g2 + co) / sqrtf(var + 1e-5f);
+        const float a = par(L.g2 + co) / sqrtf(m2[i] * invR1 + 1e-5f);
         sA2[o] = a;
-        sC2[o] = par(L.b2 + co) - mean * a;
+        sM2[o] = mean[i];
       }
     }
     __syncthreads();
@@ -227,7 +230,7 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
 #pragma unroll
         for (int co = 0; co < C1; ++co) {
           const int i = co * (H1 * W1) + hw;
-          sX1[i] = fmaxf(fmaf(out1[q][co], sA1[i], sC1[i]), 0.f);
+          sX1[i] = fmaxf(fmaf(out1[q][co] - sM1[i], sA1[i], sSmall[48 + co]), 0.f);
         }
       }
       __syncthreads();
@@ -236,7 +239,7 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
 #pragma unroll
       for (int i = 0; i < 11; ++i) {
         const int o = tid + i * kT;
-        if (o < P2) XS[(size_t)b * P2 + o] = fmaxf(fmaf(out2[i], sA2[o], sC2[o]), 0.f);
+        if (o < P2) XS[(size_t)b * P2 + o] = fmaxf(fmaf(out2[i] - sM2[o], sA2[o], sSmall[64 + o / (H2 * W2)]), 0.f);
       }
     }
     __syncthreads();
@@ -297,7 +300,7 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_kernel(const ConvParams p
 size_t conv_smem_bytes() {
   const size_t fc_tile = (size_t)KT * (FC1 + 1) + (size_t)TB * KT;     // aliases the sX1 region in phase E
   const size_t tail = fc_tile > (size_t)P1 ? fc_tile : (size_t)P1;
-  return sizeof(float) * ((size_t)C1 * 256 + (size_t)C2 * 256 + 64 + 2 * (size_t)P1 + 2 * (size_t)P2 + tail);
+  return sizeof(float) * ((size_t)C1 * 256 + (size_t)C2 * 256 + 128 + 2 * (size_t)P1 + 2 * (size_t)P2 + tail);
 }
 
 }  // namespace

@@ -20,7 +20,7 @@
 //
 // Work decomposition: one persistent 256-thread CTA per member (grid = #SMs).
 //   B  reference frames -> conv1 (25 m16 position tiles x 16 channels per frame);
-//      raw outputs go to a per-CTA global slab, shifted sums for mean / unbiased variance
+//      raw outputs go to a per-CTA global slab, Welford's mean / unbiased variance
 //      accumulate in shared memory (each (c,h,w) entry is owned by one thread: no atomics)
 //   C  reference frames: slab -> VBN1 -> ReLU -> split -> conv2 (6 m16 tiles x 32) -> stats
 //   D  observations: conv1 -> VBN1 -> ReLU -> conv2 -> VBN2 -> ReLU -> split features (slab)
@@ -39,6 +39,11 @@ constexpr int FC1 = 256;
 constexpr int NB = 32;                        // observations per fc1 tile (4 n8 fragments)
 constexpr int KPAD = 264;                     // row pitch (halves) of the conv weight tiles: conflict-free B loads
 constexpr float kLo = 4096.f, kLoInv = 1.f / 4096.f;
+// Activations (conv2's and fc1's inputs) are split at 2^-10 of their value and the GEMM result scaled back
+// (exact powers of two).  Over 0..255 frames with pixels that never change in the reference batch, VBN
+// outputs reach 1e6 (scale ~1/sqrt(1e-5) times a large difference): unscaled, hi overflows fp16's 65504 and
+// lo = (x - hi) * 2^12 already past 32768.  Scaled, both fit up to |x| ~ 3e7.
+constexpr float kAct = 1.f / 1024.f, kActInv = 1024.f;
 
 struct ConvTcParams {
   const float* theta;
@@ -73,6 +78,7 @@ __device__ __forceinline__ void split1(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn((x - __half2float(hi)) * kLo);
 }
+__device__ __forceinline__ void split_act(float x, __half& hi, __half& lo) { split1(x * kAct, hi, lo); }
 
 // d += a * b, m16n8k16, row.col, fp16 operands, fp32 accumulators
 __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -93,14 +99,11 @@ __device__ __forceinline__ uint32_t lds32(const __half* p) { return *reinterpret
 struct Smem {
   __half w1h[C1 * KPAD], w1l[C1 * KPAD];     // conv1 weights [co][k], k = ci*64 + kh*8 + kw
   __half w2h[C2 * KPAD], w2l[C2 * KPAD];     // conv2 weights [co][k], k = ci*16 + kh*4 + kw
-  float s1[P1], q1[P1];                      // VBN1: shifted sums, then scale a / shift c
-  float s2[P2], q2[P2], y2[P2];              // VBN2: shifted sums + shift, then a / c
+  float s1[P1], q1[P1];                      // VBN1: Welford mean / m2, then scale a / mean
+  float s2[P2], q2[P2];                      // VBN2: the same
   struct { __half h[CH], l[CH]; } img;       // one input channel, split
-  union {
-    float y1[P1];                            // VBN1 shift (first reference frame), phase B only
-    struct { __half h[P1], l[P1]; } x1;      // one frame's normalised layer-1 map [c][h][w], split
-  } u;
-  float small[128];                          // conv1.b 16, conv2.b 32
+  struct { __half h[P1], l[P1]; } x1;        // one frame's normalised layer-1 map [c][h][w], split
+  float small[128];                          // conv1.b 16, conv2.b 32, bn1.b 16, bn2.b 32
   float red[kT / 32];
 };
 // the fc phase reuses s1 / q1 for the hidden activations [NB][FC1]
@@ -142,6 +145,8 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
     }
     if (tid < 16) S.small[tid] = par(kC1b + tid);
     if (tid < 32) S.small[16 + tid] = par(kC2b + tid);
+    if (tid < 16) S.small[48 + tid] = par(kB1 + tid);
+    if (tid < 32) S.small[64 + tid] = par(kB2 + tid);
 
     // ---- conv1 of one frame: warp w owns position tiles w, w+8, w+16 (and 24 for warp 0);
     //      epi(tile, nb, acc) receives acc[4] = outputs (pos g / g+8, channels nb*8+2t, +1), bias added
@@ -227,8 +232,8 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
       const int kofs = (t >> 1) * W1 + (t & 1) * 2;   // a0: kh = t/2, kw = 2(t%2); a2: kh + 2
 #pragma unroll 2
       for (int ci = 0; ci < C1; ++ci) {
-        const __half* xh = S.u.x1.h + ci * HW1 + kofs;
-        const __half* xl = S.u.x1.l + ci * HW1 + kofs;
+        const __half* xh = S.x1.h + ci * HW1 + kofs;
+        const __half* xl = S.x1.l + ci * HW1 + kofs;
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
           const int nb = (warp + 8 * i) / 6;
@@ -243,10 +248,10 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
         const int u = warp + 8 * i, mt = u % 6, nb = u / 6;
         const float b0 = S.small[16 + nb * 8 + 2 * t], b1 = S.small[16 + nb * 8 + 2 * t + 1];
         float y[4];
-        y[0] = fmaf(ac[i][0], kLoInv, am[i][0]) + b0;
-        y[1] = fmaf(ac[i][1], kLoInv, am[i][1]) + b1;
-        y[2] = fmaf(ac[i][2], kLoInv, am[i][2]) + b0;
-        y[3] = fmaf(ac[i][3], kLoInv, am[i][3]) + b1;
+        y[0] = fmaf(fmaf(ac[i][0], kLoInv, am[i][0]), kActInv, b0);
+        y[1] = fmaf(fmaf(ac[i][1], kLoInv, am[i][1]), kActInv, b1);
+        y[2] = fmaf(fmaf(ac[i][2], kLoInv, am[i][2]), kActInv, b0);
+        y[3] = fmaf(fmaf(ac[i][3], kLoInv, am[i][3]), kActInv, b1);
         epi(mt, nb, y);
       }
     };
@@ -255,46 +260,44 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
     auto frag_ch = [&](int nb, int e) { return nb * 8 + 2 * t + (e & 1); };
 
     // ---------------- phase B: reference frames through conv1, VBN1 statistics
-    // shifted sums around the first frame's value: mean = y0 + s/R, var = (q - s*s/R)/(R-1)
+    // Welford's update in frame order (welford_add), as in the fp32 kernels: sums shifted by the first frame's
+    // value cancel when that frame is the outlier, (q - s*s/R) losing log2(R) bits
     for (int r = 0; r < p.R; ++r) {
       float* out = R1 + (size_t)r * P1;
+      const float inv = 1.f / (float)(r + 1);
       conv1_frame(p.xref + (size_t)r * IMG, [&](int pt, int nb, const float (&y)[4]) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int i = frag_ch(nb, e) * HW1 + frag_pos(pt, e);
           out[i] = y[e];
-          if (r == 0) { S.u.y1[i] = y[e]; S.s1[i] = 0.f; S.q1[i] = 0.f; }
-          else {
-            const float d = y[e] - S.u.y1[i];
-            S.s1[i] += d;
-            S.q1[i] = fmaf(d, d, S.q1[i]);
-          }
+          if (r == 0) { S.s1[i] = 0.f; S.q1[i] = 0.f; }
+          welford_add(y[e], inv, S.s1[i], S.q1[i]);
         }
       });
     }
     __syncthreads();
     {
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
       for (int i = tid; i < P1; i += kT) {
         const int co = i / HW1;
-        const float s = S.s1[i];
-        const float mean = S.u.y1[i] + s * invR;
-        const float var = fmaxf((S.q1[i] - s * (s * invR)) * invR1, 0.f);   // unbiased (modules.py:52)
+        const float mean = S.s1[i];
+        const float var = S.q1[i] * invR1;   // unbiased (modules.py:52)
         const float a = par(kG1 + co) / sqrtf(var + 1e-5f);
         S.s1[i] = a;
-        S.q1[i] = par(kB1 + co) - mean * a;
+        S.q1[i] = mean;
       }
     }
 
     // ---------------- phase C: reference frames through VBN1/ReLU/conv2, VBN2 statistics
     for (int r = 0; r < p.R; ++r) {
-      __syncthreads();   // previous frame's conv2 done with x1 (and phase B's y1 reads done)
+      __syncthreads();   // previous frame's conv2 done with x1 (and phase B's statistics final)
       const float* src = R1 + (size_t)r * P1;
+      const float inv = 1.f / (float)(r + 1);
       for (int i = tid; i < P1; i += kT) {
         __half h, l;
-        split1(fmaxf(fmaf(src[i], S.s1[i], S.q1[i]), 0.f), h, l);
-        S.u.x1.h[i] = h;
-        S.u.x1.l[i] = l;
+        split_act(fmaxf(fmaf(src[i] - S.q1[i], S.s1[i], S.small[48 + i / HW1]), 0.f), h, l);
+        S.x1.h[i] = h;
+        S.x1.l[i] = l;
       }
       __syncthreads();
       conv2_frame([&](int mt, int nb, const float (&y)[4]) {
@@ -303,26 +306,21 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
           const int pos = frag_pos(mt, e);
           if (pos >= HW2) continue;
           const int i = frag_ch(nb, e) * HW2 + pos;
-          if (r == 0) { S.y2[i] = y[e]; S.s2[i] = 0.f; S.q2[i] = 0.f; }
-          else {
-            const float d = y[e] - S.y2[i];
-            S.s2[i] += d;
-            S.q2[i] = fmaf(d, d, S.q2[i]);
-          }
+          if (r == 0) { S.s2[i] = 0.f; S.q2[i] = 0.f; }
+          welford_add(y[e], inv, S.s2[i], S.q2[i]);
         }
       });
     }
     __syncthreads();
     {
-      const float invR = 1.f / (float)p.R, invR1 = 1.f / (float)(p.R - 1);
+      const float invR1 = 1.f / (float)(p.R - 1);
       for (int i = tid; i < P2; i += kT) {
         const int co = i / HW2;
-        const float s = S.s2[i];
-        const float mean = S.y2[i] + s * invR;
-        const float var = fmaxf((S.q2[i] - s * (s * invR)) * invR1, 0.f);
+        const float mean = S.s2[i];
+        const float var = S.q2[i] * invR1;
         const float a = par(kG2 + co) / sqrtf(var + 1e-5f);
         S.s2[i] = a;
-        S.q2[i] = par(kB2 + co) - mean * a;
+        S.q2[i] = mean;
       }
     }
     // (the first conv1_frame below begins with a barrier that publishes s2 / q2)
@@ -334,9 +332,9 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
         for (int e = 0; e < 4; ++e) {
           const int i = frag_ch(nb, e) * HW1 + frag_pos(pt, e);
           __half h, l;
-          split1(fmaxf(fmaf(y[e], S.s1[i], S.q1[i]), 0.f), h, l);
-          S.u.x1.h[i] = h;
-          S.u.x1.l[i] = l;
+          split_act(fmaxf(fmaf(y[e] - S.q1[i], S.s1[i], S.small[48 + frag_ch(nb, e)]), 0.f), h, l);
+          S.x1.h[i] = h;
+          S.x1.l[i] = l;
         }
       });
       __syncthreads();
@@ -349,7 +347,7 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
           if (pos >= HW2) continue;
           const int i = frag_ch(nb, e) * HW2 + pos;
           __half h, l;
-          split1(fmaxf(fmaf(y[e], S.s2[i], S.q2[i]), 0.f), h, l);
+          split_act(fmaxf(fmaf(y[e] - S.q2[i], S.s2[i], S.small[64 + frag_ch(nb, e)]), 0.f), h, l);
           fh[i] = h;
           fl[i] = l;
         }
@@ -419,7 +417,7 @@ __global__ void __launch_bounds__(kT, 1) eval_conv_vbn_tc_kernel(const ConvTcPar
           for (int e = 0; e < 4; ++e) {
             const int ob = n * 8 + 2 * t + (e & 1);
             const int neuron = n0 + ((e >> 1) << 3);
-            const float h = fmaf(ac[m][n][e], kLoInv, am[m][n][e]) + ((e >> 1) ? bias1 : bias0);
+            const float h = fmaf(fmaf(ac[m][n][e], kLoInv, am[m][n][e]), kActInv, (e >> 1) ? bias1 : bias0);
             sH[ob * FC1 + neuron] = fmaxf(h, 0.f);
           }
         }

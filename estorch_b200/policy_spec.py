@@ -202,6 +202,8 @@ def conv_vbn_spec_from_module(module: nn.Module) -> Optional[ConvVBNSpec]:
         r2 = F.conv2d(r1n, c2.weight, c2.bias, stride=2)
         h2 = torch.relu(vbn(F.conv2d(h1, c2.weight, c2.bias, stride=2), r2, b2))
         want = F.linear(torch.relu(F.linear(h2.reshape(-1, 2592), f1.weight, f1.bias)), f2.weight, f2.bias)
-        if y.shape != want.shape or not torch.allclose(y, want, rtol=1e-3, atol=1e-4):
+        # max-norm relative, not element by element: over raw 0..255 reference frames that are constant at many
+        # pixels, VBN scales by ~1/sqrt(1e-5) and the small outputs carry amplified fp32 order differences
+        if y.shape != want.shape or not bool((y - want).abs().max() <= 1e-3 * want.abs().max() + 1e-4):
             return None
     return ConvVBNSpec(int(f2.out_features), int(xref.shape[0]))

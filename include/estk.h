@@ -324,8 +324,8 @@ ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precisio
  *   ESTK_PREC_F16   conv1, conv2 and fc1 on mma.sync with fp16 operands and fp32 accumulation;
  *                   every operand -- the weights theta + s*sigma*T[off+i] (formed in fp32 from the
  *                   fp32 theta and table16, the EXACT fp16 copy of `table` made by estk_shadow_f16),
- *                   the input frames and the normalised activations -- enters as hi + lo, two fp16
- *                   values (22 significant bits), so the returns stay within 1e-5 (max-norm
+ *                   the input frames and the normalised activations (those scaled by 2^-10 first, so
+ *                   values up to ~3e7 fit) -- enters as hi + lo, two fp16 values (22 significant bits), so the returns stay within 1e-5 (max-norm
  *                   relative) of the fp32 forward.  VBN statistics, normalisation, biases, fc2 and
  *                   the loss are fp32; no atomics, so the returns are the same bits run to run.
  *                   Population: table, table16.  theta, scratch and table16 16-byte aligned.
@@ -343,9 +343,11 @@ ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precisio
  * its meaning (the evaluate's scratch); here scratch holds the VBN statistics of every member,
  * [members][ESTK_CONV_VBN_STATS_FLOATS] fp32 in member order (the + members of the local pairs, then their
  * mirrors; the centre has one member), so scratch_bytes >= members * ESTK_CONV_VBN_STATS_FLOATS * 4, and
- * scratch is 16-byte aligned.  A member's entry is VBN1's scale and shift [16*20*20] each, then VBN2's
- * [32*9*9] each, folded as a = gamma / sqrtf(var + 1e-5f), c = beta - mean * a (gamma, beta the member's
- * perturbed parameters; mean, unbiased var over xref in the fp32 evaluate's accumulation order).  A call
+ * scratch is 16-byte aligned.  A member's entry is VBN1's scale a = gamma / sqrtf(var + 1e-5f) [16*20*20],
+ * then its mean [16*20*20], then VBN2's a and mean [32*9*9] each (gamma the member's perturbed parameter;
+ * mean and unbiased var over xref by Welford's update in frame order, d = y - mean, mean = fmaf(d, 1/n, mean),
+ * m2 = fmaf(d, y - mean, m2), var = m2/(R-1), which stays accurate where the mean is large and the variance
+ * near 0, e.g. 0..255 pixels that never change).  A call
  * runs one or both phases, the stats phase first:
  *   stats phase (xref != NULL): writes every member's statistics into scratch; ref_batch >= 2.  The raw
  *              conv1 outputs of the reference batch go through a per-CTA slab of the context workspace
@@ -357,7 +359,7 @@ ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precisio
  * A call with xref == NULL uses what an earlier stats call left in scratch; the caller must have made that
  * call for the same theta, offsets, pairs and sigma.  xref and obs both NULL is ESTK_ERR_INVALID.
  * Arithmetic, element by element that of the fp32 evaluate: W = theta +- (sigma*t) with two roundings,
- * conv1 / conv2 as fmaf chains from the bias in (ci, kh, kw) order, normalisation fmaxf(fmaf(y, a, c), 0),
+ * conv1 / conv2 as fmaf chains from the bias in (ci, kh, kw) order, normalisation fmaxf(fmaf(y - mean, a, beta), 0),
  * fc1 one chain from 0 in ascending k then + bias and ReLU, fc2 one chain from the bias -- a member's
  * outputs are the bits of the outputs its ESTK_PREC_FP32 evaluate computes on the same frames.  A member's
  * outputs never depend on another member's frames; no float atomics (the same bits from run to run, with

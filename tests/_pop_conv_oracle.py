@@ -1,9 +1,9 @@
 """TEST-ONLY: the action mode of estk_eval_conv_vbn (ESTK_ACTIONS) in numpy, an oracle stand-in backend that
 serves it, the Atari-example policy, and the deterministic pixel agent of the conv population tests and goldens.
 
-The oracle folds the VirtualBatchNorm statistics as the kernels do (a = gamma / sqrt(var + 1e-5),
-c = beta - mean * a, per (C, H, W) position; mean and unbiased var over the reference batch, estorch/
-modules.py:48-58) and runs the convolutions as fp32 matrix products, so it agrees with the kernels to fp32
+The oracle keeps the VirtualBatchNorm statistics as the kernels do (a = gamma / sqrt(var + 1e-5) and the
+mean per (C, H, W) position, normalising as (y - mean) * a + beta; mean and unbiased var over the reference
+batch, estorch/modules.py:48-58) and runs the convolutions as fp32 matrix products, so it agrees with the kernels to fp32
 accumulation order, not bit for bit."""
 import numpy as np
 import torch
@@ -69,23 +69,22 @@ def _params(rows, n_actions):
 
 
 def conv_stats(rows, n_actions, xref):
-    """rows [M, n], xref [R, 4, 84, 84] -> [M, STATS_FLOATS]: a1, c1 [16*20*20], a2, c2 [32*9*9] per member."""
+    """rows [M, n], xref [R, 4, 84, 84] -> [M, STATS_FLOATS]: a1, mean1 [16*20*20], a2, mean2 [32*9*9] per member."""
     p = _params(rows, n_actions)
     M = p["conv1.w"].shape[0]
     x = np.broadcast_to(np.asarray(xref, dtype=f32)[None], (M,) + tuple(xref.shape))
 
-    def fold(y, g, b):
+    def scale(y, g):
         mean = y.mean(axis=1, dtype=f32)
         var = y.var(axis=1, ddof=1, dtype=f32)
-        a = (g[:, :, None, None] / np.sqrt(var + f32(1e-5))).astype(f32)
-        return a, (b[:, :, None, None] - mean * a).astype(f32)
+        return (g[:, :, None, None] / np.sqrt(var + f32(1e-5))).astype(f32), mean
 
     r1 = _conv(x, p["conv1.w"], p["conv1.b"], 4)
-    a1, c1 = fold(r1, p["bn1.w"], p["bn1.b"])
-    h = np.maximum(r1 * a1[:, None] + c1[:, None], 0).astype(f32)
+    a1, m1 = scale(r1, p["bn1.w"])
+    h = np.maximum((r1 - m1[:, None]) * a1[:, None] + p["bn1.b"][:, None, :, None, None], 0).astype(f32)
     r2 = _conv(h, p["conv2.w"], p["conv2.b"], 2)
-    a2, c2 = fold(r2, p["bn2.w"], p["bn2.b"])
-    return np.concatenate([a1.reshape(M, -1), c1.reshape(M, -1), a2.reshape(M, -1), c2.reshape(M, -1)], 1)
+    a2, m2 = scale(r2, p["bn2.w"])
+    return np.concatenate([a1.reshape(M, -1), m1.reshape(M, -1), a2.reshape(M, -1), m2.reshape(M, -1)], 1)
 
 
 def conv_act(rows, n_actions, stats, obs):
@@ -93,10 +92,11 @@ def conv_act(rows, n_actions, stats, obs):
     p = _params(rows, n_actions)
     st = np.asarray(stats, dtype=f32)
     M = st.shape[0]
-    a1, c1 = st[:, :P1].reshape(M, 1, 16, 20, 20), st[:, P1:2 * P1].reshape(M, 1, 16, 20, 20)
-    a2, c2 = st[:, 2 * P1:2 * P1 + P2].reshape(M, 1, 32, 9, 9), st[:, 2 * P1 + P2:].reshape(M, 1, 32, 9, 9)
-    h = np.maximum(_conv(np.asarray(obs, dtype=f32), p["conv1.w"], p["conv1.b"], 4) * a1 + c1, 0).astype(f32)
-    h = np.maximum(_conv(h, p["conv2.w"], p["conv2.b"], 2) * a2 + c2, 0).astype(f32)
+    a1, m1 = st[:, :P1].reshape(M, 1, 16, 20, 20), st[:, P1:2 * P1].reshape(M, 1, 16, 20, 20)
+    a2, m2 = st[:, 2 * P1:2 * P1 + P2].reshape(M, 1, 32, 9, 9), st[:, 2 * P1 + P2:].reshape(M, 1, 32, 9, 9)
+    b1, b2 = p["bn1.b"][:, None, :, None, None], p["bn2.b"][:, None, :, None, None]
+    h = np.maximum((_conv(np.asarray(obs, dtype=f32), p["conv1.w"], p["conv1.b"], 4) - m1) * a1 + b1, 0).astype(f32)
+    h = np.maximum((_conv(h, p["conv2.w"], p["conv2.b"], 2) - m2) * a2 + b2, 0).astype(f32)
     h = h.reshape(M, h.shape[1], 2592)
     h = np.maximum(np.matmul(h, p["fc1.w"].transpose(0, 2, 1)) + p["fc1.b"][:, None], 0).astype(f32)
     return (np.matmul(h, p["fc2.w"].transpose(0, 2, 1)) + p["fc2.b"][:, None]).astype(f32)

@@ -125,14 +125,15 @@ def test_conv_f16_shapes_order_and_guards(be, R, B, A, use_order):
     f32 = _run(be, "fp32", A, theta, table, offs, order, pairs, sigma, xref, x, tgt)
     e16, e32 = rel_err(got, want), rel_err(f32, want)
     print(f"R={R} B={B} A={A} order={use_order}: f16 vs oracle {e16:.2e}, fp32 kernel vs oracle {e32:.2e}")
-    # With two or five random reference frames some (c,h,w) variances are near zero and VBN
-    # divides by them: returns reach -1e3 and both kernels' rounding is amplified.  The bar is
-    # 1e-5 or, where the fp32 kernel itself is that far off, a fixed multiple of its error.
-    assert e16 < max(1e-5, 20 * e32)
+    # With two random reference frames some (c,h,w) variances are near zero and VBN divides by
+    # them: returns reach -1e3 and the fp32 rounding of both kernels (and of the numpy oracle) is
+    # amplified to ~1e-4.  The bar is 1e-5 or, where the fp32 kernel itself is that far off, 8x its
+    # error (on an H100 the f16 kernel measured up to 1.7x for the population, 5.0x for the centre).
+    assert e16 < max(1e-5, 8 * e32)
     centre = _run(be, "f16", A, theta, None, None, None, 1, 0.0, xref, x, tgt, guard=8)[0]
     c32 = _run(be, "fp32", A, theta, None, None, None, 1, 0.0, xref, x, tgt)[0]
     wc = float(orc.synthetic_return(orc.atari_forward(theta, A, xref, x), tgt))
-    assert abs(centre - wc) < max(1e-5, 20 * abs(c32 - wc) / abs(wc)) * abs(wc)
+    assert abs(centre - wc) < max(1e-5, 8 * abs(c32 - wc) / abs(wc)) * abs(wc)
 
 
 # ------------------------------------------------------------------ 4. full size

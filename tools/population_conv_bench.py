@@ -80,13 +80,13 @@ def torch_step(rows, stats, obs, P):
     for s in sz:
         parts.append(rows[:, o:o + s])
         o += s
-    w1, b1, _, _, w2, b2, _, _, f1w, f1b, f2w, f2b = parts
-    a1, c1 = stats[:, :6400].view(P, 16, 20, 20), stats[:, 6400:12800].view(P, 16, 20, 20)
-    a2, c2 = stats[:, 12800:15392].view(P, 32, 9, 9), stats[:, 15392:].view(P, 32, 9, 9)
+    w1, b1, _, be1, w2, b2, _, be2, f1w, f1b, f2w, f2b = parts
+    a1, m1 = stats[:, :6400].view(P, 16, 20, 20), stats[:, 6400:12800].view(P, 16, 20, 20)
+    a2, m2 = stats[:, 12800:15392].view(P, 32, 9, 9), stats[:, 15392:].view(P, 32, 9, 9)
     x = F.conv2d(obs.view(1, P * 4, 84, 84), w1.reshape(P * 16, 4, 8, 8), b1.reshape(-1), stride=4, groups=P)
-    x = torch.relu(x.view(P, 16, 20, 20) * a1 + c1)
+    x = torch.relu((x.view(P, 16, 20, 20) - m1) * a1 + be1.view(P, 16, 1, 1))
     x = F.conv2d(x.view(1, P * 16, 20, 20), w2.reshape(P * 32, 16, 4, 4), b2.reshape(-1), stride=2, groups=P)
-    x = torch.relu(x.view(P, 32, 9, 9) * a2 + c2).view(P, 1, 2592)
+    x = torch.relu((x.view(P, 32, 9, 9) - m2) * a2 + be2.view(P, 32, 1, 1)).view(P, 1, 2592)
     h = torch.relu(torch.bmm(x, f1w.view(P, 256, 2592).transpose(1, 2)) + f1b[:, None])
     return torch.bmm(h, f2w.view(P, A, 256).transpose(1, 2)) + f2b[:, None]
 
