@@ -22,6 +22,9 @@ ESTK_ACT_TANH = 1
 ESTK_ACT_ELU = 3
 ESTK_ACT_SILU = 4
 ESTK_ACT_LEAKY_RELU = 5
+# recurrent cells in the hidden field, with ESTK_ACTIONS only: one GRUCell / LSTMCell step + a Linear head
+ESTK_CELL_GRU = 8
+ESTK_CELL_LSTM = 9
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
 ESTK_ACTIONS = 3 << 16

@@ -96,8 +96,16 @@ class PopulationAgent:
     every perturbed policy; ``members == 1`` is the unperturbed policy.  ``act`` never synchronises with
     the device, so an episode loop that keeps its state on the device runs without host round trips.
 
+    A recurrent policy -- one ``nn.GRUCell`` or ``nn.LSTMCell``, one ``nn.Linear`` head and optionally a Tanh
+    output, whose ``forward(x, state=None)`` returns ``(y, new_state)`` -- is stepped with
+    ``act(obs, state=None) -> (out, new_state)``.  ``state`` is h, ``[members, H]`` or ``[members, B, H]``
+    (GRU), or the pair (h, c) of those (LSTM), in the same member order as ``obs``; None means zeros, as in
+    torch.  In population mode one fused launch computes every member's cell step and head; the returned
+    state is the next call's ``state``, and the agent owns it (resetting it where an episode ends, say).
+
     ``rollout(policy)`` -- the reference protocol -- is ``rollout_population`` with ``members == 1`` and
-    ``act = policy``, so the same object also runs in hooks mode and under the reference itself.
+    ``act = policy`` (with the state passed through for a recurrent policy), so the same object also runs
+    in hooks mode and under the reference itself.
     ``device`` is where the agent creates its tensors; ``ES`` sets it to the engine's device in
     population mode and to the policy's device otherwise."""
 
@@ -109,12 +117,27 @@ class PopulationAgent:
 
     def rollout(self, policy):
         p = next(policy.parameters())
+
+        def act(o, *state):
+            if not state:                       # a memoryless policy: policy(obs)
+                return policy(o.to(p.device)).to(o.device)
+            y, s = policy(o.to(p.device), _state_to(state[0], p.device))
+            return y.to(o.device), _state_to(s, o.device)
         with torch.no_grad():
-            res = self.rollout_population(lambda o: policy(o.to(p.device)).to(o.device), 1)
+            res = self.rollout_population(act, 1)
         if isinstance(res, tuple):
             ret, bc = res
             return float(torch.as_tensor(ret).reshape(-1)[0]), torch.as_tensor(bc).reshape(1, -1)[0].cpu().numpy().copy()
         return float(torch.as_tensor(res).reshape(-1)[0])
+
+
+def _state_to(state, device):
+    """A recurrent state (None, h, or a tuple (h, c)) moved to ``device``."""
+    if state is None:
+        return None
+    if isinstance(state, (tuple, list)):
+        return tuple(s.to(device) for s in state)
+    return state.to(device)
 
 
 SyntheticAgent = DeviceAgent

@@ -241,6 +241,32 @@ class CudaBackend:
             B, per, None, self._stream()), "estk_eval_mlp[actions]")
         self.launches += 1
 
+    def act_rnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act, table16=None):
+        """One step of every perturbed recurrent policy (estk_eval_mlp with ESTK_CELL_GRU / ESTK_CELL_LSTM and
+        ESTK_ACTIONS, fp32).  ``dims`` = (in, H, out); ``act``: the cell | output code (ESTK_ACTIONS is added
+        here).  Population: ``obs`` ``[2*pairs, B, in + S]`` (x, then the state h, and c for LSTM) ->
+        ``out`` ``[2*pairs, B, out + S]`` (y, then h', and c'), S = H (GRU) or 2H (LSTM); ``offsets`` None =
+        the centre, ``[1, B, ...]`` for theta.  ``table16``: the exact fp16 copy of ``table``, read instead of it."""
+        M = 1 if offsets is None else 2 * int(pairs)
+        din, H, dout = (int(d) for d in dims)
+        S = H if (int(act) & 0xff) == _capi.ESTK_CELL_GRU else 2 * H
+        if obs.dim() != 3 or tuple(obs.shape) != (M, obs.shape[1], din + S) or \
+                tuple(out.shape) != (M, obs.shape[1], dout + S):
+            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match the recurrent policy "
+                             f"{[din, H, dout]} (state width {S}) for {M} members")
+        d = mlp_desc(dims, (int(act) & 0xffff) | _capi.ESTK_ACTIONS)
+        B, per = int(obs.shape[1]), int(obs.shape[1]) * (dout + S)
+        t32 = None if table16 is not None else table
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), _capi.ESTK_PREC_FP32, self._ptr(theta, torch.float32, "theta"), None,
+            self._ptr(t32, torch.float32, "table"), self._ptr(table16, torch.float16, "table16"),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+            float(sigma), self._ptr(obs, torch.float32, "obs"), None, B, None, None,
+            self._ptr(out, torch.float32, "out"),
+            None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size()),
+            B, per, None, self._stream()), "estk_eval_mlp[recurrent actions]")
+        self.launches += 1
+
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),
                                                              int(B)))

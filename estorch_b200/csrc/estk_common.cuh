@@ -33,15 +33,17 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
-// estk_mlp_desc.activation: the twenty-five defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
+// estk_mlp_desc.activation: the twenty-nine defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
 // LeakyReLU x output identity / Tanh with the squared error, x identity output with the cross-entropy,
-// and x output identity / Tanh with ESTK_ACTIONS)
+// and x output identity / Tanh with ESTK_ACTIONS; each recurrent cell GRU / LSTM x output identity / Tanh
+// with ESTK_ACTIONS)
 static inline bool estk_act_valid(int a) {
   const int h = a & 0xff, rest = a & ~0xff;
+  const bool actions = rest == ESTK_ACTIONS || rest == (ESTK_ACT_OUT_TANH | ESTK_ACTIONS);
+  if (h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM) return actions;
   const bool hidden = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
                       h == ESTK_ACT_LEAKY_RELU;
-  return hidden && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || rest == ESTK_ACTIONS ||
-                    rest == (ESTK_ACT_OUT_TANH | ESTK_ACTIONS));
+  return hidden && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions);
 }
 // a defined code whose loss field is ESTK_ACTIONS: no return, the outputs themselves (fp32 only)
 static inline bool estk_act_actions(int a) { return estk_act_valid(a) && (a & 0xff0000) == ESTK_ACTIONS; }
@@ -152,6 +154,12 @@ int eval_mlp_actions(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, co
                      const float* table, const uint16_t* table16, const int64_t* offsets, const int32_t* order,
                      int pairs, float sigma, const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs,
                      int bc_dim, const float* centre_return_out, cudaStream_t stream);
+// the same with a recurrent cell code (ESTK_CELL_GRU / ESTK_CELL_LSTM), after eval_mlp_actions' checks of
+// the precision and the pointers: one step of the cell + head kernel (estk_act_rnn.cu)
+int eval_rnn_actions(estk_ctx* ctx, const estk_mlp_desc& d, const float* theta, const float* table,
+                     const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
+                     const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs, int bc_dim,
+                     cudaStream_t stream);
 // ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
 // shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
 int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);

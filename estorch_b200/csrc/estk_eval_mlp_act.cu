@@ -241,6 +241,10 @@ int eval_mlp_actions(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, co
   ESTK_CHECK_ARG(bc_obs > 0 && bc_dim > 0, "%s: bc_obs/bc_dim must be positive", who);
   ESTK_CHECK_ARG(!centre_return_out, "%s: centre_return_out is not an ESTK_ACTIONS output", who);
   const estk_mlp_desc& d = *desc;
+  const int cell = d.activation & 0xff;
+  if (cell == ESTK_CELL_GRU || cell == ESTK_CELL_LSTM)
+    return eval_rnn_actions(ctx, d, theta, table, table16, offsets, order, pairs, sigma, obs, B, bc_plus, bc_minus,
+                            bc_obs, bc_dim, stream);
   ESTK_CHECK_ARG(d.n_layers >= 1 && d.n_layers <= ESTK_MAX_LAYERS, "%s: n_layers=%d", who, d.n_layers);
   int maxw = 0;
   for (int l = 0; l <= d.n_layers; ++l) {

@@ -19,11 +19,12 @@ Three execution modes, chosen per instance:
             overridden: a generation is a handful of kernel launches, nothing
             touches the host unless the user reads an attribute.
 * population -- PopulationAgent (environments stepped by user code, one per
-            member) + recognised MLP or conv + VirtualBatchNorm policy + Adam +
-            no hook overridden, on one GPU: every environment step is one launch
+            member) + recognised MLP, conv + VirtualBatchNorm or recurrent
+            (GRUCell / LSTMCell + Linear head) policy + Adam + no hook
+            overridden, on one GPU: every environment step is one launch
             that evaluates every perturbed policy on its member's own observation
-            (estk_eval_mlp / estk_eval_conv_vbn with ESTK_ACTIONS; the conv
-            policy's VBN statistics are one more launch per generation); ranks,
+            (and state) (estk_eval_mlp / estk_eval_conv_vbn with ESTK_ACTIONS; the
+            conv policy's VBN statistics are one more launch per generation); ranks,
             gradient and Adam as in fused mode.
 * hooks  -- anything else (host agents such as gym loops, custom subclasses
             overriding ``_sample_policy`` / ``_calculate_grad`` / ..., other
@@ -47,7 +48,7 @@ import torch
 from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
 from .agents import DeviceAgent, PopulationAgent
 from .backend import adam_desc, new_state, read_state, write_state
-from .policy_spec import ConvVBNSpec, conv_vbn_spec_from_module, mlp_spec_from_module
+from .policy_spec import ConvVBNSpec, RNNSpec, conv_vbn_spec_from_module, mlp_spec_from_module, rnn_spec_from_module
 from .population import LazyPopulation, NoiseHandle
 
 __all__ = ["ES", "NS_ES", "NSR_ES", "NSRA_ES", "rank_transformation"]
@@ -302,8 +303,12 @@ class ES:
         self.target = policy(**policy_kwargs).to(self.device)       # estorch.py:142
         parameters = torch.nn.utils.parameters_to_vector(self.target.parameters())
         self.n_parameters = parameters.shape[0]
-        self._spec = mlp_spec_from_module(self.target) or conv_vbn_spec_from_module(self.target)
+        # the recurrent recogniser comes last and draws from a private generator only: the global RNG stream
+        # that the other two leave behind is the one every policy saw before recurrent policies were recognised
+        self._spec = (mlp_spec_from_module(self.target) or conv_vbn_spec_from_module(self.target)
+                      or rnn_spec_from_module(self.target))
         self._is_conv = isinstance(self._spec, ConvVBNSpec)
+        self._is_rnn = isinstance(self._spec, RNNSpec)
         self._fused = self._decide_fused(optimizer)
         self._population = self._fused and isinstance(self.agent, PopulationAgent)
         if isinstance(self.agent, PopulationAgent):
@@ -403,6 +408,8 @@ class ES:
         if not (self._device_agent or population) or self._spec is None:
             return False
         if population and self.n_workers > 1:
+            return False
+        if self._is_rnn and not population:     # a recurrent policy has no device-agent evaluate: hooks mode
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -1046,6 +1053,8 @@ class ES:
         drawn offsets around ``slot.theta_prev`` (+ members first, then their mirrors); centre: M = 1, theta."""
         if self._is_conv:
             return self._population_act_conv(slot, centre)
+        if self._is_rnn:
+            return self._population_act_rnn(slot, centre)
         be, dims, dev, code = self._be, self._spec.dims, self._dev, self._spec.act
         M = 1 if centre else self.population_size
         t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
@@ -1064,6 +1073,49 @@ class ES:
                 be.act_mlp(dims, slot.theta_prev, self._table, self._offsets, self._order, self._pairs_local,
                            self.sigma, x3, out, act=code, table16=t16)
             return out[:, 0] if single else out
+        return act
+
+    def _population_act_rnn(self, slot, centre):
+        """``act(obs, state=None) -> (out, new_state)`` for a recurrent policy (RNNSpec): observations ``[M, in]``
+        or ``[M, B, in]``, the state h (GRU) or (h, c) (LSTM) of ``[M, H]`` or ``[M, B, H]`` tensors, None for
+        zeros.  One launch per call: the kernel's rows are [x | state] -> [y | state'] (estk_eval_mlp with
+        ESTK_CELL_GRU / ESTK_CELL_LSTM and ESTK_ACTIONS); the returned outputs and state are views of its
+        output rows."""
+        be, dev, spec = self._be, self._dev, self._spec
+        (din, H, dout), lstm = spec.dims, spec.cell == "lstm"
+        M = 1 if centre else self.population_size
+        # the fp32 table, not its fp16 copy: the step forms its tiles from scalar noise loads and is not bound by
+        # their bytes, and with the fp16 copy the LSTM step measured slower (DESIGN §9)
+
+        def act(obs, state=None):
+            x = torch.as_tensor(obs).to(device=dev, dtype=torch.float32)
+            single = x.dim() == 2
+            x3 = x.unsqueeze(1) if single else x
+            if x3.dim() != 3 or x3.shape[0] != M or x3.shape[2] != din:
+                raise ValueError(f"act: observations {tuple(x.shape)}, expected [{M}, {din}] or [{M}, B, {din}]")
+            lead = tuple(x.shape[:-1])
+            if state is None:
+                parts = [torch.zeros(*lead, H * (2 if lstm else 1), dtype=torch.float32, device=dev)]
+            else:
+                parts = list(state) if lstm else [state]
+                if len(parts) != (2 if lstm else 1) or any(not torch.is_tensor(p_) or tuple(p_.shape) != lead + (H,)
+                                                           for p_ in parts):
+                    want = f"(h, c), each [{', '.join(map(str, lead + (H,)))}]" if lstm else \
+                        f"h [{', '.join(map(str, lead + (H,)))}]"
+                    raise ValueError(f"act: the state must be None or {want}")
+                parts = [p_.to(device=dev, dtype=torch.float32) for p_ in parts]
+            xs = torch.cat([x] + parts, -1)
+            xs = (xs.unsqueeze(1) if single else xs).contiguous()
+            out = torch.empty(M, xs.shape[1], dout + spec.state_width, dtype=torch.float32, device=dev)
+            if centre:
+                be.act_rnn(spec.dims, slot.theta, None, None, None, 1, 0.0, xs, out, spec.act)
+            else:
+                be.act_rnn(spec.dims, slot.theta_prev, self._table, self._offsets, self._order, self._pairs_local,
+                           self.sigma, xs, out, spec.act)
+            if single:
+                out = out[:, 0]
+            y, h = out[..., :dout], out[..., dout:dout + H]
+            return y, ((h, out[..., dout + H:]) if lstm else h)
         return act
 
     def _population_act_conv(self, slot, centre):

@@ -7,7 +7,10 @@ architecture, so the module is inspected once: a chain
 SiLU or LeakyReLU (slope 0.01), the same on every hidden layer, whose parameters are registered in forward order
 (examples/cartpole_es.py:6-20, examples/nsra_es.py:52-67) becomes an ``MLPSpec``.
 Anything else returns ``None`` and the engine uses the materialising path (rows
-built on the device, rollout on the host).
+built on the device, rollout on the host).  The conv + VirtualBatchNorm policy of the
+Atari example becomes a ``ConvVBNSpec``, and a recurrent policy (one GRUCell / LSTMCell
+and one Linear head, ``forward(x, state=None) -> (y, new_state)``) an ``RNNSpec``, which
+population mode steps.
 """
 from __future__ import annotations
 
@@ -142,6 +145,128 @@ def mlp_spec_from_module(module: nn.Module, probe: bool = True) -> Optional[MLPS
         if len(hits) != 1 or not _matches(y, _chain(x, linears, own, *hits[0])):
             return None
     return MLPSpec(tuple(dims), *hits[0])
+
+
+_CELL_CODES = {"gru": 8, "lstm": 9}  # estk.h ESTK_CELL_GRU / ESTK_CELL_LSTM
+
+
+@dataclass(frozen=True)
+class RNNSpec:
+    """A recurrent policy: one ``nn.GRUCell`` / ``nn.LSTMCell`` (in -> H, with biases), then one ``nn.Linear``
+    head (H -> out, with bias), optionally a Tanh output; ``forward(x, state=None) -> (y, new_state)`` with
+    ``state`` = h (GRU) or (h, c) (LSTM), None meaning zeros."""
+    cell: str                   # "gru" or "lstm"
+    dims: tuple                 # (in, H, out)
+    output: str = "identity"    # "identity" or "tanh"
+
+    @property
+    def act(self) -> int:
+        """The ``estk_mlp_desc.activation`` code without ESTK_ACTIONS (include/estk.h)."""
+        return _CELL_CODES[self.cell] | _OUTPUT_CODES[self.output]
+
+    @property
+    def gates(self) -> int:
+        return 3 if self.cell == "gru" else 4
+
+    @property
+    def state_width(self) -> int:
+        """S: the floats of state per observation (h, and c for LSTM)."""
+        return self.dims[1] * (1 if self.cell == "gru" else 2)
+
+    @property
+    def n_parameters(self) -> int:
+        i, h, o = self.dims
+        return self.gates * h * (i + h + 2) + o * (h + 1)
+
+
+def _cell_step(cell, x, state, w_ih, w_hh, b_ih, b_hh):
+    """torch's GRUCell / LSTMCell step from explicit parameters; ``state`` None = zeros."""
+    H = w_hh.shape[1]
+    if cell == "gru":
+        h = torch.zeros(x.shape[0], H, dtype=x.dtype, device=x.device) if state is None else state
+        a = torch.nn.functional.linear(x, w_ih, b_ih).chunk(3, 1)
+        b = torch.nn.functional.linear(h, w_hh, b_hh).chunk(3, 1)
+        r, z = torch.sigmoid(a[0] + b[0]), torch.sigmoid(a[1] + b[1])
+        n = torch.tanh(a[2] + r * b[2])
+        return (1 - z) * n + z * h
+    h, c = (torch.zeros(x.shape[0], H, dtype=x.dtype, device=x.device),) * 2 if state is None else state
+    g = (torch.nn.functional.linear(x, w_ih, b_ih) + torch.nn.functional.linear(h, w_hh, b_hh)).chunk(4, 1)
+    c2 = torch.sigmoid(g[1]) * c + torch.sigmoid(g[0]) * torch.tanh(g[2])
+    return torch.sigmoid(g[3]) * torch.tanh(c2), c2
+
+
+def _max_rel_ok(y, want) -> bool:
+    return (torch.is_tensor(y) and y.shape == want.shape and
+            bool((y - want).abs().max() <= 1e-4 * want.abs().max() + 1e-5))
+
+
+def rnn_spec_from_module(module: nn.Module) -> Optional[RNNSpec]:
+    """Return the RNNSpec of ``module`` or None.
+
+    Structural test: the leaf modules are exactly one ``nn.GRUCell`` / ``nn.LSTMCell`` with ``bias=True``,
+    one ``nn.Linear`` with a bias whose input width is the cell's ``hidden_size``, and at most one
+    ``nn.Tanh``; the parameters are registered in the order cell, head.  Behavioural test: with parameters
+    redrawn at a scale that keeps every gate and output O(1), the module's ``forward(x, state)`` and
+    ``forward(x, None)`` are compared with the cell step + head for an identity and a Tanh output; the
+    module is accepted only when exactly one output matches both, and it matches under the module's own
+    parameters too.  Only a private ``torch.Generator`` draws: the global RNG stream is not touched.
+    Stacked cells, ``nn.GRU`` / ``nn.LSTM``, ``nn.RNNCell``, deeper heads, a Linear before the cell and a
+    forward that ignores the state all return None."""
+    leaves = _leaf_modules(module)
+    cells = [m for m in leaves if type(m) in (nn.GRUCell, nn.LSTMCell)]
+    linears = [m for m in leaves if type(m) is nn.Linear]
+    tanhs = [m for m in leaves if type(m) is nn.Tanh]
+    if len(cells) != 1 or len(linears) != 1 or len(tanhs) > 1 or len(leaves) != 2 + len(tanhs):
+        return None
+    cell, head = cells[0], linears[0]
+    if not cell.bias or head.bias is None or head.in_features != cell.hidden_size:
+        return None
+    params = list(module.parameters())
+    expect = [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh, head.weight, head.bias]
+    if len(params) != len(expect) or any(a is not b for a, b in zip(params, expect)):
+        return None
+    kind = "gru" if isinstance(cell, nn.GRUCell) else "lstm"
+    I, H, O = cell.input_size, cell.hidden_size, head.out_features
+    names = [n for n, _ in module.named_parameters()]
+    dev, dt = params[0].device, params[0].dtype
+    g = torch.Generator().manual_seed(0x5EED)
+    rnd = lambda *s: torch.randn(*s, generator=g, dtype=dt).to(dev)  # noqa: E731
+
+    def states():
+        return rnd(5, H) if kind == "gru" else (rnd(5, H), rnd(5, H))
+
+    def want(x, state, ps, output):
+        s = _cell_step(kind, x, state, *ps[:4])
+        h = s if kind == "gru" else s[0]
+        y = torch.nn.functional.linear(h, ps[4], ps[5])
+        return (torch.tanh(y) if output == "tanh" else y), s
+
+    def same(got, x, state, ps, output):
+        if not (isinstance(got, tuple) and len(got) == 2):
+            return False
+        y, s = want(x, state, ps, output)
+        if not _max_rel_ok(got[0], y):
+            return False
+        if kind == "gru":
+            return _max_rel_ok(got[1], s)
+        return (isinstance(got[1], tuple) and len(got[1]) == 2 and _max_rel_ok(got[1][0], s[0])
+                and _max_rel_ok(got[1][1], s[1]))
+
+    with torch.no_grad():
+        redrawn = [rnd(cell.weight_ih.shape[0], I) / I ** 0.5, rnd(cell.weight_hh.shape[0], H) / H ** 0.5,
+                   rnd(cell.weight_ih.shape[0]), rnd(cell.weight_ih.shape[0]), rnd(O, H) / H ** 0.5, rnd(O)]
+        own = [p.detach() for p in params]
+        xr, sr, x, s = rnd(5, I), states(), rnd(5, I), states()
+        try:
+            call = lambda ps, xx, ss: torch.func.functional_call(module, dict(zip(names, ps)), (xx, ss))  # noqa
+            got_r, got_r0, got, got0 = call(redrawn, xr, sr), call(redrawn, xr, None), call(own, x, s), call(own, x, None)
+        except Exception:
+            return None
+        hits = [o for o in ("identity", "tanh")
+                if same(got_r, xr, sr, redrawn, o) and same(got_r0, xr, None, redrawn, o)]
+        if len(hits) != 1 or not (same(got, x, s, own, hits[0]) and same(got0, x, None, own, hits[0])):
+            return None
+    return RNNSpec(kind, (I, H, O), hits[0])
 
 
 @dataclass(frozen=True)

@@ -85,8 +85,10 @@ typedef struct {
  *              ESTK_ACT_ELU (3) y > 0 ? y : expm1(y)             (torch.nn.ELU(), alpha = 1),
  *              ESTK_ACT_SILU (4) y / (1 + exp(-y))               (torch.nn.SiLU()),
  *              ESTK_ACT_LEAKY_RELU (5) y > 0 ? y : y * 0.01      (torch.nn.LeakyReLU(), slope 0.01);
- *              2 and every value above 5 are undefined (2 is kept unassigned: callers have used
- *              it as the example of a refused code);
+ *              or a recurrent cell, valid with ESTK_ACTIONS only (below):
+ *              ESTK_CELL_GRU (8) torch.nn.GRUCell, ESTK_CELL_LSTM (9) torch.nn.LSTMCell;
+ *              2, 6, 7 and every value above 9 are undefined (2 is kept unassigned: callers have
+ *              used it as the example of a refused code);
  *   bits 8-15  output activation, applied after the last Linear, before the squared
  *              error and the behaviour characteristic: 0 identity, ESTK_ACT_OUT_TANH tanh(y);
  *   bits 16-23 the loss, i.e. what a member's return is:
@@ -119,9 +121,32 @@ typedef struct {
  *              when every member is given the same observations.  A member's outputs never depend on
  *              another member's observations; no float atomics (the same bits from run to run, with
  *              or without order, from table or table16).  Any widths, any B >= 1.
+ *              Recurrent cells (ESTK_CELL_GRU / ESTK_CELL_LSTM in bits 0-7, with ESTK_ACTIONS and
+ *              an identity or ESTK_ACT_OUT_TANH output): one step of a policy that is one
+ *              GRUCell / LSTMCell (bias=True) followed by one Linear head.  n_layers must be 2 and
+ *              dims = (in, H, out).  The parameters are torch's, in registration order: weight_ih
+ *              [G*H][in], weight_hh [G*H][H], bias_ih [G*H], bias_hh [G*H] (G = 3 gates r, z, n
+ *              for GRU; G = 4 gates i, f, g, o for LSTM), then the head's weight [out][H] and bias.
+ *              The step is the function [x | state] -> [y | state']: obs rows are in + S wide
+ *              and output rows out + S, S = H (GRU: h) or 2H (LSTM: h then c); bc_plus /
+ *              bc_minus receive the output rows exactly as above (bc_obs = B, bc_dim =
+ *              B*(out+S) for all of them).  Arithmetic, fp32: W = theta +- (sigma*t) with two
+ *              roundings; per gate row the input half (x against weight_ih) and the hidden half
+ *              (h against weight_hh) are separate fmaf chains from 0 in ascending k, each + its own
+ *              bias, a = chain_ih + b_ih and b = chain_hh + b_hh; s(v) = 1.0f / (1.0f + expf(-v))
+ *              with an IEEE divide, tanhf as above.
+ *                GRU:  r = s(a_r + b_r), z = s(a_z + b_z), n = tanhf(fmaf(r, b_n, a_n)),
+ *                      h' = fmaf(z, h - n, n)          (= (1 - z)*n + z*h, torch's form)
+ *                LSTM: i = s(a_i + b_i), f = s(a_f + b_f), g = tanhf(a_g + b_g), o = s(a_o + b_o),
+ *                      c' = fmaf(f, c, i*g), h' = o * tanhf(c')
+ *              then the head is the act-mode layer above on h' (fmaf chain, + bias, tanhf for
+ *              ESTK_ACT_OUT_TANH).  Any other cell combination (another output or loss, n_layers
+ *              != 2) is refused by the general rule below; the same determinism guarantees hold.
  * The defined codes are, for each hidden kind h in {ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU,
  * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH, h | ESTK_LOSS_XENT, h | ESTK_ACTIONS
- * and h | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (25 codes).  Loss value 2 (0x20000) is undefined.
+ * and h | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (25 codes), and for each cell c in {ESTK_CELL_GRU,
+ * ESTK_CELL_LSTM}: c | ESTK_ACTIONS and c | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (4 codes, 29 in all).
+ * Loss value 2 (0x20000) is undefined.
  * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
  * and makes estk_eval_mlp_supported return 0.
@@ -140,6 +165,8 @@ typedef struct {
 #define ESTK_ACT_ELU 3
 #define ESTK_ACT_SILU 4
 #define ESTK_ACT_LEAKY_RELU 5
+#define ESTK_CELL_GRU 8
+#define ESTK_CELL_LSTM 9
 #define ESTK_ACT_OUT_TANH (1 << 8)
 #define ESTK_LOSS_XENT (1 << 16)
 #define ESTK_ACTIONS (3 << 16)
