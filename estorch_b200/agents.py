@@ -77,6 +77,55 @@ class DeviceAgent:
         return None
 
 
+class SequenceAgent(DeviceAgent):
+    """A fixed batch of sequences for a recurrent policy, evaluated by the fused CUDA kernel.
+
+    ``obs`` is ``[B, T, in]`` and ``target`` ``[B, T, out]``.  Every sequence starts from the zero state; at
+    step t the policy sees ``obs[:, t]`` and the state it returned at step t - 1.  The return scores all B*T
+    steps as ``DeviceAgent`` scores its batch: ``loss="mse"`` is minus the mean squared error over every
+    step and output, ``loss="cross_entropy"`` minus the mean over the B*T steps of each step's cross-entropy
+    (its target row holds class weights).  A step whose cross-entropy target row is all zeros contributes 0,
+    so a task can score only some steps, e.g. the last one.  The behaviour characteristic (NS family) is the
+    outputs of the first ``bc_obs`` sequences, flattened in (b, t, out) order, then ``[:bc_dim]``.
+
+    The policy is one ``nn.GRUCell`` or ``nn.LSTMCell``, one ``nn.Linear`` head and optionally a Tanh output,
+    whose ``forward(x, state=None)`` returns ``(y, new_state)`` (see ``PopulationAgent``); with Adam and no
+    overridden hook ``ES`` evaluates every perturbed member over the whole batch in one fused launch."""
+
+    def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0, *,
+                 loss: str = "mse"):
+        if obs.dim() != 3 or target.dim() != 3 or tuple(obs.shape[:2]) != tuple(target.shape[:2]) or \
+                obs.shape[1] < 1:
+            raise ValueError("obs must be [B, T, in] and target [B, T, out] with the same B and T >= 1")
+        super().__init__(obs.reshape(obs.shape[0], -1), target.reshape(target.shape[0], -1), bc_obs, bc_dim,
+                         loss=loss)
+        self.obs = self.obs.reshape(obs.shape)
+        self.target = self.target.reshape(target.shape)
+
+    def rollout(self, policy):
+        with torch.no_grad():
+            p = next(policy.parameters())
+            obs, tgt = self.obs.to(p.device), self.target.to(p.device)
+            state, ys = None, []
+            for t in range(obs.shape[1]):
+                # state None: policy(x), which is forward(x, state=None) for a recurrent policy
+                res = policy(obs[:, t]) if state is None else policy(obs[:, t], state)
+                if isinstance(res, tuple):
+                    y, state = res
+                else:                           # a memoryless policy: y only, and the state stays None
+                    y = res
+                ys.append(y)
+            out = torch.stack(ys, 1)            # [B, T, out]
+            if self.loss == "cross_entropy":
+                reward = float((tgt * torch.log_softmax(out, 2)).sum(2).mean())
+            else:
+                reward = float(-((out - tgt) ** 2).mean())
+            if self.bc_dim:
+                bc = out[:self.bc_obs].flatten()[:self.bc_dim].detach().cpu().numpy().copy()
+                return reward, bc
+        return reward
+
+
 class PopulationAgent:
     """An environment agent that steps one environment per population member, all members at once.
 

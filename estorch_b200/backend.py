@@ -41,14 +41,19 @@ def write_state(state: torch.Tensor, **fields):
     state.copy_(torch.from_numpy(rec.view(np.uint8).copy()))
 
 
-def mlp_desc(dims: Sequence[int], act: int = 0) -> _capi.EstkMlpDesc:
-    """``act``: the ``estk_mlp_desc.activation`` code (``MLPSpec.act``; 0 = ReLU hidden, identity output)."""
+def mlp_desc(dims: Sequence[int], act: int = 0, steps: int = 0) -> _capi.EstkMlpDesc:
+    """``act``: the ``estk_mlp_desc.activation`` code (``MLPSpec.act``; 0 = ReLU hidden, identity output).
+    ``steps``: T of a recurrent sequence evaluate, stored in ``dims[3]`` after ``dims = (in, H, out)``."""
     if not (2 <= len(dims) <= _capi.ESTK_MAX_LAYERS + 1):
         raise ValueError(f"MLP with {len(dims) - 1} Linear layers is outside 1..{_capi.ESTK_MAX_LAYERS}")
     d = _capi.EstkMlpDesc()
     d.n_layers = len(dims) - 1
     for i, w in enumerate(dims):
         d.dims[i] = int(w)
+    if steps:
+        if len(dims) != 3:
+            raise ValueError("steps belongs to a recurrent policy's dims = (in, H, out)")
+        d.dims[3] = int(steps)
     d.activation = int(act)
     return d
 
@@ -266,6 +271,34 @@ class CudaBackend:
             None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size()),
             B, per, None, self._stream()), "estk_eval_mlp[recurrent actions]")
         self.launches += 1
+
+    def eval_rnn_seq(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
+                     bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
+        """Sequence evaluate of a recurrent policy (estk_eval_mlp with ESTK_CELL_GRU / ESTK_CELL_LSTM and a
+        return, fp32): ``dims`` = (in, H, out), ``obs`` ``[B, T, in]``, ``target`` ``[B, T, out]``; ``act``: the
+        cell | output | loss code.  The arguments are ``eval_mlp``'s fp32 ones, so the engine calls either the
+        same way; ``precision`` other than "fp32" is refused by the library."""
+        code, _dt16 = self._precision(precision)
+        B, T = int(obs.shape[0]), int(obs.shape[1]) if obs.dim() == 3 else 0
+        if obs.dim() != 3 or tuple(obs.shape) != (B, T, dims[0]) or tuple(target.shape) != (B, T, dims[-1]):
+            raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match the recurrent "
+                             f"policy {list(dims)}: expected [B, T, {dims[0]}] / [B, T, {dims[-1]}]")
+        d = mlp_desc(dims, act, steps=T)
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"), None,
+            self._ptr(table, torch.float32, "table"), None, self._ptr(offsets, torch.int64, "offsets"),
+            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
+            self._ptr(target, torch.float32, "target"), B,
+            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
+            int(bc_obs), int(bc_dim), None, self._stream()), f"estk_eval_mlp[recurrent sequence, {precision}]")
+        self.launches += 1
+
+    def eval_rnn_seq_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
+                            precision="fp32", act=0):
+        """Unperturbed recurrent policy: ``ret_out[0]`` = return of theta, ``bc_out`` its behaviour characteristic."""
+        self.eval_rnn_seq(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
+                          bc_dim, precision=precision, act=act)
 
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),

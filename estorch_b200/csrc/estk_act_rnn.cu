@@ -67,8 +67,6 @@ __device__ __forceinline__ float ld_noise1h(const uint16_t* p) {
   return __half2float(__ushort_as_half(v));
 }
 
-__device__ __forceinline__ float sigmoid_rn(float v) { return __fdiv_rn(1.f, 1.f + expf(-v)); }
-
 template <int BC, int CELL, bool OUT_TANH, bool SLAB>
 __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p) {
   constexpr bool GRU = CELL == ESTK_CELL_GRU;
@@ -184,15 +182,15 @@ __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p)
       const float h = X[(size_t)(in + u) * ROWS + r];
       float hn, cn = 0.f;
       if constexpr (GRU) {
-        const float rg = sigmoid_rn(Gt[(size_t)u * ROWS + r]);
-        const float z = sigmoid_rn(Gt[(size_t)(H + u) * ROWS + r]);
+        const float rg = estk_sigmoid_rn(Gt[(size_t)u * ROWS + r]);
+        const float z = estk_sigmoid_rn(Gt[(size_t)(H + u) * ROWS + r]);
         const float n = tanhf(fmaf(rg, Gt[(size_t)(GH + u) * ROWS + r], Gt[(size_t)(2 * H + u) * ROWS + r]));
         hn = fmaf(z, h - n, n);
       } else {
-        const float ig = sigmoid_rn(Gt[(size_t)u * ROWS + r]);
-        const float fg = sigmoid_rn(Gt[(size_t)(H + u) * ROWS + r]);
+        const float ig = estk_sigmoid_rn(Gt[(size_t)u * ROWS + r]);
+        const float fg = estk_sigmoid_rn(Gt[(size_t)(H + u) * ROWS + r]);
         const float gg = tanhf(Gt[(size_t)(2 * H + u) * ROWS + r]);
-        const float og = sigmoid_rn(Gt[(size_t)(3 * H + u) * ROWS + r]);
+        const float og = estk_sigmoid_rn(Gt[(size_t)(3 * H + u) * ROWS + r]);
         const bool ok = b0 + b < p.B && !(centre && s);
         const float cc = ok ? __ldg(p.obs + ((size_t)member_of(s) * p.B + b0 + b) * XW + in + H + u) : 0.f;
         cn = fmaf(fg, cc, ig * gg);

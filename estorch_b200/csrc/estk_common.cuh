@@ -33,20 +33,22 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
-// estk_mlp_desc.activation: the twenty-nine defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
-// LeakyReLU x output identity / Tanh with the squared error, x identity output with the cross-entropy,
-// and x output identity / Tanh with ESTK_ACTIONS; each recurrent cell GRU / LSTM x output identity / Tanh
-// with ESTK_ACTIONS)
+// estk_mlp_desc.activation: the thirty-five defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
+// LeakyReLU and each recurrent cell GRU / LSTM x output identity / Tanh with the squared error, x identity
+// output with the cross-entropy, and x output identity / Tanh with ESTK_ACTIONS)
 static inline bool estk_act_valid(int a) {
   const int h = a & 0xff, rest = a & ~0xff;
   const bool actions = rest == ESTK_ACTIONS || rest == (ESTK_ACT_OUT_TANH | ESTK_ACTIONS);
-  if (h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM) return actions;
-  const bool hidden = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
-                      h == ESTK_ACT_LEAKY_RELU;
-  return hidden && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions);
+  const bool known = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
+                     h == ESTK_ACT_LEAKY_RELU || h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM;
+  return known && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions);
 }
 // a defined code whose loss field is ESTK_ACTIONS: no return, the outputs themselves (fp32 only)
 static inline bool estk_act_actions(int a) { return estk_act_valid(a) && (a & 0xff0000) == ESTK_ACTIONS; }
+// a defined code with a recurrent cell in bits 0-7 (ESTK_ACTIONS: one step; else the sequence evaluate)
+static inline bool estk_act_cell(int a) {
+  return estk_act_valid(a) && ((a & 0xff) == ESTK_CELL_GRU || (a & 0xff) == ESTK_CELL_LSTM);
+}
 
 #ifdef __CUDACC__
 // y / d rounded to nearest-even in fp32 -- the bits of the IEEE divide y / d -- for d >= 1 or d = +inf,
@@ -81,6 +83,10 @@ __device__ __forceinline__ float estk_hidden_act(float y) {
   else if constexpr (H == ESTK_ACT_LEAKY_RELU) return y > 0.f ? y : y * 0.01f;
   else return fmaxf(y, 0.f);
 }
+
+// the recurrent cells' s(v) = 1.0f / (1.0f + expf(-v)) with an IEEE divide (estk.h); the step and the
+// sequence kernels share it, so their outputs are the same bits
+__device__ __forceinline__ float estk_sigmoid_rn(float v) { return __fdiv_rn(1.f, 1.f + expf(-v)); }
 #endif
 
 // ---------------------------------------------------------------- context
@@ -160,6 +166,13 @@ int eval_rnn_actions(estk_ctx* ctx, const estk_mlp_desc& d, const float* theta, 
                      const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
                      const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs, int bc_dim,
                      cudaStream_t stream);
+// estk_eval_mlp with a recurrent cell code and a return (squared error or ESTK_LOSS_XENT): its own argument
+// checks, then the sequence evaluate over obs [B][T][in] (estk_eval_rnn_seq.cu)
+int eval_rnn_sequence(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta,
+                      const float* table, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
+                      const float* obs, const float* target, int B, float* returns_plus, float* returns_minus,
+                      float* bc_plus, float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out,
+                      cudaStream_t stream);
 // ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
 // shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
 int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);

@@ -606,6 +606,10 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
   if (desc && estk_act_actions(desc->activation))
     return eval_mlp_actions(ctx, desc, precision, theta, table, table16, offsets, order, pairs, sigma, obs, B,
                             bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, (cudaStream_t)stream);
+  if (desc && estk_act_cell(desc->activation))
+    return eval_rnn_sequence(ctx, desc, precision, theta, table, offsets, order, pairs, sigma, obs, target, B,
+                             returns_plus, returns_minus, bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out,
+                             (cudaStream_t)stream);
   ESTK_CHECK_ARG(tc || precision == ESTK_PREC_FP32, "estk_eval_mlp: unknown precision %d", precision);
   ESTK_CHECK_ARG(ctx && desc && theta && obs && target && returns_plus && (theta16 || !shadows) &&
                  (centre || (table && (table16 || !t16) && returns_minus)), "estk_eval_mlp: null argument");

@@ -46,7 +46,7 @@ import numpy as np
 import torch
 
 from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
-from .agents import DeviceAgent, PopulationAgent
+from .agents import DeviceAgent, PopulationAgent, SequenceAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import ConvVBNSpec, RNNSpec, conv_vbn_spec_from_module, mlp_spec_from_module, rnn_spec_from_module
 from .population import LazyPopulation, NoiseHandle
@@ -319,12 +319,15 @@ class ES:
         if self._population and eval_precision not in ("auto", "fp32"):
             raise ValueError("population mode (a PopulationAgent) computes every member's actions in fp32 only: "
                              "eval_precision must be 'auto' or 'fp32'")
+        if self._fused and self._is_rnn and eval_precision not in ("auto", "fp32"):
+            raise ValueError("the recurrent sequence evaluate (a SequenceAgent) is fp32 only: "
+                             "eval_precision must be 'auto' or 'fp32'")
         self._precision = "fp32"
         if self._fused and self._is_conv and eval_precision in ("bf16", "bf16s"):
             raise ValueError("the conv + VirtualBatchNorm evaluate kernel has 'fp32' and 'f16' modes only")
         if self._fused and self._is_conv and eval_precision == "f16":
             self._precision = "f16"
-        if self._fused and not self._is_conv and not self._population and eval_precision != "fp32":
+        if self._fused and not (self._is_conv or self._is_rnn or self._population) and eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
             act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
             supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
@@ -401,15 +404,17 @@ class ES:
         return not getattr(getattr(type(self), name), "_estk_builtin", False)
 
     def _decide_fused(self, optimizer_cls):
-        """Fused mode for a DeviceAgent, population mode for a PopulationAgent (a recognised MLP or conv +
-        VirtualBatchNorm policy on one GPU: the multi-GPU population generation is not implemented, hooks
-        mode serves it)."""
+        """Fused mode for a DeviceAgent (an MLP or conv + VirtualBatchNorm policy) or a SequenceAgent (a
+        recurrent policy), population mode for a PopulationAgent (a recognised MLP, conv + VirtualBatchNorm or
+        recurrent policy on one GPU: the multi-GPU population generation is not implemented, hooks mode
+        serves it)."""
         population = isinstance(self.agent, PopulationAgent)
         if not (self._device_agent or population) or self._spec is None:
             return False
         if population and self.n_workers > 1:
             return False
-        if self._is_rnn and not population:     # a recurrent policy has no device-agent evaluate: hooks mode
+        # a recurrent policy is evaluated over sequences, other policies over a batch of observations
+        if not population and self._is_rnn != isinstance(self.agent, SequenceAgent):
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -427,6 +432,10 @@ class ES:
                 return False
             if tuple(self.agent.obs.shape[1:]) != (4, 84, 84) or \
                     tuple(self.agent.target.shape[1:]) != (self._spec.n_actions,):
+                return False
+        elif self._is_rnn:
+            if tuple(self.agent.obs.shape[2:]) != (self._spec.dims[0],) or \
+                    tuple(self.agent.target.shape[2:]) != (self._spec.dims[-1],):
                 return False
         elif tuple(self.agent.obs.shape[1:]) != (self._spec.dims[0],) or \
                 tuple(self.agent.target.shape[1:]) != (self._spec.dims[-1],):
@@ -454,8 +463,8 @@ class ES:
         wants to observe episode_reward / the best snapshot before the next generation."""
         if getattr(self, "_pending_centre", False):
             slot = self._active
-            self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
-                                     **self._mlp_kw(slot, True))
+            self._eval_fns()[1](self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
+                                **self._mlp_kw(slot, True))
             self._be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
             self._pending_centre = False
             self._host_cache = {}
@@ -852,6 +861,12 @@ class ES:
             kw["table16"] = self._table16 if self._precision == "bf16s" else self._table_h
         return kw
 
+    def _eval_fns(self):
+        """(population, centre) evaluate of the fused generation: the recurrent sequence evaluate or the MLP one
+        (the same arguments)."""
+        be = self._be
+        return (be.eval_rnn_seq, be.eval_rnn_seq_center) if self._is_rnn else (be.eval_mlp, be.eval_mlp_center)
+
     def _act_code(self):
         """``estk_mlp_desc.activation`` of the MLP evaluate: the policy's activations (include/estk.h
         ESTK_ACT_*) and the agent's loss (ESTK_LOSS_XENT for ``loss="cross_entropy"``)."""
@@ -962,8 +977,8 @@ class ES:
             kw = self._mlp_kw(slot)
             if folded:        # the previous generation's post-update rollout rides in this launch
                 kw["centre_out"] = self._episode
-            be.eval_mlp(dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
-                        self._obs, self._tgt, ret_p, ret_m, **kw)
+            self._eval_fns()[0](dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
+                                self._obs, self._tgt, ret_p, ret_m, **kw)
             if folded:        # theta is still the previous update's result here (estorch.py:182-185)
                 be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
                 self._pending_centre = False
@@ -977,7 +992,7 @@ class ES:
             be.eval_conv_vbn(self._spec.n_actions, slot.theta, None, None, None, 1, 0.0, self._xref, self._obs,
                              self._tgt, self._episode, None, self._conv_scratch, **self._eval_kw(slot, True))
         else:
-            be.eval_mlp_center(dims, slot.theta, self._obs, self._tgt, self._episode, **self._mlp_kw(slot, True))
+            self._eval_fns()[1](dims, slot.theta, self._obs, self._tgt, self._episode, **self._mlp_kw(slot, True))
         be.track_best(slot.state, self._episode, slot.theta, slot.best_theta)
 
     # ------------------------------------------------------------------ CUDA-graph replay of a generation
@@ -1575,8 +1590,8 @@ class NS_ES(ES):
         if self._population:
             return self._population_centre(slot)
         ag = self.agent
-        self._be.eval_mlp_center(self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
-                                 self._bc_center[0], ag.bc_obs, ag.bc_dim, **self._mlp_kw(slot, True))
+        self._eval_fns()[1](self._spec.dims, slot.theta, self._obs, self._tgt, self._episode,
+                            self._bc_center[0], ag.bc_obs, ag.bc_dim, **self._mlp_kw(slot, True))
 
     def _archive_tensor(self):
         return torch.from_numpy(np.ascontiguousarray(np.stack(self._archive), dtype=np.float32)).to(self._dev)
@@ -1618,10 +1633,10 @@ class NS_ES(ES):
             R, N = self._returns, self._novelty
             ret_p, ret_m = R[pb: pb + pl], R[pairs + pb: pairs + pb + pl]
             nov_p, nov_m = N[pb: pb + pl], N[pairs + pb: pairs + pb + pl]
-        be.eval_mlp(dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
-                    self._obs, self._tgt, ret_p, ret_m,
-                    BC[pb: pb + pl], BC[pairs + pb: pairs + pb + pl], ag.bc_obs, ag.bc_dim,
-                    **self._mlp_kw(slot))
+        self._eval_fns()[0](dims, slot.theta, self._table, self._offsets, self._order, pl, self.sigma,
+                            self._obs, self._tgt, ret_p, ret_m,
+                            BC[pb: pb + pl], BC[pairs + pb: pairs + pb + pl], ag.bc_obs, ag.bc_dim,
+                            **self._mlp_kw(slot))
         be.knn_novelty(BC[pb: pb + pl], self._arch_dev, self.k, nov_p)
         be.knn_novelty(BC[pairs + pb: pairs + pb + pl], self._arch_dev, self.k, nov_m)
         self._update_step(slot, R, N, np.float32(self._w_rew()), np.float32(self._w_nov()), rm)

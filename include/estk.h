@@ -85,7 +85,7 @@ typedef struct {
  *              ESTK_ACT_ELU (3) y > 0 ? y : expm1(y)             (torch.nn.ELU(), alpha = 1),
  *              ESTK_ACT_SILU (4) y / (1 + exp(-y))               (torch.nn.SiLU()),
  *              ESTK_ACT_LEAKY_RELU (5) y > 0 ? y : y * 0.01      (torch.nn.LeakyReLU(), slope 0.01);
- *              or a recurrent cell, valid with ESTK_ACTIONS only (below):
+ *              or a recurrent cell (one step with ESTK_ACTIONS, or the sequence evaluate; below):
  *              ESTK_CELL_GRU (8) torch.nn.GRUCell, ESTK_CELL_LSTM (9) torch.nn.LSTMCell;
  *              2, 6, 7 and every value above 9 are undefined (2 is kept unassigned: callers have
  *              used it as the example of a refused code);
@@ -140,12 +140,34 @@ typedef struct {
  *                LSTM: i = s(a_i + b_i), f = s(a_f + b_f), g = tanhf(a_g + b_g), o = s(a_o + b_o),
  *                      c' = fmaf(f, c, i*g), h' = o * tanhf(c')
  *              then the head is the act-mode layer above on h' (fmaf chain, + bias, tanhf for
- *              ESTK_ACT_OUT_TANH).  Any other cell combination (another output or loss, n_layers
- *              != 2) is refused by the general rule below; the same determinism guarantees hold.
+ *              ESTK_ACT_OUT_TANH).  n_layers != 2 is ESTK_ERR_INVALID; the same determinism
+ *              guarantees hold.
+ * Recurrent sequence evaluate (a cell in bits 0-7 with the squared error, identity or ESTK_ACT_OUT_TANH
+ * output, or with ESTK_LOSS_XENT, identity output): every member runs over B sequences of T steps and
+ * its return scores all B*T steps.  n_layers = 2, dims = (in, H, out) as for the step and dims[3] = T >= 1
+ * (the entry a 2-layer desc otherwise leaves unused); obs is [B][T][in] and target [B][T][out], the same
+ * for every member.  Every member starts from a zero state (h, and c for LSTM); at step t it reads
+ * x = obs[b][t] and the state the previous step left, and computes the ESTK_ACTIONS step above element by
+ * element, so its outputs are the bits that T chained ESTK_ACTIONS launches produce when each launch is fed
+ * the previous launch's [h' | c'].  Per step (b, t) in fp32: the squared error s_bt = fmaf chain over c
+ * ascending from 0 of d*d, d = y_btc - t_btc; the cross-entropy ce_bt is the MLP formula above on y_bt
+ * (a step whose target row is all zeros then contributes 0 for finite logits: a task can score only some
+ * steps, e.g. the last; the return scales by a constant and the ranks do not change).  Then L_b = the sum
+ * of the step values over t in ascending order from 0, S = the sum of L_b over b in ascending order from 0
+ * (the work item of a pair that finishes last adds them), and return = -(S / (float)(B*T*out)) for the
+ * squared error, -(S / (float)(B*T)) for the cross-entropy (the integer count converted to fp32 once, an
+ * IEEE divide).  No float atomics: the same bits from run to run, with or without order; sigma = 0 gives
+ * every member the centre's return.  bc_plus / bc_minus receive y of the first bc_obs sequences flattened
+ * in (b, t, c) order, then [:bc_dim]; the population and centre forms are those of the MLP evaluate.
+ * ESTK_PREC_FP32 only, reading table (table16 is not read); a tensor-core precision, and a non-null
+ * centre_return_out, are ESTK_ERR_UNSUPPORTED before any launch; T < 1, a NULL target or NULL returns,
+ * and n_layers != 2 are ESTK_ERR_INVALID before any launch.  The per-sequence sums live in the context
+ * workspace (pairs * 2 * B floats; ESTK_ERR_NOMEM under capture when it must grow).
  * The defined codes are, for each hidden kind h in {ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU,
  * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH, h | ESTK_LOSS_XENT, h | ESTK_ACTIONS
  * and h | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (25 codes), and for each cell c in {ESTK_CELL_GRU,
- * ESTK_CELL_LSTM}: c | ESTK_ACTIONS and c | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (4 codes, 29 in all).
+ * ESTK_CELL_LSTM}: c | ESTK_ACTIONS and c | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (4 codes; the MLP and step
+ * codes, 29 in all; the sequence codes add 6: c, c | ESTK_ACT_OUT_TANH and c | ESTK_LOSS_XENT, 35 in all).
  * Loss value 2 (0x20000) is undefined.
  * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
@@ -325,10 +347,10 @@ ESTK_API int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t pre
                   float* centre_return_out, void* stream);
 
 /* 1 when the tensor-core `precision` (F16, BF16 or BF16S) can evaluate `desc` at batch B (the
- * shape rules above, and a defined activation code that computes a return, i.e. not ESTK_ACTIONS),
- * else 0 -- also for a null desc and for any other precision code.  F16_ANY: 1 for every desc with
- * 1..ESTK_MAX_LAYERS layers, positive widths and a defined activation code other than the
- * ESTK_ACTIONS ones, at every B >= 1. */
+ * shape rules above, and a defined activation code that computes a return, i.e. not ESTK_ACTIONS, and
+ * no recurrent cell), else 0 -- also for a null desc and for any other precision code.  F16_ANY: 1 for
+ * every desc with 1..ESTK_MAX_LAYERS layers, positive widths and a defined activation code other than
+ * the ESTK_ACTIONS and recurrent-cell ones, at every B >= 1. */
 ESTK_API int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B);
 
 /* ---- conv + VirtualBatchNorm policy of examples/atari.py:14-37 (BASELINE config 5):
