@@ -28,6 +28,23 @@ ESTK_CELL_LSTM = 9
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
 ESTK_ACTIONS = 3 << 16
+# bits 24-31: n_conv, the number of leading Conv2d layers of a convolutional policy (the CNN evaluate, fp32);
+# its dims[0] is ESTK_CNN_INPUT(c, h, w) and dims[1..n_conv] ESTK_CNN_CONV(out_c, k, stride, pad)
+ESTK_CNN_SHIFT = 24
+ESTK_CNN_MAX_CONV = 7
+
+
+def ESTK_CNN_N_CONV(n):
+    return int(n) << ESTK_CNN_SHIFT
+
+
+def ESTK_CNN_INPUT(c, h, w):
+    return int(c) | int(h) << 10 | int(w) << 20
+
+
+def ESTK_CNN_CONV(out_c, k, stride, pad):
+    return int(out_c) | int(k) << 12 | int(stride) << 18 | int(pad) << 24
+
 # estk_eval_conv_vbn with n_actions | ESTK_ACTIONS: VBN statistics per member, in floats
 ESTK_CONV_VBN_STATS_FLOATS = 17984
 # evaluate precision codes (estk_eval_mlp, estk_eval_conv_vbn)

@@ -58,6 +58,30 @@ def mlp_desc(dims: Sequence[int], act: int = 0, steps: int = 0) -> _capi.EstkMlp
     return d
 
 
+def cnn_desc(spec, code: int) -> _capi.EstkMlpDesc:
+    """The ``estk_mlp_desc`` of a convolutional policy: ``spec`` is a ``CNNSpec`` or its packed ``dims``
+    (``ESTK_CNN_INPUT``, one ``ESTK_CNN_CONV`` per conv, the Linear widths); ``code`` the activation code,
+    whose bits 24-31 hold n_conv."""
+    dims = spec.dims if hasattr(spec, "dims") else tuple(spec)
+    if not (code >> _capi.ESTK_CNN_SHIFT) & 0xff:
+        raise ValueError(f"activation code {code:#x} has no conv layers in bits 24-31")
+    d = _capi.EstkMlpDesc()
+    d.n_layers = len(dims) - 1
+    if not 1 <= d.n_layers <= _capi.ESTK_MAX_LAYERS:
+        raise ValueError(f"CNN with {len(dims) - 1} layers is outside 1..{_capi.ESTK_MAX_LAYERS}")
+    for i, w in enumerate(dims):
+        d.dims[i] = C.c_int32(int(w)).value
+    d.activation = C.c_int32(int(code)).value
+    return d
+
+
+def cnn_shapes(dims, code):
+    """((c, h, w), out) of the packed ``dims`` and activation ``code`` of a convolutional policy."""
+    dims = [int(x) & 0xffffffff for x in dims]
+    c, h, w = dims[0] & 1023, (dims[0] >> 10) & 1023, (dims[0] >> 20) & 1023
+    return (c, h, w), dims[-1]
+
+
 def adam_desc(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, clamp=1.0) -> _capi.EstkAdamDesc:
     a = _capi.EstkAdamDesc()
     a.lr, a.beta1, a.beta2, a.eps = float(lr), float(betas[0]), float(betas[1]), float(eps)
@@ -299,6 +323,36 @@ class CudaBackend:
         """Unperturbed recurrent policy: ``ret_out[0]`` = return of theta, ``bc_out`` its behaviour characteristic."""
         self.eval_rnn_seq(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
                           bc_dim, precision=precision, act=act)
+
+    def eval_cnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
+                 bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
+        """Fixed-batch evaluate of a convolutional policy (estk_eval_mlp with n_conv in bits 24-31 of ``act``,
+        fp32): ``dims`` the packed descriptor (``CNNSpec.dims``, or the spec itself), ``obs`` ``[B, c, h, w]``,
+        ``target`` ``[B, out]``.  The arguments are ``eval_mlp``'s fp32 ones, so the engine calls either the same
+        way; ``precision`` other than "fp32" is refused by the library."""
+        code, _dt16 = self._precision(precision)
+        d = cnn_desc(dims, act)
+        (c, h, w), out = cnn_shapes([d.dims[i] for i in range(d.n_layers + 1)], act)
+        B = int(obs.shape[0])
+        if tuple(obs.shape) != (B, c, h, w) or tuple(target.shape) != (B, out):
+            raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match the convolutional "
+                             f"policy: expected [B, {c}, {h}, {w}] / [B, {out}]")
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"), None,
+            self._ptr(table, torch.float32, "table"), None, self._ptr(offsets, torch.int64, "offsets"),
+            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
+            self._ptr(target, torch.float32, "target"), B,
+            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
+            int(bc_obs), int(bc_dim), None, self._stream()), f"estk_eval_mlp[convolutional, {precision}]")
+        self.launches += 1
+
+    def eval_cnn_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
+                        precision="fp32", act=0):
+        """Unperturbed convolutional policy: ``ret_out[0]`` = return of theta, ``bc_out`` its behaviour
+        characteristic."""
+        self.eval_cnn(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
+                      bc_dim, precision=precision, act=act)
 
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),

@@ -173,6 +173,12 @@ int eval_rnn_sequence(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, c
                       const float* obs, const float* target, int B, float* returns_plus, float* returns_minus,
                       float* bc_plus, float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out,
                       cudaStream_t stream);
+// estk_eval_mlp with n_conv != 0 in bits 24-31 of the activation code: its own argument checks, then the
+// convolutional evaluate over obs [B][c][h][w] (estk_eval_cnn.cu)
+int eval_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta, const float* table,
+             const int64_t* offsets, const int32_t* order, int pairs, float sigma, const float* obs,
+             const float* target, int B, float* returns_plus, float* returns_minus, float* bc_plus,
+             float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out, cudaStream_t stream);
 // ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
 // shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
 int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);

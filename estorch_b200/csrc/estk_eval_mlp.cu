@@ -603,6 +603,9 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
   const bool shadows = precision == ESTK_PREC_BF16S;                 // reads theta16, and table16 as a bf16 shadow
   const bool t16 = shadows || f16;                                   // a population reads table16
   const bool centre = offsets == nullptr;
+  if (desc && ((desc->activation >> 24) & 0xff) != 0)
+    return eval_cnn(ctx, desc, precision, theta, table, offsets, order, pairs, sigma, obs, target, B, returns_plus,
+                    returns_minus, bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, (cudaStream_t)stream);
   if (desc && estk_act_actions(desc->activation))
     return eval_mlp_actions(ctx, desc, precision, theta, table, table16, offsets, order, pairs, sigma, obs, B,
                             bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, (cudaStream_t)stream);

@@ -48,7 +48,8 @@ import torch
 from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
 from .agents import DeviceAgent, PopulationAgent, SequenceAgent
 from .backend import adam_desc, new_state, read_state, write_state
-from .policy_spec import ConvVBNSpec, RNNSpec, conv_vbn_spec_from_module, mlp_spec_from_module, rnn_spec_from_module
+from .policy_spec import (CNNSpec, ConvVBNSpec, RNNSpec, cnn_spec_from_module, conv_vbn_spec_from_module,
+                          mlp_spec_from_module, rnn_spec_from_module)
 from .population import LazyPopulation, NoiseHandle
 
 __all__ = ["ES", "NS_ES", "NSR_ES", "NSRA_ES", "rank_transformation"]
@@ -307,8 +308,14 @@ class ES:
         # that the other two leave behind is the one every policy saw before recurrent policies were recognised
         self._spec = (mlp_spec_from_module(self.target) or conv_vbn_spec_from_module(self.target)
                       or rnn_spec_from_module(self.target))
+        # a Conv2d stack does not fix H and W: the CNN recogniser takes the shape of a device agent's images,
+        # and comes after the other three for the same reason as the recurrent one
+        if self._spec is None and type(self.agent) is not SequenceAgent and isinstance(self.agent, DeviceAgent) \
+                and self.agent.obs.dim() == 4:
+            self._spec = cnn_spec_from_module(self.target, tuple(self.agent.obs.shape[1:]))
         self._is_conv = isinstance(self._spec, ConvVBNSpec)
         self._is_rnn = isinstance(self._spec, RNNSpec)
+        self._is_cnn = isinstance(self._spec, CNNSpec)
         self._fused = self._decide_fused(optimizer)
         self._population = self._fused and isinstance(self.agent, PopulationAgent)
         if isinstance(self.agent, PopulationAgent):
@@ -322,12 +329,16 @@ class ES:
         if self._fused and self._is_rnn and eval_precision not in ("auto", "fp32"):
             raise ValueError("the recurrent sequence evaluate (a SequenceAgent) is fp32 only: "
                              "eval_precision must be 'auto' or 'fp32'")
+        if self._fused and self._is_cnn and eval_precision not in ("auto", "fp32"):
+            raise ValueError("the convolutional evaluate (a Conv2d stack + Linear head) is fp32 only: "
+                             "eval_precision must be 'auto' or 'fp32'")
         self._precision = "fp32"
         if self._fused and self._is_conv and eval_precision in ("bf16", "bf16s"):
             raise ValueError("the conv + VirtualBatchNorm evaluate kernel has 'fp32' and 'f16' modes only")
         if self._fused and self._is_conv and eval_precision == "f16":
             self._precision = "f16"
-        if self._fused and not (self._is_conv or self._is_rnn or self._population) and eval_precision != "fp32":
+        if self._fused and not (self._is_conv or self._is_rnn or self._is_cnn or self._population) and \
+                eval_precision != "fp32":
             probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
             act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
             supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
@@ -404,10 +415,11 @@ class ES:
         return not getattr(getattr(type(self), name), "_estk_builtin", False)
 
     def _decide_fused(self, optimizer_cls):
-        """Fused mode for a DeviceAgent (an MLP or conv + VirtualBatchNorm policy) or a SequenceAgent (a
-        recurrent policy), population mode for a PopulationAgent (a recognised MLP, conv + VirtualBatchNorm or
-        recurrent policy on one GPU: the multi-GPU population generation is not implemented, hooks mode
-        serves it)."""
+        """Fused mode for a DeviceAgent (an MLP, conv + VirtualBatchNorm or generic Conv2d + Linear policy) or a
+        SequenceAgent (a recurrent policy), population mode for a PopulationAgent (a recognised MLP, conv +
+        VirtualBatchNorm or recurrent policy on one GPU: the multi-GPU population generation is not
+        implemented, hooks mode serves it).  A generic CNN with a PopulationAgent stays in hooks mode: it is
+        recognised for a DeviceAgent's images only (there is no population-mode CNN kernel)."""
         population = isinstance(self.agent, PopulationAgent)
         if not (self._device_agent or population) or self._spec is None:
             return False
@@ -415,6 +427,8 @@ class ES:
             return False
         # a recurrent policy is evaluated over sequences, other policies over a batch of observations
         if not population and self._is_rnn != isinstance(self.agent, SequenceAgent):
+            return False
+        if self._is_cnn and (population or isinstance(self.agent, SequenceAgent)):
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -432,6 +446,10 @@ class ES:
                 return False
             if tuple(self.agent.obs.shape[1:]) != (4, 84, 84) or \
                     tuple(self.agent.target.shape[1:]) != (self._spec.n_actions,):
+                return False
+        elif self._is_cnn:
+            if tuple(self.agent.obs.shape[1:]) != self._spec.input_shape or \
+                    tuple(self.agent.target.shape[1:]) != (self._spec.out,):
                 return False
         elif self._is_rnn:
             if tuple(self.agent.obs.shape[2:]) != (self._spec.dims[0],) or \
@@ -862,9 +880,11 @@ class ES:
         return kw
 
     def _eval_fns(self):
-        """(population, centre) evaluate of the fused generation: the recurrent sequence evaluate or the MLP one
-        (the same arguments)."""
+        """(population, centre) evaluate of the fused generation: the recurrent sequence evaluate, the
+        convolutional one or the MLP one (the same arguments)."""
         be = self._be
+        if self._is_cnn:
+            return be.eval_cnn, be.eval_cnn_center
         return (be.eval_rnn_seq, be.eval_rnn_seq_center) if self._is_rnn else (be.eval_mlp, be.eval_mlp_center)
 
     def _act_code(self):

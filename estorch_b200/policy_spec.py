@@ -270,6 +270,181 @@ def rnn_spec_from_module(module: nn.Module) -> Optional[RNNSpec]:
 
 
 @dataclass(frozen=True)
+class CNNSpec:
+    """A convolutional policy on a fixed batch: Conv2d layers (square kernel and stride, symmetric zero padding,
+    bias, groups 1, dilation 1), each followed by the hidden activation, then the output flattened in torch's
+    (c, h, w) order into Linear layers as in ``MLPSpec``."""
+    input_shape: tuple          # (c, h, w) of one observation
+    convs: tuple                # ((out_c, k, stride, pad), ...)
+    linears: tuple              # output widths of the Linear layers
+    hidden: str = "relu"
+    output: str = "identity"
+
+    def conv_shapes(self):
+        """[(c, h, w)] of the input and of every conv's output."""
+        c, h, w = self.input_shape
+        shapes = [(c, h, w)]
+        for oc, k, s, p in self.convs:
+            c, h, w = oc, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+            shapes.append((c, h, w))
+        return shapes
+
+    @property
+    def flat(self) -> int:
+        c, h, w = self.conv_shapes()[-1]
+        return c * h * w
+
+    @property
+    def out(self) -> int:
+        return self.linears[-1]
+
+    @property
+    def dims(self) -> tuple:
+        """The packed ``estk_mlp_desc.dims``: ESTK_CNN_INPUT(c, h, w), one ESTK_CNN_CONV per conv, the Linear
+        widths (include/estk.h)."""
+        c, h, w = self.input_shape
+        return ((c | h << 10 | w << 20,) + tuple(oc | k << 12 | s << 18 | p << 24 for oc, k, s, p in self.convs)
+                + tuple(self.linears))
+
+    @property
+    def act(self) -> int:
+        """The ``estk_mlp_desc.activation`` code: hidden | output | n_conv << 24."""
+        return _HIDDEN_CODES[self.hidden] | _OUTPUT_CODES[self.output] | len(self.convs) << 24
+
+    @property
+    def n_parameters(self) -> int:
+        n, shapes = 0, self.conv_shapes()
+        for (cin, _, _), (oc, k, _, _) in zip(shapes, self.convs):
+            n += oc * cin * k * k + oc
+        fan = self.flat
+        for o in self.linears:
+            n += o * fan + o
+            fan = o
+        return n
+
+
+def _cnn_chain(x, convs, linears, params, hidden, output):
+    F = torch.nn.functional
+    h, i = x, 0
+    for (_, k, s, p) in convs:
+        h = _HIDDEN[hidden][1](F.conv2d(h, params[i], params[i + 1], stride=s, padding=p))
+        i += 2
+    h = h.reshape(h.shape[0], -1)
+    for li in range(len(linears)):
+        h = F.linear(h, params[i], params[i + 1])
+        i += 2
+        if li + 1 < len(linears):
+            h = _HIDDEN[hidden][1](h)
+    return torch.tanh(h) if output == "tanh" else h
+
+
+def _conv_geometry(m: nn.Conv2d):
+    """(k, stride, pad) of a Conv2d the kernel computes, or None."""
+    if m.bias is None or m.groups != 1 or tuple(m.dilation) != (1, 1) or m.padding_mode != "zeros":
+        return None
+    k, s = tuple(m.kernel_size), tuple(m.stride)
+    if k[0] != k[1] or s[0] != s[1]:
+        return None
+    if isinstance(m.padding, str):
+        if m.padding != "valid":
+            return None
+        p = 0
+    else:
+        pp = tuple(m.padding)
+        if pp[0] != pp[1]:
+            return None
+        p = int(pp[0])
+    if not (1 <= k[0] <= 63 and 1 <= s[0] <= 63 and 0 <= p < k[0] and 1 <= m.out_channels <= 4095):
+        return None
+    return k[0], s[0], p
+
+
+def cnn_spec_from_module(module: nn.Module, input_shape) -> Optional[CNNSpec]:
+    """Return the CNNSpec of ``module`` on observations of shape ``input_shape`` = (c, h, w), or None.
+
+    Structural test: the leaf modules are Conv2d layers (``_conv_geometry``), then at most one default
+    ``nn.Flatten``, then Linear layers with biases, with activation modules of one hidden kind (default
+    parameters) anywhere; 1..7 convs, 1 + n_conv..8 layers; channels and widths chain from ``input_shape``; the
+    parameters are registered in forward order.  Behavioural test: as ``mlp_spec_from_module``'s, with
+    parameters redrawn at a scale that keeps every layer O(1); every (hidden, output) candidate is compared with
+    the module's forward and exactly one must match, under its own parameters too.  Only a private
+    ``torch.Generator`` draws: the global RNG stream is not touched.  MaxPool, BatchNorm, VirtualBatchNorm,
+    mixed kinds, a conv after a Linear and anything else return None."""
+    if len(tuple(input_shape)) != 3 or any(int(d) < 1 or int(d) > 1023 for d in input_shape):
+        return None
+    input_shape = tuple(int(d) for d in input_shape)
+    leaves = _leaf_modules(module)
+    acts = tuple(t for t, _ in _HIDDEN.values())
+    layers = [m for m in leaves if type(m) in (nn.Conv2d, nn.Linear)]
+    flats = [m for m in leaves if type(m) is nn.Flatten]
+    if any(not isinstance(m, (nn.Conv2d, nn.Linear, nn.Flatten) + acts) or not _default_params(m) for m in leaves):
+        return None
+    if any(type(m) not in (nn.Conv2d, nn.Linear, nn.Flatten) and type(m) not in acts for m in leaves):
+        return None
+    if len(flats) > 1 or any((f.start_dim, f.end_dim) != (1, -1) for f in flats):
+        return None
+    kinds_present = {type(m) for m in leaves if isinstance(m, acts)}
+    if len(kinds_present) > 2 or (len(kinds_present) == 2 and nn.Tanh not in kinds_present):
+        return None                     # mixed hidden kinds (a Tanh module may be the output)
+    n_conv = 0
+    while n_conv < len(layers) and type(layers[n_conv]) is nn.Conv2d:
+        n_conv += 1
+    linears = layers[n_conv:]
+    if not 1 <= n_conv <= 7 or not linears or len(layers) > 8 or any(type(m) is not nn.Linear for m in linears):
+        return None
+    if any(l.bias is None for l in linears):
+        return None
+    convs, c, h, w = [], *input_shape
+    for m in layers[:n_conv]:
+        g = _conv_geometry(m)
+        if g is None or m.in_channels != c:
+            return None
+        k, s, p = g
+        if h + 2 * p < k or w + 2 * p < k:
+            return None
+        convs.append((m.out_channels, k, s, p))
+        c, h, w = m.out_channels, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    fan = c * h * w
+    for l in linears:
+        if l.in_features != fan:
+            return None
+        fan = l.out_features
+    params = list(module.parameters())
+    expect = [t for m in layers for t in (m.weight, m.bias)]
+    if len(params) != len(expect) or any(a is not b for a, b in zip(params, expect)):
+        return None
+    kinds = [k for k, (t, _) in _HIDDEN.items() if t in kinds_present] or list(_HIDDEN)
+    outputs = ["identity"] + (["tanh"] if "tanh" in kinds else [])
+    cands = [(hk, o) for hk in kinds for o in outputs]
+    spec_convs, spec_lin = tuple(convs), tuple(l.out_features for l in linears)
+
+    def close(y, want):
+        return (torch.is_tensor(y) and y.shape == want.shape and
+                bool((y - want).abs().max() <= 1e-4 * want.abs().max() + 1e-5))
+
+    with torch.no_grad():
+        dev, dt = params[0].device, params[0].dtype
+        g = torch.Generator().manual_seed(0x5EED)
+        rnd = lambda *s: torch.randn(*s, generator=g, dtype=dt).to(dev)  # noqa: E731
+        redrawn = []
+        for m in layers:
+            fan_in = m.weight[0].numel()
+            redrawn += [rnd(*m.weight.shape) / fan_in ** 0.5, rnd(*m.bias.shape)]
+        names = [n for n, _ in module.named_parameters()]
+        xr, x = rnd(3, *input_shape), rnd(2, *input_shape)
+        own = [p_.detach() for p_ in params]
+        try:
+            yr = torch.func.functional_call(module, dict(zip(names, redrawn)), (xr,))
+            y = module(x)
+        except Exception:
+            return None
+        hits = [cd for cd in cands if close(yr, _cnn_chain(xr, spec_convs, spec_lin, redrawn, *cd))]
+        if len(hits) != 1 or not close(y, _cnn_chain(x, spec_convs, spec_lin, own, *hits[0])):
+            return None
+    return CNNSpec(input_shape, spec_convs, spec_lin, *hits[0])
+
+
+@dataclass(frozen=True)
 class ConvVBNSpec:
     """The conv + VirtualBatchNorm policy of the reference's Atari example
     (examples/atari.py:14-37): conv1 4->16 k8 s4, VBN(16), conv2 16->32 k4 s2,

@@ -163,6 +163,35 @@ typedef struct {
  * centre_return_out, are ESTK_ERR_UNSUPPORTED before any launch; T < 1, a NULL target or NULL returns,
  * and n_layers != 2 are ESTK_ERR_INVALID before any launch.  The per-sequence sums live in the context
  * workspace (pairs * 2 * B floats; ESTK_ERR_NOMEM under capture when it must grow).
+ * Convolutional evaluate (bits 24-31 = n_conv, 1..7: the number of leading Conv2d layers): a policy
+ * Conv2d -> act -> ... -> Conv2d -> act -> flatten -> Linear -> act -> ... -> Linear [-> out_act] over a fixed
+ * batch of B images.  dims[0] = ESTK_CNN_INPUT(c, h, w) (c, h, w in 1..1023); dims[1..n_conv] =
+ * ESTK_CNN_CONV(out_c, k, stride, pad), one per conv (out_c 1..4095, a square kernel k 1..63, stride 1..63,
+ * symmetric zero padding 0..63 with pad < k; dilation 1, groups 1); dims[n_conv+1..n_layers] are the Linear
+ * output widths, n_layers - n_conv >= 1.  The first Linear's input width is C*H*W of the last conv's output
+ * flattened in torch's (c, h, w) order -- derived, never passed.  A conv's output is H' = (H + 2*pad - k) /
+ * stride + 1 (and W' likewise), which must be >= 1.  Bits 0-23 keep their meaning: the hidden kind (ReLU,
+ * Tanh, ELU, SiLU, LeakyReLU) follows every conv and every Linear but the last, the output is identity or
+ * ESTK_ACT_OUT_TANH, the loss 0 (squared error) or ESTK_LOSS_XENT (identity output only).  The parameters
+ * are in parameters_to_vector order: each conv's weight [out_c][in_c][k][k] then its bias, then each Linear's
+ * weight [out][in] and bias.  obs is [B][c][h][w], target [B][out]; bc_plus / bc_minus receive
+ * policy(obs[:bc_obs]).flatten()[:bc_dim]; the population and centre forms are those of the MLP evaluate.
+ * Arithmetic, fp32: W = theta +- (sigma*t) with two roundings; each conv output is one fmaf chain from 0 over
+ * the taps in ascending (ci, kh, kw) order (taps in the zero padding contribute nothing), then + bias, then
+ * the hidden activation; each Linear output is the fp32 MLP evaluate's chain (from 0 in ascending k, + bias).
+ * So a conv whose kernel covers its whole input (k = h = w, stride 1, pad 0) computes the bits of the fp32
+ * MLP evaluate's first Linear on the flattened input.  The per-image value is the squared error, an fmaf
+ * chain over the outputs c ascending from 0 of d*d, d = y_bc - t_bc, or the cross-entropy ce_b of the MLP
+ * formula; S = the sum of the per-image values over b in ascending order from 0 (kept in the context
+ * workspace, pairs * 2 * B floats; the work item of a pair that finishes last adds them), and return =
+ * -(S / (float)(B*out)) for the squared error, -(S / (float)B) for the cross-entropy.  No float atomics: the
+ * same bits from run to run, whatever the chunking, the schedule or order; sigma = 0 gives every member the
+ * centre's bits.  ESTK_PREC_FP32 only, reading table: a tensor-core precision is ESTK_ERR_UNSUPPORTED before
+ * any other check of the code, as are a non-null centre_return_out and, under ESTK_PREC_FP32, ESTK_ACTIONS or
+ * a recurrent cell in bits 0-23.  n_conv > 7, undefined bits 0-23, malformed packed fields (zero channels,
+ * pad >= k, a conv larger than its padded input), n_layers <= n_conv, and more than 2^30 inputs, taps or
+ * outputs per image in one layer are ESTK_ERR_INVALID before any launch.  estk_eval_mlp_supported returns 0
+ * for every code with bits 24-31 != 0.
  * The defined codes are, for each hidden kind h in {ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU,
  * ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU}: h, h | ESTK_ACT_OUT_TANH, h | ESTK_LOSS_XENT, h | ESTK_ACTIONS
  * and h | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (25 codes), and for each cell c in {ESTK_CELL_GRU,
@@ -192,6 +221,11 @@ typedef struct {
 #define ESTK_ACT_OUT_TANH (1 << 8)
 #define ESTK_LOSS_XENT (1 << 16)
 #define ESTK_ACTIONS (3 << 16)
+/* the convolutional evaluate (above): n_conv in bits 24-31 of the activation code, packed dims */
+#define ESTK_CNN_N_CONV(n) ((int32_t)((uint32_t)(n) << 24))
+#define ESTK_CNN_INPUT(c, h, w) ((int32_t)((uint32_t)(c) | (uint32_t)(h) << 10 | (uint32_t)(w) << 20))
+#define ESTK_CNN_CONV(out_c, k, stride, pad) \
+  ((int32_t)((uint32_t)(out_c) | (uint32_t)(k) << 12 | (uint32_t)(stride) << 18 | (uint32_t)(pad) << 24))
 
 /* Arithmetic of the evaluate kernels (estk_eval_mlp, estk_eval_conv_vbn); what each one
  * computes is stated at those functions. */
