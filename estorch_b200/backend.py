@@ -134,8 +134,8 @@ class CudaBackend:
 
     # ---------------------------------------------------------------- helpers
     def _ptr(self, t: Optional[torch.Tensor], dtype=None, name="tensor"):
-        if t is None:
-            return None
+        if t is None or isinstance(t, C.c_void_p):   # no buffer, or a pointer made (and checked) by the caller
+            return t
         if t.device != self.device:
             raise ValueError(f"{name} is on {t.device}, backend is on {self.device}")
         if dtype is not None and t.dtype != dtype:
@@ -219,6 +219,22 @@ class CudaBackend:
                     "estk_shadow_bf16")
         self.launches += 1
 
+    def _eval_mlp(self, what, d, code, B, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus,
+                  ret_minus, bc_plus, bc_minus, bc_obs, bc_dim, dt16=None, theta16=None, table16=None, centre_out=None,
+                  launches=1):
+        """One estk_eval_mlp call on the current stream: ``d`` the descriptor, ``code`` the ESTK_PREC_* code,
+        ``dt16`` the dtype of theta16 / table16; ``what`` names the call in an error."""
+        _capi.check(self.lib.estk_eval_mlp(
+            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"),
+            self._ptr(theta16, dt16, "theta16"), self._ptr(table, torch.float32, "table"),
+            self._ptr(table16, dt16, "table16"), self._ptr(offsets, torch.int64, "offsets"),
+            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
+            self._ptr(target, torch.float32, "target"), int(B),
+            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
+            int(bc_obs), int(bc_dim), self._ptr(centre_out, torch.float32, "centre_out"), self._stream()), what)
+        self.launches += launches
+
     def eval_mlp(self, dims, theta, table, offsets, order, pairs, sigma, obs, target,
                  ret_plus, ret_minus, bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32",
                  theta16=None, table16=None, centre_out=None, act=0):
@@ -227,18 +243,11 @@ class CudaBackend:
         d = mlp_desc(dims, act)
         if obs.shape != (obs.shape[0], dims[0]) or target.shape != (obs.shape[0], dims[-1]):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match dims {list(dims)}")
-        _capi.check(self.lib.estk_eval_mlp(
-            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"),
-            self._ptr(theta16, dt16, "theta16"), self._ptr(table, torch.float32, "table"),
-            self._ptr(table16, dt16, "table16"), self._ptr(offsets, torch.int64, "offsets"),
-            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
-            self._ptr(target, torch.float32, "target"), int(obs.shape[0]),
-            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
-            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
-            int(bc_obs), int(bc_dim), self._ptr(centre_out, torch.float32, "centre_out"), self._stream()),
-            f"estk_eval_mlp[{precision}]")
         # "f16_any" off the cluster kernel's shapes: the observation split, then the streamed kernel
-        self.launches += 2 if precision == "f16_any" and not self.eval_supports_f16(dims, obs.shape[0], act) else 1
+        launches = 2 if precision == "f16_any" and not self.eval_supports_f16(dims, obs.shape[0], act) else 1
+        self._eval_mlp(f"estk_eval_mlp[{precision}]", d, code, obs.shape[0], theta, table, offsets, order, pairs,
+                       sigma, obs, target, ret_plus, ret_minus, bc_plus, bc_minus, bc_obs, bc_dim, dt16=dt16,
+                       theta16=theta16, table16=table16, centre_out=centre_out, launches=launches)
 
     def eval_mlp_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
                         precision="fp32", theta16=None, act=0):
@@ -252,23 +261,8 @@ class CudaBackend:
         of the local pairs, the rest their mirrors.  ``offsets`` None = the centre: ``obs`` / ``out``
         ``[1, B, ...]`` for theta.  ``act``: the policy's hidden / output code (ESTK_ACTIONS is added here);
         ``table16``: the exact fp16 copy of ``table``, read instead of it."""
-        M = 1 if offsets is None else 2 * int(pairs)
-        if obs.dim() != 3 or tuple(obs.shape) != (M, obs.shape[1], dims[0]) or \
-                tuple(out.shape) != (M, obs.shape[1], dims[-1]):
-            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match dims {list(dims)} for "
-                             f"{M} members")
-        d = mlp_desc(dims, (int(act) & 0xffff) | _capi.ESTK_ACTIONS)
-        B, per = int(obs.shape[1]), int(obs.shape[1]) * int(dims[-1])
-        t32 = None if table16 is not None else table
-        _capi.check(self.lib.estk_eval_mlp(
-            self._ctx, C.byref(d), _capi.ESTK_PREC_FP32, self._ptr(theta, torch.float32, "theta"), None,
-            self._ptr(t32, torch.float32, "table"), self._ptr(table16, torch.float16, "table16"),
-            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
-            float(sigma), self._ptr(obs, torch.float32, "obs"), None, B, None, None,
-            self._ptr(out, torch.float32, "out"),
-            None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size()),
-            B, per, None, self._stream()), "estk_eval_mlp[actions]")
-        self.launches += 1
+        self._act(dims, 0, "estk_eval_mlp[actions]", theta, table, offsets, order, pairs, sigma, obs, out, act,
+                  table16)
 
     def act_rnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act, table16=None):
         """One step of every perturbed recurrent policy (estk_eval_mlp with ESTK_CELL_GRU / ESTK_CELL_LSTM and
@@ -276,25 +270,24 @@ class CudaBackend:
         here).  Population: ``obs`` ``[2*pairs, B, in + S]`` (x, then the state h, and c for LSTM) ->
         ``out`` ``[2*pairs, B, out + S]`` (y, then h', and c'), S = H (GRU) or 2H (LSTM); ``offsets`` None =
         the centre, ``[1, B, ...]`` for theta.  ``table16``: the exact fp16 copy of ``table``, read instead of it."""
-        M = 1 if offsets is None else 2 * int(pairs)
         din, H, dout = (int(d) for d in dims)
         S = H if (int(act) & 0xff) == _capi.ESTK_CELL_GRU else 2 * H
-        if obs.dim() != 3 or tuple(obs.shape) != (M, obs.shape[1], din + S) or \
-                tuple(out.shape) != (M, obs.shape[1], dout + S):
-            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match the recurrent policy "
-                             f"{[din, H, dout]} (state width {S}) for {M} members")
+        self._act(dims, S, "estk_eval_mlp[recurrent actions]", theta, table, offsets, order, pairs, sigma, obs, out,
+                  act, table16)
+
+    def _act(self, dims, S, what, theta, table, offsets, order, pairs, sigma, obs, out, act, table16):
+        """act_mlp (``S`` = 0) and act_rnn (``S`` the width of the recurrent state after x in obs and y in out)."""
+        M = 1 if offsets is None else 2 * int(pairs)
+        if obs.dim() != 3 or tuple(obs.shape) != (M, obs.shape[1], dims[0] + S) or \
+                tuple(out.shape) != (M, obs.shape[1], dims[-1] + S):
+            policy = f"the recurrent policy {[int(w) for w in dims]} (state width {S})" if S else f"dims {list(dims)}"
+            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match {policy} for {M} members")
         d = mlp_desc(dims, (int(act) & 0xffff) | _capi.ESTK_ACTIONS)
-        B, per = int(obs.shape[1]), int(obs.shape[1]) * (dout + S)
-        t32 = None if table16 is not None else table
-        _capi.check(self.lib.estk_eval_mlp(
-            self._ctx, C.byref(d), _capi.ESTK_PREC_FP32, self._ptr(theta, torch.float32, "theta"), None,
-            self._ptr(t32, torch.float32, "table"), self._ptr(table16, torch.float16, "table16"),
-            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
-            float(sigma), self._ptr(obs, torch.float32, "obs"), None, B, None, None,
-            self._ptr(out, torch.float32, "out"),
-            None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size()),
-            B, per, None, self._stream()), "estk_eval_mlp[recurrent actions]")
-        self.launches += 1
+        B, per = int(obs.shape[1]), int(obs.shape[1]) * (int(dims[-1]) + S)
+        minus = None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * per * out.element_size())
+        self._eval_mlp(what, d, _capi.ESTK_PREC_FP32, B, theta, None if table16 is not None else table, offsets,
+                       order, pairs, sigma, obs, None, None, None, self._ptr(out, torch.float32, "out"), minus, B, per,
+                       dt16=torch.float16, table16=table16)
 
     def eval_rnn_seq(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
                      bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
@@ -307,16 +300,9 @@ class CudaBackend:
         if obs.dim() != 3 or tuple(obs.shape) != (B, T, dims[0]) or tuple(target.shape) != (B, T, dims[-1]):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match the recurrent "
                              f"policy {list(dims)}: expected [B, T, {dims[0]}] / [B, T, {dims[-1]}]")
-        d = mlp_desc(dims, act, steps=T)
-        _capi.check(self.lib.estk_eval_mlp(
-            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"), None,
-            self._ptr(table, torch.float32, "table"), None, self._ptr(offsets, torch.int64, "offsets"),
-            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
-            self._ptr(target, torch.float32, "target"), B,
-            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
-            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
-            int(bc_obs), int(bc_dim), None, self._stream()), f"estk_eval_mlp[recurrent sequence, {precision}]")
-        self.launches += 1
+        self._eval_mlp(f"estk_eval_mlp[recurrent sequence, {precision}]", mlp_desc(dims, act, steps=T), code, B,
+                       theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus, bc_plus,
+                       bc_minus, bc_obs, bc_dim)
 
     def eval_rnn_seq_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
                             precision="fp32", act=0):
@@ -337,15 +323,8 @@ class CudaBackend:
         if tuple(obs.shape) != (B, c, h, w) or tuple(target.shape) != (B, out):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match the convolutional "
                              f"policy: expected [B, {c}, {h}, {w}] / [B, {out}]")
-        _capi.check(self.lib.estk_eval_mlp(
-            self._ctx, C.byref(d), code, self._ptr(theta, torch.float32, "theta"), None,
-            self._ptr(table, torch.float32, "table"), None, self._ptr(offsets, torch.int64, "offsets"),
-            self._ptr(order, torch.int32, "order"), int(pairs), float(sigma), self._ptr(obs, torch.float32, "obs"),
-            self._ptr(target, torch.float32, "target"), B,
-            self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
-            self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
-            int(bc_obs), int(bc_dim), None, self._stream()), f"estk_eval_mlp[convolutional, {precision}]")
-        self.launches += 1
+        self._eval_mlp(f"estk_eval_mlp[convolutional, {precision}]", d, code, B, theta, table, offsets, order, pairs,
+                       sigma, obs, target, ret_plus, ret_minus, bc_plus, bc_minus, bc_obs, bc_dim)
 
     def eval_cnn_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
                         precision="fp32", act=0):

@@ -445,71 +445,70 @@ int launch_act(estk_ctx* ctx, ActParams& p, cudaStream_t stream) {
 
 }  // namespace
 
-int eval_conv_actions(estk_ctx* ctx, int precision, int32_t code, const float* theta, const float* table,
-                      const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                      const float* xref, int ref_batch, const float* obs, int B, float* returns_plus,
-                      float* returns_minus, void* scratch, int64_t scratch_bytes, cudaStream_t stream) {
+int eval_conv_actions(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream) {
   const char* who = "estk_eval_conv_vbn[ESTK_ACTIONS]";
-  if (precision != ESTK_PREC_FP32) {
-    estk_set_error("%s: actions are computed with ESTK_PREC_FP32 only (precision %d)", who, precision);
+  if (c.precision != ESTK_PREC_FP32) {
+    estk_set_error("%s: actions are computed with ESTK_PREC_FP32 only (precision %d)", who, c.precision);
     return ESTK_ERR_UNSUPPORTED;
   }
-  const int A = code & 0xff;
-  const bool centre = offsets == nullptr;
-  ESTK_CHECK_ARG((code & ~0xff) == ESTK_ACTIONS && A >= 1 && A <= 64,
+  const int A = c.A & 0xff;
+  const bool centre = c.offsets == nullptr;
+  ESTK_CHECK_ARG((c.A & ~0xff) == ESTK_ACTIONS && A >= 1 && A <= 64,
                  "%s: n_actions=0x%x (bits 0-7 the action count 1..64, bits 8-15 zero, bits 16-23 ESTK_ACTIONS)",
-                 who, (unsigned)code);
-  ESTK_CHECK_ARG(xref || obs, "%s: xref and obs are both NULL (a call runs the stats phase, the act phase or both)",
-                 who);
-  ESTK_CHECK_ARG(ctx && theta && scratch && (centre || table || table16),
+                 who, (unsigned)c.A);
+  ESTK_CHECK_ARG(c.xref || c.obs,
+                 "%s: xref and obs are both NULL (a call runs the stats phase, the act phase or both)", who);
+  ESTK_CHECK_ARG(ctx && c.theta && c.scratch && (centre || c.table || c.table16),
                  "%s: null argument (theta, scratch, and for a population table or table16)", who);
-  ESTK_CHECK_ARG(!obs || (returns_plus && (centre || returns_minus)),
+  ESTK_CHECK_ARG(!c.obs || (c.ret_plus && (centre || c.ret_minus)),
                  "%s: the act phase needs returns_plus (and returns_minus for a population)", who);
-  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, pairs);
-  ESTK_CHECK_ARG(!xref || (ref_batch >= 2 && ESTK_ALIGNED16(xref)),
+  ESTK_CHECK_ARG(centre || (c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, c.pairs);
+  ESTK_CHECK_ARG(!c.xref || (c.R >= 2 && ESTK_ALIGNED16(c.xref)),
                  "%s: the stats phase needs ref_batch >= 2 (unbiased variance) and a 16-byte aligned xref", who);
-  ESTK_CHECK_ARG(!obs || (B >= 1 && ESTK_ALIGNED16(obs)), "%s: the act phase needs B >= 1 and 16-byte aligned obs",
-                 who);
-  ESTK_CHECK_ARG(ESTK_ALIGNED16(scratch), "%s: scratch must be 16-byte aligned", who);
-  const int members = centre ? 1 : 2 * pairs;
+  ESTK_CHECK_ARG(!c.obs || (c.B >= 1 && ESTK_ALIGNED16(c.obs)),
+                 "%s: the act phase needs B >= 1 and 16-byte aligned obs", who);
+  ESTK_CHECK_ARG(ESTK_ALIGNED16(c.scratch), "%s: scratch must be 16-byte aligned", who);
+  const int members = centre ? 1 : 2 * c.pairs;
   const int64_t need = (int64_t)members * ESTK_CONV_VBN_STATS_FLOATS * (int64_t)sizeof(float);
-  ESTK_CHECK_ARG(scratch_bytes >= need, "%s: scratch %lld < %lld bytes (members * ESTK_CONV_VBN_STATS_FLOATS * 4)",
-                 who, (long long)scratch_bytes, (long long)need);
+  ESTK_CHECK_ARG(c.scratch_bytes >= need,
+                 "%s: scratch %lld < %lld bytes (members * ESTK_CONV_VBN_STATS_FLOATS * 4)", who,
+                 (long long)c.scratch_bytes, (long long)need);
 
-  const int nb = !obs ? 1 : B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
+  const int B = c.B, nb = !c.obs ? 1 : B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
   const int stats_grid = std::min(ctx->sm_count, members);
-  const int64_t chunks = obs ? (B + nb - 1) / nb : 1;
-  const int act_grid = (int)std::min<int64_t>((centre ? 1 : pairs) * chunks, ctx->sm_count);
+  const int64_t chunks = c.obs ? (B + nb - 1) / nb : 1;
+  const int act_grid = (int)std::min<int64_t>((centre ? 1 : c.pairs) * chunks, ctx->sm_count);
   int64_t slab = 0;
-  if (xref) slab = (int64_t)stats_grid * ref_batch * P1;
-  if (obs && nb == 8) slab = std::max<int64_t>(slab, (int64_t)act_grid * 2 * 8 * P2);
+  if (c.xref) slab = (int64_t)stats_grid * c.R * P1;
+  if (c.obs && nb == 8) slab = std::max<int64_t>(slab, (int64_t)act_grid * 2 * 8 * P2);
   if (slab) {
     const int rc = estk_ctx_reserve(ctx, 0, 0, stream, who, slab);
     if (rc) return rc;
   }
-  float* const stats = reinterpret_cast<float*>(scratch);
-  if (xref) {
+  float* const stats = reinterpret_cast<float*>(c.scratch);
+  if (c.xref) {
     StatsParams s = {};
-    s.theta = theta; s.offsets = offsets; s.R = ref_batch; s.xref = xref; s.stats = stats; s.slab = ctx->eval_slab;
+    s.theta = c.theta; s.offsets = c.offsets; s.R = c.R; s.xref = c.xref; s.stats = stats; s.slab = ctx->eval_slab;
     s.members = members;
     if (centre) {
       s.pairs = 1;
     } else {
-      s.table = table; s.table16 = table16; s.order = order; s.pairs = pairs; s.sigma = sigma;
+      s.table = c.table; s.table16 = c.table16; s.order = c.order; s.pairs = c.pairs; s.sigma = c.sigma;
     }
     const size_t smem = stats_smem_bytes();
     ESTK_CUDA(cudaFuncSetAttribute(conv_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     conv_stats_kernel<<<stats_grid, kT, smem, stream>>>(s);
     ESTK_CUDA(cudaGetLastError());
   }
-  if (!obs) return ESTK_OK;
+  if (!c.obs) return ESTK_OK;
   ActParams a = {};
-  a.theta = theta; a.offsets = offsets; a.A = A; a.B = B; a.chunks = (int)chunks; a.obs = obs; a.stats = stats;
-  a.out_plus = returns_plus;
+  a.theta = c.theta; a.offsets = c.offsets; a.A = A; a.B = B; a.chunks = (int)chunks; a.obs = c.obs; a.stats = stats;
+  a.out_plus = c.ret_plus;
   if (centre) {
     a.pairs = 1;
   } else {
-    a.table = table; a.table16 = table16; a.order = order; a.pairs = pairs; a.sigma = sigma; a.out_minus = returns_minus;
+    a.table = c.table; a.table16 = c.table16; a.order = c.order; a.pairs = c.pairs; a.sigma = c.sigma;
+    a.out_minus = c.ret_minus;
   }
   switch (nb) {
     case 1: return launch_act<1>(ctx, a, stream);

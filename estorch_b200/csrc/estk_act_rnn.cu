@@ -273,30 +273,24 @@ int launch_bc(estk_ctx* ctx, RnnParams& p, int code, cudaStream_t stream, const 
 
 }  // namespace
 
-int eval_rnn_actions(estk_ctx* ctx, const estk_mlp_desc& d, const float* theta, const float* table,
-                     const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                     const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs, int bc_dim,
-                     cudaStream_t stream) {
+int eval_rnn_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   const char* who = "estk_eval_mlp[recurrent cell, ESTK_ACTIONS]";
-  const bool centre = offsets == nullptr;
+  if (const int rc = eval_actions_check(ctx, c)) return rc;
+  const estk_mlp_desc& d = c.desc;
   ESTK_CHECK_ARG(d.n_layers == 2, "%s: a recurrent cell is n_layers = 2, dims = (in, H, out) (n_layers=%d)", who,
                  d.n_layers);
   for (int l = 0; l <= 2; ++l) ESTK_CHECK_ARG(d.dims[l] >= 1, "%s: dims[%d]=%d", who, l, d.dims[l]);
   // the parameter count and every row width fit comfortably in 32 bits for the widths accepted here
   ESTK_CHECK_ARG(d.dims[0] <= (1 << 16) && d.dims[1] <= (1 << 13) && d.dims[2] <= (1 << 16),
                  "%s: dims (%d, %d, %d) exceed (65536, 8192, 65536)", who, d.dims[0], d.dims[1], d.dims[2]);
-  ESTK_CHECK_ARG(B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, pairs);
+  ESTK_CHECK_ARG(c.B >= 1, "%s: B must be positive", who);
+  ESTK_CHECK_ARG(c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, c.pairs);
   RnnParams p = {};
   p.in = d.dims[0]; p.H = d.dims[1]; p.out = d.dims[2];
-  p.theta = theta; p.offsets = offsets; p.obs = obs; p.B = B;
-  p.bc_plus = bc_plus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  if (centre) {
-    p.pairs = 1;
-  } else {
-    p.table = table; p.table16 = table16; p.order = order; p.pairs = pairs; p.sigma = sigma; p.bc_minus = bc_minus;
-  }
-  const int bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
+  p.theta = c.theta; p.table = c.table; p.table16 = c.table16; p.offsets = c.offsets; p.order = c.order;
+  p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.B = c.B;
+  p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
+  const int B = c.B, bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
   p.chunks = (B + bc - 1) / bc;
   switch (bc) {
     case 1: return launch_bc<1>(ctx, p, d.activation, stream, who);

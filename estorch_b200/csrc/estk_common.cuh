@@ -43,11 +43,17 @@ static inline bool estk_act_valid(int a) {
                      h == ESTK_ACT_LEAKY_RELU || h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM;
   return known && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions);
 }
-// a defined code whose loss field is ESTK_ACTIONS: no return, the outputs themselves (fp32 only)
-static inline bool estk_act_actions(int a) { return estk_act_valid(a) && (a & 0xff0000) == ESTK_ACTIONS; }
-// a defined code with a recurrent cell in bits 0-7 (ESTK_ACTIONS: one step; else the sequence evaluate)
-static inline bool estk_act_cell(int a) {
-  return estk_act_valid(a) && ((a & 0xff) == ESTK_CELL_GRU || (a & 0xff) == ESTK_CELL_LSTM);
+// The estk_eval_mlp back end of an activation code: n_conv != 0 in bits 24-31 the convolutional evaluate;
+// a defined code whose loss field is ESTK_ACTIONS (no return, the outputs themselves) one step of the MLP or
+// of the recurrent cell in bits 0-7; a defined recurrent cell code with a return the sequence evaluate;
+// anything else the dense MLP evaluate, which refuses an undefined code.
+enum EvalRoute { kRouteDense, kRouteCnn, kRouteActions, kRouteActionsCell, kRouteSequence };
+static inline EvalRoute estk_eval_route(int a) {
+  if ((a >> 24) & 0xff) return kRouteCnn;
+  if (!estk_act_valid(a)) return kRouteDense;
+  const bool cell = (a & 0xff) == ESTK_CELL_GRU || (a & 0xff) == ESTK_CELL_LSTM;
+  if ((a & 0xff0000) == ESTK_ACTIONS) return cell ? kRouteActionsCell : kRouteActions;
+  return cell ? kRouteSequence : kRouteDense;
 }
 
 #ifdef __CUDACC__
@@ -129,9 +135,11 @@ int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStre
                      int64_t slab_floats = 0);
 
 // ---------------------------------------------------------------- evaluate back ends
-// estk_eval_mlp and estk_eval_conv_vbn check their arguments once, then hand the call to the
-// kernel file of the requested precision.  A centre call (offsets == NULL) arrives with table =
-// theta, pairs = 1, sigma = 0 and no minus outputs; buffers the precision does not read are null.
+// estk_eval_mlp checks the precision code, builds this record once and hands it to the back end of the
+// activation code (estk_eval_route), which makes its own argument checks.  A centre call (offsets == NULL)
+// carries pairs = 1, sigma = 0 and null table, table16, order and minus outputs; centre_out is carried as
+// passed, so that every back end can refuse it on a centre call.  The dense MLP evaluate then puts theta
+// (and theta16) in place of the table and nulls the 16-bit buffers its precision does not read.
 struct EvalMlpCall {
   estk_mlp_desc desc;
   int precision;  // ESTK_PREC_*
@@ -154,38 +162,26 @@ struct EvalMlpCall {
   float* centre_out;
 };
 int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);     // estk_eval_mlp_tc.cu
-// estk_eval_mlp with an ESTK_ACTIONS code: its own argument checks, then the act-mode kernel
-// (estk_eval_mlp_act.cu); target and the returns are not part of the call
-int eval_mlp_actions(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta,
-                     const float* table, const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                     int pairs, float sigma, const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs,
-                     int bc_dim, const float* centre_return_out, cudaStream_t stream);
-// the same with a recurrent cell code (ESTK_CELL_GRU / ESTK_CELL_LSTM), after eval_mlp_actions' checks of
-// the precision and the pointers: one step of the cell + head kernel (estk_act_rnn.cu)
-int eval_rnn_actions(estk_ctx* ctx, const estk_mlp_desc& d, const float* theta, const float* table,
-                     const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                     const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs, int bc_dim,
-                     cudaStream_t stream);
-// estk_eval_mlp with a recurrent cell code and a return (squared error or ESTK_LOSS_XENT): its own argument
-// checks, then the sequence evaluate over obs [B][T][in] (estk_eval_rnn_seq.cu)
-int eval_rnn_sequence(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta,
-                      const float* table, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                      const float* obs, const float* target, int B, float* returns_plus, float* returns_minus,
-                      float* bc_plus, float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out,
-                      cudaStream_t stream);
-// estk_eval_mlp with n_conv != 0 in bits 24-31 of the activation code: its own argument checks, then the
-// convolutional evaluate over obs [B][c][h][w] (estk_eval_cnn.cu)
-int eval_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta, const float* table,
-             const int64_t* offsets, const int32_t* order, int pairs, float sigma, const float* obs,
-             const float* target, int B, float* returns_plus, float* returns_minus, float* bc_plus,
-             float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out, cudaStream_t stream);
+// the first checks of both ESTK_ACTIONS back ends: fp32 only, the pointers, the bc layout, no
+// centre_return_out (target and the returns are not part of the call; estk_eval_mlp_act.cu)
+int eval_actions_check(estk_ctx* ctx, const EvalMlpCall& c);
+// kRouteActions: eval_actions_check, its own checks, then the act-mode kernel (estk_eval_mlp_act.cu)
+int eval_mlp_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
+// kRouteActionsCell: eval_actions_check, then one step of the cell + head kernel (estk_act_rnn.cu)
+int eval_rnn_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
+// kRouteSequence: its own argument checks, then the sequence evaluate over obs [B][T][in] (estk_eval_rnn_seq.cu)
+int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
+// kRouteCnn: its own argument checks, then the convolutional evaluate over obs [B][c][h][w] (estk_eval_cnn.cu)
+int eval_cnn(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
 // ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
 // shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
 int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
 int eval_mlp_tc_stream_supported(const estk_mlp_desc& d, int B, const char** why);
 
+// estk_eval_conv_vbn's arguments as passed (a centre call included), for both of its paths
 struct EvalConvCall {
-  int A, R, B;  // n_actions, ref_batch, batch
+  int precision;  // ESTK_PREC_*
+  int A, R, B;    // n_actions (with ESTK_ACTIONS: the whole n_actions | ESTK_ACTIONS code), ref_batch, batch
   const float* theta;
   const float* table;
   const uint16_t* table16;
@@ -199,15 +195,13 @@ struct EvalConvCall {
   float* ret_plus;
   float* ret_minus;
   void* scratch;
+  int64_t scratch_bytes;
 };
 int64_t eval_conv_tc_scratch_per_cta(int R, int B);                              // estk_eval_conv_tc.cu
 int eval_conv_tc(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream);
 // estk_eval_conv_vbn with n_actions | ESTK_ACTIONS: its own argument checks, then the stats and / or act
 // kernels (estk_act_conv.cu); target is not part of the call, scratch holds the per-member VBN stats
-int eval_conv_actions(estk_ctx* ctx, int precision, int32_t code, const float* theta, const float* table,
-                      const uint16_t* table16, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                      const float* xref, int ref_batch, const float* obs, int B, float* returns_plus,
-                      float* returns_minus, void* scratch, int64_t scratch_bytes, cudaStream_t stream);
+int eval_conv_actions(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream);
 
 // ---------------------------------------------------------------- hashing
 // splitmix64 finaliser; must stay in lock-step with oracle/es_oracle.py:mix64

@@ -271,29 +271,23 @@ int launch_hid(estk_ctx* ctx, CnnParams& p, int head, cudaStream_t stream, const
 
 }  // namespace
 
-int eval_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta, const float* table,
-             const int64_t* offsets, const int32_t* order, int pairs, float sigma, const float* obs,
-             const float* target, int B, float* returns_plus, float* returns_minus, float* bc_plus,
-             float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out, cudaStream_t stream) {
+int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   const char* who = "estk_eval_mlp[convolutional]";
-  const bool centre = offsets == nullptr;
-  ESTK_CHECK_ARG(precision == ESTK_PREC_FP32 || precision == ESTK_PREC_F16 || precision == ESTK_PREC_BF16 ||
-                 precision == ESTK_PREC_BF16S || precision == ESTK_PREC_F16_ANY, "%s: unknown precision %d", who,
-                 precision);
-  if (precision != ESTK_PREC_FP32) {
+  const bool centre = call.offsets == nullptr;
+  if (call.precision != ESTK_PREC_FP32) {
     estk_set_error("%s: precision %d is not supported: a convolutional policy is computed with ESTK_PREC_FP32 "
-                   "only", who, precision);
+                   "only", who, call.precision);
     return ESTK_ERR_UNSUPPORTED;
   }
-  if (centre_return_out) {
+  if (call.centre_out) {
     estk_set_error("%s: centre_return_out (folded centre rollout) needs a tensor-core precision", who);
     return ESTK_ERR_UNSUPPORTED;
   }
-  const estk_mlp_desc& d = *desc;
+  const estk_mlp_desc& d = call.desc;
   const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
   ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
                  n_conv, code);
-  if (estk_act_actions(low) || estk_act_cell(low)) {
+  if (estk_eval_route(low) != kRouteDense) {
     estk_set_error("%s: ESTK_ACTIONS and the recurrent cells are not supported with a conv stack (code 0x%x)", who,
                    code);
     return ESTK_ERR_UNSUPPORTED;
@@ -303,14 +297,16 @@ int eval_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const floa
   ESTK_CHECK_ARG(d.n_layers > n_conv && d.n_layers <= ESTK_MAX_LAYERS,
                  "%s: n_layers=%d must exceed n_conv=%d (at least one Linear) and be at most %d", who, d.n_layers,
                  n_conv, ESTK_MAX_LAYERS);
-  ESTK_CHECK_ARG(ctx && theta && obs && target && returns_plus && (centre || (table && returns_minus)),
+  ESTK_CHECK_ARG(ctx && call.theta && call.obs && call.target && call.ret_plus &&
+                 (centre || (call.table && call.ret_minus)),
                  "%s: null argument (theta, obs, target, returns_plus, and for a population table and "
                  "returns_minus)", who);
-  ESTK_CHECK_ARG(centre || (bc_plus == nullptr) == (bc_minus == nullptr),
+  ESTK_CHECK_ARG(centre || (call.bc_plus == nullptr) == (call.bc_minus == nullptr),
                  "%s: bc_plus/bc_minus must both be set or both null", who);
-  ESTK_CHECK_ARG(!bc_plus || (bc_obs > 0 && bc_dim > 0), "%s: bc_obs/bc_dim must be positive with bc outputs", who);
-  ESTK_CHECK_ARG(B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, pairs);
+  ESTK_CHECK_ARG(!call.bc_plus || (call.bc_obs > 0 && call.bc_dim > 0),
+                 "%s: bc_obs/bc_dim must be positive with bc outputs", who);
+  ESTK_CHECK_ARG(call.B >= 1, "%s: B must be positive", who);
+  ESTK_CHECK_ARG(call.pairs >= 1 && call.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, call.pairs);
 
   CnnParams p = {};
   const uint32_t in = (uint32_t)d.dims[0];
@@ -350,14 +346,10 @@ int eval_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const floa
   p.n_layers = d.n_layers;
   p.out = c;
   p.maxact = (int)maxact;
-  p.theta = theta; p.offsets = offsets; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.bc_plus = bc_plus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  if (centre) {
-    p.pairs = 1;
-  } else {
-    p.table = table; p.order = order; p.pairs = pairs; p.sigma = sigma;
-    p.ret_minus = returns_minus; p.bc_minus = bc_minus;
-  }
+  p.theta = call.theta; p.table = call.table; p.offsets = call.offsets; p.order = call.order;
+  p.pairs = call.pairs; p.sigma = call.sigma; p.obs = call.obs; p.target = call.target; p.B = call.B;
+  p.ret_plus = call.ret_plus; p.ret_minus = call.ret_minus;
+  p.bc_plus = call.bc_plus; p.bc_minus = call.bc_minus; p.bc_obs = call.bc_obs; p.bc_dim = call.bc_dim;
   const int head = (low & ESTK_LOSS_XENT) ? kHeadXent : (low & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
   switch (low & 0xff) {
     case ESTK_ACT_TANH: return launch_hid<ESTK_ACT_TANH>(ctx, p, head, stream, who);

@@ -319,10 +319,9 @@ extern "C" int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_ac
                                   int32_t B, float* returns_plus, float* returns_minus, void* scratch,
                                   int64_t scratch_bytes, void* stream) {
   const bool f16 = precision == ESTK_PREC_F16;
-  if (((n_actions >> 16) & 0xff) == (ESTK_ACTIONS >> 16))
-    return eval_conv_actions(ctx, precision, n_actions, theta, table, table16, offsets, order, pairs, sigma, xref,
-                             ref_batch, obs, B, returns_plus, returns_minus, scratch, scratch_bytes,
-                             (cudaStream_t)stream);
+  const EvalConvCall c = {precision, n_actions, ref_batch, B, theta, table, table16, offsets, order, pairs, sigma,
+                          xref, obs, target, returns_plus, returns_minus, scratch, scratch_bytes};
+  if (((n_actions >> 16) & 0xff) == (ESTK_ACTIONS >> 16)) return eval_conv_actions(ctx, c, (cudaStream_t)stream);
   ESTK_CHECK_ARG(ctx && theta && xref && obs && target && returns_plus && scratch, "estk_eval_conv_vbn: null argument");
   ESTK_CHECK_ARG(offsets == nullptr || (table && (table16 || !f16) && returns_minus),
                  "estk_eval_conv_vbn: table%s/returns_minus required with offsets", f16 ? "/table16" : "");
@@ -338,11 +337,7 @@ extern "C" int estk_eval_conv_vbn(estk_ctx* ctx, int32_t precision, int32_t n_ac
   }
   const int64_t need = estk_eval_conv_vbn_scratch_bytes(ctx, precision, ref_batch, B);
   ESTK_CHECK_ARG(scratch_bytes >= need, "estk_eval_conv_vbn: scratch %lld < %lld bytes", (long long)scratch_bytes, (long long)need);
-  if (f16) {
-    const EvalConvCall c = {n_actions, ref_batch, B, theta, table, table16, offsets, order, pairs, sigma,
-                            xref, obs, target, returns_plus, returns_minus, scratch};
-    return eval_conv_tc(ctx, c, (cudaStream_t)stream);
-  }
+  if (f16) return eval_conv_tc(ctx, c, (cudaStream_t)stream);
   ConvParams p = {};
   p.theta = theta; p.table = table; p.offsets = offsets; p.order = order; p.pairs = pairs; p.sigma = sigma;
   p.A = n_actions; p.R = ref_batch; p.B = B; p.xref = xref; p.obs = obs; p.target = target;

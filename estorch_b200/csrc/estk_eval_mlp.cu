@@ -590,8 +590,9 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
 
 }  // namespace
 
-// The one MLP evaluate entry point of every precision: the argument checks of all of them, then
-// run_eval (fp32, here) or eval_mlp_tc (estk_eval_mlp_tc.cu).
+// The one evaluate entry point of every policy kind and precision: the precision check, the call record, then
+// the back end of the activation code.  The dense MLP evaluate is this function's own: its argument checks,
+// then run_eval (fp32, here) or eval_mlp_tc (estk_eval_mlp_tc.cu).
 extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t precision, const float* theta,
                              const uint16_t* theta16, const float* table, const uint16_t* table16,
                              const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
@@ -603,17 +604,26 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
   const bool shadows = precision == ESTK_PREC_BF16S;                 // reads theta16, and table16 as a bf16 shadow
   const bool t16 = shadows || f16;                                   // a population reads table16
   const bool centre = offsets == nullptr;
-  if (desc && ((desc->activation >> 24) & 0xff) != 0)
-    return eval_cnn(ctx, desc, precision, theta, table, offsets, order, pairs, sigma, obs, target, B, returns_plus,
-                    returns_minus, bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, (cudaStream_t)stream);
-  if (desc && estk_act_actions(desc->activation))
-    return eval_mlp_actions(ctx, desc, precision, theta, table, table16, offsets, order, pairs, sigma, obs, B,
-                            bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out, (cudaStream_t)stream);
-  if (desc && estk_act_cell(desc->activation))
-    return eval_rnn_sequence(ctx, desc, precision, theta, table, offsets, order, pairs, sigma, obs, target, B,
-                             returns_plus, returns_minus, bc_plus, bc_minus, bc_obs, bc_dim, centre_return_out,
-                             (cudaStream_t)stream);
   ESTK_CHECK_ARG(tc || precision == ESTK_PREC_FP32, "estk_eval_mlp: unknown precision %d", precision);
+  EvalMlpCall c = {};
+  if (desc) c.desc = *desc;
+  c.precision = precision; c.theta = theta; c.theta16 = theta16; c.obs = obs; c.target = target; c.B = B;
+  c.ret_plus = returns_plus; c.bc_plus = bc_plus; c.bc_obs = bc_obs; c.bc_dim = bc_dim;
+  c.centre_out = centre_return_out;
+  if (centre) {
+    c.pairs = 1;
+  } else {
+    c.table = table; c.table16 = table16; c.offsets = offsets; c.order = order; c.pairs = pairs; c.sigma = sigma;
+    c.ret_minus = returns_minus; c.bc_minus = bc_minus;
+  }
+  const cudaStream_t s = (cudaStream_t)stream;
+  switch (desc ? estk_eval_route(desc->activation) : kRouteDense) {
+    case kRouteCnn: return eval_cnn(ctx, c, s);
+    case kRouteActions: return eval_mlp_actions(ctx, c, s);
+    case kRouteActionsCell: return eval_rnn_actions(ctx, c, s);
+    case kRouteSequence: return eval_rnn_sequence(ctx, c, s);
+    case kRouteDense: break;
+  }
   ESTK_CHECK_ARG(ctx && desc && theta && obs && target && returns_plus && (theta16 || !shadows) &&
                  (centre || (table && (table16 || !t16) && returns_minus)), "estk_eval_mlp: null argument");
   ESTK_CHECK_ARG(centre || (bc_plus == nullptr) == (bc_minus == nullptr),
@@ -628,22 +638,17 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
     estk_set_error("estk_eval_mlp: centre_return_out (folded centre rollout) needs a tensor-core precision");
     return ESTK_ERR_UNSUPPORTED;
   }
-  EvalMlpCall c = {};
-  c.desc = *desc; c.precision = precision; c.theta = theta; c.obs = obs; c.target = target; c.B = B;
-  c.ret_plus = returns_plus; c.bc_plus = bc_plus; c.bc_obs = bc_obs; c.bc_dim = bc_dim;
   c.theta16 = shadows ? theta16 : nullptr;
   if (centre) {
-    c.table = theta; c.table16 = c.theta16; c.pairs = 1; c.sigma = 0.f;
-  } else {
-    c.table = table; c.table16 = t16 ? table16 : nullptr; c.offsets = offsets; c.order = order;
-    c.pairs = pairs; c.sigma = sigma; c.ret_minus = returns_minus; c.bc_minus = bc_minus;
-    c.centre_out = centre_return_out;
+    c.table = theta; c.table16 = c.theta16;
+  } else if (!t16) {
+    c.table16 = nullptr;
   }
-  if (tc) return eval_mlp_tc(ctx, c, (cudaStream_t)stream);
+  if (tc) return eval_mlp_tc(ctx, c, s);
   EvalParams p = {};
   p.desc = c.desc; p.theta = c.theta; p.table = c.table; p.offsets = c.offsets; p.order = c.order;
   p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.target = c.target; p.B = c.B;
   p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
-  return run_eval(ctx, p, (cudaStream_t)stream, "estk_eval_mlp");
+  return run_eval(ctx, p, s, "estk_eval_mlp");
 }

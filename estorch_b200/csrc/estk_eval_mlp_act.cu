@@ -223,45 +223,36 @@ int launch_bc(estk_ctx* ctx, ActParams& p, cudaStream_t stream, const char* who)
 
 }  // namespace
 
-int eval_mlp_actions(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta,
-                     const float* table, const uint16_t* table16, const int64_t* offsets, const int32_t* order,
-                     int pairs, float sigma, const float* obs, int B, float* bc_plus, float* bc_minus, int bc_obs,
-                     int bc_dim, const float* centre_return_out, cudaStream_t stream) {
+int eval_actions_check(estk_ctx* ctx, const EvalMlpCall& c) {
   const char* who = "estk_eval_mlp[ESTK_ACTIONS]";
-  const bool centre = offsets == nullptr;
-  ESTK_CHECK_ARG(precision == ESTK_PREC_FP32 || precision == ESTK_PREC_F16 || precision == ESTK_PREC_BF16 ||
-                 precision == ESTK_PREC_BF16S || precision == ESTK_PREC_F16_ANY, "%s: unknown precision %d", who,
-                 precision);
-  if (precision != ESTK_PREC_FP32) {
-    estk_set_error("%s: actions are computed with ESTK_PREC_FP32 only (precision %d)", who, precision);
+  if (c.precision != ESTK_PREC_FP32) {
+    estk_set_error("%s: actions are computed with ESTK_PREC_FP32 only (precision %d)", who, c.precision);
     return ESTK_ERR_UNSUPPORTED;
   }
-  ESTK_CHECK_ARG(ctx && theta && obs && bc_plus && (centre || ((table || table16) && bc_minus)),
+  ESTK_CHECK_ARG(ctx && c.theta && c.obs && c.bc_plus && (!c.offsets || ((c.table || c.table16) && c.bc_minus)),
                  "%s: null argument (theta, obs, bc_plus, and for a population table or table16 and bc_minus)", who);
-  ESTK_CHECK_ARG(bc_obs > 0 && bc_dim > 0, "%s: bc_obs/bc_dim must be positive", who);
-  ESTK_CHECK_ARG(!centre_return_out, "%s: centre_return_out is not an ESTK_ACTIONS output", who);
-  const estk_mlp_desc& d = *desc;
-  const int cell = d.activation & 0xff;
-  if (cell == ESTK_CELL_GRU || cell == ESTK_CELL_LSTM)
-    return eval_rnn_actions(ctx, d, theta, table, table16, offsets, order, pairs, sigma, obs, B, bc_plus, bc_minus,
-                            bc_obs, bc_dim, stream);
+  ESTK_CHECK_ARG(c.bc_obs > 0 && c.bc_dim > 0, "%s: bc_obs/bc_dim must be positive", who);
+  ESTK_CHECK_ARG(!c.centre_out, "%s: centre_return_out is not an ESTK_ACTIONS output", who);
+  return ESTK_OK;
+}
+
+int eval_mlp_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
+  const char* who = "estk_eval_mlp[ESTK_ACTIONS]";
+  if (const int rc = eval_actions_check(ctx, c)) return rc;
+  const estk_mlp_desc& d = c.desc;
   ESTK_CHECK_ARG(d.n_layers >= 1 && d.n_layers <= ESTK_MAX_LAYERS, "%s: n_layers=%d", who, d.n_layers);
   int maxw = 0;
   for (int l = 0; l <= d.n_layers; ++l) {
     ESTK_CHECK_ARG(d.dims[l] >= 1, "%s: dims[%d]=%d", who, l, d.dims[l]);
     maxw = std::max(maxw, d.dims[l]);
   }
-  ESTK_CHECK_ARG(B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, pairs);
+  ESTK_CHECK_ARG(c.B >= 1, "%s: B must be positive", who);
+  ESTK_CHECK_ARG(c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, c.pairs);
   ActParams p = {};
-  p.desc = d; p.theta = theta; p.offsets = offsets; p.obs = obs; p.B = B; p.maxw = maxw;
-  p.bc_plus = bc_plus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  if (centre) {
-    p.pairs = 1;
-  } else {
-    p.table = table; p.table16 = table16; p.order = order; p.pairs = pairs; p.sigma = sigma; p.bc_minus = bc_minus;
-  }
-  const int bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
+  p.desc = d; p.theta = c.theta; p.table = c.table; p.table16 = c.table16; p.offsets = c.offsets; p.order = c.order;
+  p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.B = c.B; p.maxw = maxw;
+  p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
+  const int B = c.B, bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
   p.chunks = (B + bc - 1) / bc;
   switch (bc) {
     case 1: return launch_bc<1>(ctx, p, stream, who);

@@ -826,8 +826,7 @@ extern "C" ESTK_API int estk_tc_profile(void* buf, int32_t* warps, int32_t* cons
 
 extern "C" int estk_eval_mlp_supported(const estk_mlp_desc* desc, int32_t precision, int32_t B) {
   const char* why = "";
-  if (desc && estk_act_actions(desc->activation)) return 0;     // act mode is fp32 only
-  if (desc && estk_act_cell(desc->activation)) return 0;        // so are the recurrent sequence evaluates
+  if (desc && estk_eval_route(desc->activation) != kRouteDense) return 0;   // every other back end is fp32 only
   if (desc && precision == ESTK_PREC_F16_ANY) return eval_mlp_tc_stream_supported(*desc, B, &why);
   const int mode = mode_of(precision);
   return desc && mode >= 0 ? tc_supported(*desc, B, &why, mode) : 0;

@@ -324,31 +324,26 @@ int launch_bc(estk_ctx* ctx, SeqParams& p, int code, cudaStream_t stream, const 
 
 }  // namespace
 
-int eval_rnn_sequence(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, const float* theta,
-                      const float* table, const int64_t* offsets, const int32_t* order, int pairs, float sigma,
-                      const float* obs, const float* target, int B, float* returns_plus, float* returns_minus,
-                      float* bc_plus, float* bc_minus, int bc_obs, int bc_dim, const float* centre_return_out,
-                      cudaStream_t stream) {
+int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   const char* who = "estk_eval_mlp[recurrent cell, sequence]";
-  const bool centre = offsets == nullptr;
-  ESTK_CHECK_ARG(precision == ESTK_PREC_FP32 || precision == ESTK_PREC_F16 || precision == ESTK_PREC_BF16 ||
-                 precision == ESTK_PREC_BF16S || precision == ESTK_PREC_F16_ANY, "%s: unknown precision %d", who,
-                 precision);
-  if (precision != ESTK_PREC_FP32) {
-    estk_set_error("%s: the sequence evaluate is computed with ESTK_PREC_FP32 only (precision %d)", who, precision);
+  const bool centre = c.offsets == nullptr;
+  if (c.precision != ESTK_PREC_FP32) {
+    estk_set_error("%s: the sequence evaluate is computed with ESTK_PREC_FP32 only (precision %d)", who,
+                   c.precision);
     return ESTK_ERR_UNSUPPORTED;
   }
-  if (centre_return_out) {
+  if (c.centre_out) {
     estk_set_error("%s: centre_return_out (folded centre rollout) needs a tensor-core precision", who);
     return ESTK_ERR_UNSUPPORTED;
   }
-  ESTK_CHECK_ARG(ctx && theta && obs && target && returns_plus && (centre || (table && returns_minus)),
+  ESTK_CHECK_ARG(ctx && c.theta && c.obs && c.target && c.ret_plus && (centre || (c.table && c.ret_minus)),
                  "%s: null argument (theta, obs, target, returns_plus, and for a population table and "
                  "returns_minus)", who);
-  ESTK_CHECK_ARG(centre || (bc_plus == nullptr) == (bc_minus == nullptr),
+  ESTK_CHECK_ARG(centre || (c.bc_plus == nullptr) == (c.bc_minus == nullptr),
                  "%s: bc_plus/bc_minus must both be set or both null", who);
-  ESTK_CHECK_ARG(!bc_plus || (bc_obs > 0 && bc_dim > 0), "%s: bc_obs/bc_dim must be positive with bc outputs", who);
-  const estk_mlp_desc& d = *desc;
+  ESTK_CHECK_ARG(!c.bc_plus || (c.bc_obs > 0 && c.bc_dim > 0), "%s: bc_obs/bc_dim must be positive with bc outputs",
+                 who);
+  const estk_mlp_desc& d = c.desc;
   ESTK_CHECK_ARG(d.n_layers == 2, "%s: a recurrent cell is n_layers = 2, dims = (in, H, out, T) (n_layers=%d)", who,
                  d.n_layers);
   for (int l = 0; l <= 2; ++l) ESTK_CHECK_ARG(d.dims[l] >= 1, "%s: dims[%d]=%d", who, l, d.dims[l]);
@@ -356,20 +351,16 @@ int eval_rnn_sequence(estk_ctx* ctx, const estk_mlp_desc* desc, int precision, c
   // the parameter count and every row width fit comfortably in 32 bits for the widths accepted here
   ESTK_CHECK_ARG(d.dims[0] <= (1 << 16) && d.dims[1] <= (1 << 13) && d.dims[2] <= (1 << 16),
                  "%s: dims (%d, %d, %d) exceed (65536, 8192, 65536)", who, d.dims[0], d.dims[1], d.dims[2]);
-  ESTK_CHECK_ARG(B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d", who, pairs);
+  ESTK_CHECK_ARG(c.B >= 1, "%s: B must be positive", who);
+  ESTK_CHECK_ARG(c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, c.pairs);
   SeqParams p = {};
   p.in = d.dims[0]; p.H = d.dims[1]; p.out = d.dims[2]; p.T = d.dims[3];
-  p.theta = theta; p.offsets = offsets; p.obs = obs; p.target = target; p.B = B;
-  p.ret_plus = returns_plus; p.bc_plus = bc_plus; p.bc_obs = bc_obs; p.bc_dim = bc_dim;
-  if (centre) {
-    p.pairs = 1;
-  } else {
-    p.table = table; p.order = order; p.pairs = pairs; p.sigma = sigma;
-    p.ret_minus = returns_minus; p.bc_minus = bc_minus;
-  }
+  p.theta = c.theta; p.table = c.table; p.offsets = c.offsets; p.order = c.order; p.pairs = c.pairs;
+  p.sigma = c.sigma; p.obs = c.obs; p.target = c.target; p.B = c.B;
+  p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
+  p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
   // chunk of sequences per work item: the bits do not depend on it (the returns are summed per sequence)
-  if (B == 1) return launch_bc<1>(ctx, p, d.activation, stream, who);
-  if (B <= 4) return launch_bc<4>(ctx, p, d.activation, stream, who);
+  if (c.B == 1) return launch_bc<1>(ctx, p, d.activation, stream, who);
+  if (c.B <= 4) return launch_bc<4>(ctx, p, d.activation, stream, who);
   return launch_bc<16>(ctx, p, d.activation, stream, who);
 }
