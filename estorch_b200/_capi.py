@@ -1,4 +1,4 @@
-"""ctypes binding of libestk.so (the C ABI declared in include/estk.h).
+"""ctypes binding of libestk.so (the C ABI declared in include/estk.h and include/estk_batch.h).
 
 The library is built in-tree by ``estorch_b200/csrc/build.sh`` (or
 ``__graft_entry__.build()``).  There is NO fallback: if the shared object is
@@ -109,6 +109,11 @@ SIGNATURES = {
     "estk_knn_novelty": [_P, _P, _I32, _P, _I32, _I32, _I32, _P, _P],
 }
 
+# include/estk_batch.h: the minibatch sampler, declared beside the core of estk.h
+BATCH_SIGNATURES = {
+    "estk_sample_batch": [_P, _U64, _P, _I64, _I64, _I32, _P, _I64, _P, _P, _I64, _P, _P, _P],
+}
+
 _lib = None
 
 
@@ -123,7 +128,7 @@ def load():
             "`bash estorch_b200/csrc/build.sh` (or `python -c 'import __graft_entry__ as g; "
             "g.build()'`). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in SIGNATURES.items():
+    for name, argtypes in {**SIGNATURES, **BATCH_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = (C.c_char_p if name == "estk_last_error" else

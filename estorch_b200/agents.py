@@ -15,6 +15,9 @@ reference protocol (``rollout``) with plain torch, so the very same object
 runs under the CPU reference -- that is how the goldens and the CPU baseline
 are produced.
 
+``DeviceAgent(..., batch_size=B)`` holds a whole dataset and evaluates each generation on a fresh minibatch of
+B rows of it, drawn on the device (``batches.batch_indices`` states which rows).
+
 Any other agent (a gym loop, ...) is a *host agent*: the engine materialises
 each member's parameter row on the device and calls ``rollout`` on the host,
 exactly like estorch.py:195-202.
@@ -23,7 +26,10 @@ from __future__ import annotations
 
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
+
+from .batches import batch_indices
 
 
 LOSSES = ("mse", "cross_entropy")
@@ -35,14 +41,30 @@ class DeviceAgent:
     ``loss="mse"`` (default): the return is minus the mean squared error against ``target``.
     ``loss="cross_entropy"``: ``target`` is ``[B, C]`` class weights per observation (one-hot or
     soft labels, finite and >= 0) and the return is minus the mean over the batch of the
-    cross-entropy between those weights and the softmax of the policy's output."""
+    cross-entropy between those weights and the softmax of the policy's output.
+
+    ``batch_size=B``: ``obs`` / ``target`` are a whole dataset of N rows (``dataset_obs`` / ``dataset_target``)
+    and every generation is scored on a minibatch of B of them, the same minibatch for every member.
+    Minibatch g takes positions g*B .. g*B + B - 1 of a stream of per-epoch permutations of the rows keyed by
+    ``batch_seed`` (``batch_indices``), so each epoch visits every row once.  ``obs`` / ``target`` hold the
+    current minibatch: batch 0 after construction, batch g after ``set_generation(g)``.  In fused mode ``ES``
+    gathers each generation's minibatch on the device (the host copy is not updated); in hooks mode it calls
+    ``set_generation`` before every generation.  ``rollout`` scores the current minibatch, and under the
+    unmodified reference nothing advances it.  A behaviour characteristic needs fixed inputs, so
+    ``batch_size`` with ``bc_obs`` / ``bc_dim`` is refused."""
+
+    batch_size = None
+    batch_seed = 0
+    dataset_obs = dataset_target = None
 
     def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0, *,
-                 loss: str = "mse"):
+                 loss: str = "mse", batch_size: Optional[int] = None, batch_seed: int = 0):
         if obs.dim() < 2 or target.dim() != 2 or obs.shape[0] != target.shape[0]:
             raise ValueError("obs must be [B, in] (or [B, C, H, W] for conv policies) and target [B, out]")
         if loss not in LOSSES:
             raise ValueError(f"loss must be one of {LOSSES}, got {loss!r}")
+        if batch_size is not None:      # before the dataset is copied
+            _check_batches(obs.shape[0], batch_size, bc_obs, bc_dim)
         self.obs = obs.detach().to(torch.float32).contiguous()
         self.target = target.detach().to(torch.float32).contiguous()
         if loss == "cross_entropy" and not (target.is_floating_point() and bool(torch.isfinite(self.target).all())
@@ -53,6 +75,22 @@ class DeviceAgent:
         self.bc_dim = int(bc_dim)
         if bool(self.bc_obs) != bool(self.bc_dim):
             raise ValueError("bc_obs and bc_dim must both be zero or both be positive")
+        if batch_size is not None:
+            self._init_batches(batch_size, batch_seed)
+
+    # -- minibatches of a dataset ---------------------------------------------
+    def _init_batches(self, batch_size, batch_seed):
+        self.batch_size, self.batch_seed = int(batch_size), int(batch_seed)
+        self.dataset_obs, self.dataset_target = self.obs, self.target
+        self.set_generation(0)
+
+    def set_generation(self, generation: int):
+        """Make ``obs`` / ``target`` minibatch ``generation`` of the dataset (``batch_size`` agents only)."""
+        if self.batch_size is None:
+            raise ValueError("set_generation needs an agent constructed with batch_size")
+        idx = torch.from_numpy(batch_indices(self.batch_seed, generation, self.dataset_obs.shape[0],
+                                             self.batch_size))
+        self.obs, self.target = self.dataset_obs[idx], self.dataset_target[idx]
 
     # -- reference protocol (host / torch) ---------------------------------
     def rollout(self, policy):
@@ -77,6 +115,17 @@ class DeviceAgent:
         return None
 
 
+def _check_batches(n, batch_size, bc_obs, bc_dim):
+    """The rules of ``batch_size`` for a dataset of ``n`` rows."""
+    if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or not 1 <= batch_size <= n:
+        raise ValueError(f"batch_size must be an int in [1, {n}] (the dataset's rows), got {batch_size!r}")
+    if n >= 1 << 31:
+        raise ValueError(f"a dataset of {n} rows is too large for minibatches (at most 2^31 - 1 rows)")
+    if bc_obs or bc_dim:
+        raise ValueError("batch_size cannot be combined with bc_obs / bc_dim: a behaviour characteristic needs "
+                         "fixed inputs")
+
+
 class SequenceAgent(DeviceAgent):
     """A fixed batch of sequences for a recurrent policy, evaluated by the fused CUDA kernel.
 
@@ -93,14 +142,18 @@ class SequenceAgent(DeviceAgent):
     overridden hook ``ES`` evaluates every perturbed member over the whole batch in one fused launch."""
 
     def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0, *,
-                 loss: str = "mse"):
+                 loss: str = "mse", batch_size: Optional[int] = None, batch_seed: int = 0):
         if obs.dim() != 3 or target.dim() != 3 or tuple(obs.shape[:2]) != tuple(target.shape[:2]) or \
                 obs.shape[1] < 1:
             raise ValueError("obs must be [B, T, in] and target [B, T, out] with the same B and T >= 1")
+        if batch_size is not None:
+            _check_batches(obs.shape[0], batch_size, bc_obs, bc_dim)
         super().__init__(obs.reshape(obs.shape[0], -1), target.reshape(target.shape[0], -1), bc_obs, bc_dim,
                          loss=loss)
         self.obs = self.obs.reshape(obs.shape)
         self.target = self.target.reshape(target.shape)
+        if batch_size is not None:      # ``obs`` / ``target`` are a dataset of N sequences: minibatches of them
+            self._init_batches(batch_size, batch_seed)
 
     def rollout(self, policy):
         with torch.no_grad():

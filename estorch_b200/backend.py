@@ -179,6 +179,27 @@ class CudaBackend:
             self._stream()), "estk_perturb_rows")
         self.launches += 1
 
+    # ---------------------------------------------------------------- minibatches
+    def sample_batch(self, seed, state, gen_host, obs_src, obs_dst, tgt_src, tgt_dst, index_out=None):
+        """Generation g's minibatch of the dataset ``obs_src`` ``[N, ...]`` / ``tgt_src`` ``[N, ...]`` into
+        ``obs_dst`` ``[B, ...]`` / ``tgt_dst`` ``[B, ...]`` (estk_sample_batch; ``batch_indices`` states the rows);
+        g = ``gen_host`` plus the generation in ``state`` (None: ``gen_host`` alone).  ``index_out`` (int64
+        ``[B]``, optional) receives the row indices."""
+        N, B = int(obs_src.shape[0]), int(obs_dst.shape[0])
+        if obs_src.dim() < 1 or tuple(obs_dst.shape[1:]) != tuple(obs_src.shape[1:]) or \
+                tuple(tgt_src.shape[:1]) != (N,) or tuple(tgt_dst.shape) != (B,) + tuple(tgt_src.shape[1:]):
+            raise ValueError(f"sample_batch: obs {tuple(obs_src.shape)} -> {tuple(obs_dst.shape)}, target "
+                             f"{tuple(tgt_src.shape)} -> {tuple(tgt_dst.shape)} are not [N, ...] -> [B, ...]")
+        if index_out is not None and tuple(index_out.shape) != (B,):
+            raise ValueError(f"sample_batch: index_out {tuple(index_out.shape)}, expected [{B}]")
+        _capi.check(self.lib.estk_sample_batch(
+            self._ctx, int(seed) & (2**64 - 1), self._ptr(state, torch.uint8, "state"), int(gen_host), N, B,
+            self._ptr(obs_src, torch.float32, "obs_src"), obs_src[0].numel() if N else 0,
+            self._ptr(obs_dst, torch.float32, "obs_dst"), self._ptr(tgt_src, torch.float32, "tgt_src"),
+            tgt_src[0].numel() if N else 0, self._ptr(tgt_dst, torch.float32, "tgt_dst"),
+            self._ptr(index_out, torch.int64, "index_out"), self._stream()), "estk_sample_batch")
+        self.launches += 1
+
     # ---------------------------------------------------------------- evaluate
     def _precision(self, precision):
         """ESTK_PREC_* code and the dtype of the 16-bit buffers (theta16 / table16) of an evaluate precision."""

@@ -16,7 +16,7 @@ FLAGS=(-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -I"$ROOT/i
 OBJS=()
 for src in "$HERE"/*.cu; do
   obj="$OBJDIR/$(basename "${src%.cu}").o"
-  if [[ ! -f "$obj" || "$src" -nt "$obj" || "$HERE/estk_common.cuh" -nt "$obj" || "$HERE/estk_tc.cuh" -nt "$obj" || "$HERE/estk_sort.cuh" -nt "$obj" || "$ROOT/include/estk.h" -nt "$obj" ]]; then
+  if [[ ! -f "$obj" || "$src" -nt "$obj" || "$HERE/estk_common.cuh" -nt "$obj" || "$HERE/estk_tc.cuh" -nt "$obj" || "$HERE/estk_sort.cuh" -nt "$obj" || "$ROOT/include/estk.h" -nt "$obj" || "$ROOT/include/estk_batch.h" -nt "$obj" ]]; then
     "$NVCC" "${FLAGS[@]}" ${ESTK_EXTRA_FLAGS:-} ${ESTK_PTXAS_V:+-Xptxas -v} -c "$src" -o "$obj"
   fi
   OBJS+=("$obj")

@@ -301,6 +301,11 @@ class ES:
 
         self.agent = agent(**agent_kwargs)
         self._device_agent = isinstance(self.agent, DeviceAgent)
+        # a device agent with batch_size: every generation evaluates a fresh minibatch of its dataset
+        self._sampling = self._device_agent and self.agent.batch_size is not None
+        if self._sampling and type(self.agent).next_batch is not DeviceAgent.next_batch:
+            raise ValueError("an agent with batch_size draws its minibatches on the device; it cannot also "
+                             "override next_batch (one batch source per agent)")
         self.target = policy(**policy_kwargs).to(self.device)       # estorch.py:142
         parameters = torch.nn.utils.parameters_to_vector(self.target.parameters())
         self.n_parameters = parameters.shape[0]
@@ -385,6 +390,12 @@ class ES:
         if self._device_agent:
             self._obs = self.agent.obs.to(self._dev).contiguous()
             self._tgt = self.agent.target.to(self._dev).contiguous()
+        self._data_obs = self._data_tgt = None
+        if self._fused and self._sampling:
+            # the whole dataset lives on the device; _obs / _tgt are the evaluate's batch buffers, refilled by
+            # estk_sample_batch at the head of every generation
+            self._data_obs = self.agent.dataset_obs.to(self._dev).contiguous()
+            self._data_tgt = self.agent.dataset_target.to(self._dev).contiguous()
 
         self._xref = self._conv_scratch = self._conv_stats = None
         if self._fused and self._is_conv:
@@ -961,10 +972,10 @@ class ES:
     def _defers_centre(self):
         """Whether this generation's post-update rollout (estorch.py:181-185) is deferred and folded into the
         next generation's evaluate launch: it is a single 30 us task, so it waits when nobody can observe it
-        before then (no log() due, not the last generation, the observation batch does not change).  Only
-        the tensor-core MLP evaluate can carry it."""
+        before then (no log() due, not the last generation, the observation batch does not change: never
+        with minibatches, whose next batch is not this one).  Only the tensor-core MLP evaluate can carry it."""
         return (self._precision in ("f16", "bf16", "bf16s") and not self._is_conv and not self._stop
-                and not self._streaming
+                and not self._streaming and not self._sampling
                 and (self.step + 1) % self._log_interval != 0 and self.step + 1 < self.n_steps)
 
     def _fused_generation(self, slot):
@@ -976,6 +987,9 @@ class ES:
         be, pairs, pl, pb, W = self._be, self._pairs, self._pairs_local, self._pair_begin, self.n_workers
         dims = None if self._is_conv else self._spec.dims
         self._upload_batch()
+        if self._sampling:    # this generation's minibatch: the generation index is read from slot.state
+            be.sample_batch(self.agent.batch_seed, slot.state, 0, self._data_obs, self._obs, self._data_tgt,
+                            self._tgt)
         slot.theta_prev.copy_(slot.theta)
         folded = self._pending_centre
         self._draw_offsets(slot.state, 1 if folded else 0)
@@ -1323,6 +1337,8 @@ class ES:
                     self._active = self._select_slot()
                     self._graphed_generation(self._active)
                 else:
+                    if self._sampling:      # host rollouts see the minibatch the fused generation would gather
+                        self.agent.set_generation(self._generation)
                     self._hooks_generation()
                 if (self.step + 1) % self._log_interval == 0:
                     if self.rank == 0:
