@@ -28,9 +28,6 @@
 // at the reference's P = 100, B = 1 that is 50 CTAs on 132 SMs.  The k-split of fc1 across CTAs that
 // would fill the rest needs a combine pass; DESIGN.md section 4.7 has the measured cost of not doing it.
 #include "estk_common.cuh"
-#include <cuda_fp16.h>
-#include <algorithm>
-#include <climits>
 
 namespace {
 
@@ -47,26 +44,6 @@ static_assert(kStats == ESTK_CONV_VBN_STATS_FLOATS, "stats layout: a1, mean1 [64
 // parameter offsets, registration order of examples/atari.py:17-23
 constexpr int64_t oC1W = 0, oC1B = 4096, oG1 = 4112, oB1 = 4128, oC2W = 4144, oC2B = 12336, oG2 = 12368,
                   oB2 = 12400, oF1W = 12432, oF1B = oF1W + (int64_t)FC1 * P2, oF2W = oF1B + FC1;
-
-__device__ __forceinline__ float ld_noise1h(const uint16_t* p) {
-  unsigned short v;
-  asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(v) : "l"(p));
-  return __half2float(__ushort_as_half(v));
-}
-
-// one pair's noise row: fp32 table, its exact fp16 copy, or theta itself for the centre (sigma 0)
-struct NoiseRow {
-  const float* t32;
-  const uint16_t* t16;
-  __device__ __forceinline__ float operator()(int64_t i) const { return t16 ? ld_noise1h(t16 + i) : ld_noise1(t32 + i); }
-};
-
-__device__ __forceinline__ NoiseRow noise_row(const float* theta, const float* table, const uint16_t* table16,
-                                              const int64_t* offsets, int j) {
-  if (offsets == nullptr) return NoiseRow{theta, nullptr};
-  const int64_t toff = offsets[j];
-  return table16 ? NoiseRow{nullptr, table16 + toff} : NoiseRow{table + toff, nullptr};
-}
 
 struct StatsParams {
   const float* theta;
@@ -283,21 +260,14 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
     const NoiseRow nz = noise_row(p.theta, p.table, p.table16, p.offsets, j);
     const int b0 = chunk * NB, nb = min(NB, p.B - b0);
     const int signs = centre ? 1 : 2;
-    // W+ = theta + sigma*t, W- = theta - sigma*t: the bits of theta + (-sigma)*t (the evaluate's minus member)
-    auto form = [&](int64_t idx, float& wp, float& wm) {
-      const float th = __ldg(p.theta + idx);
-      const float ep = __fmul_rn(sigma, nz(idx));
-      wp = __fadd_rn(th, ep);
-      wm = __fsub_rn(th, ep);
-    };
 
     __syncthreads();   // the previous item's readers of shared memory are done
-    for (int i = tid; i < C1 * 256; i += kT) form(oC1W + i, sW1[i], sW1[C1 * 256 + i]);
-    for (int i = tid; i < C2 * 256; i += kT) form(oC2W + i, sW2[i], sW2[C2 * 256 + i]);
-    if (tid < 16) form(oC1B + tid, sB[tid], sB[16 + tid]);
-    if (tid < 32) form(oC2B + tid, sB[32 + tid], sB[64 + tid]);
-    if (tid < 16) form(oB1 + tid, sB[96 + tid], sB[112 + tid]);
-    if (tid < 32) form(oB2 + tid, sB[128 + tid], sB[160 + tid]);
+    for (int i = tid; i < C1 * 256; i += kT) estk_form_pm(p.theta, nz, sigma, oC1W + i, sW1[i], sW1[C1 * 256 + i]);
+    for (int i = tid; i < C2 * 256; i += kT) estk_form_pm(p.theta, nz, sigma, oC2W + i, sW2[i], sW2[C2 * 256 + i]);
+    if (tid < 16) estk_form_pm(p.theta, nz, sigma, oC1B + tid, sB[tid], sB[16 + tid]);
+    if (tid < 32) estk_form_pm(p.theta, nz, sigma, oC2B + tid, sB[32 + tid], sB[64 + tid]);
+    if (tid < 16) estk_form_pm(p.theta, nz, sigma, oB1 + tid, sB[96 + tid], sB[112 + tid]);
+    if (tid < 32) estk_form_pm(p.theta, nz, sigma, oB2 + tid, sB[128 + tid], sB[160 + tid]);
     __syncthreads();
 
     // ---------------- each sign's frames: conv1, VBN1, ReLU, conv2, VBN2, ReLU -> F[s][b]
@@ -378,7 +348,8 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
       __syncthreads();   // features written / the previous tile consumed
       for (int e = tid; e < FC1 * KT; e += kT) {      // one noise read per weight, both signs; coalesced along k
         const int k = e % KT, jn = e / KT;
-        form(oF1W + (int64_t)jn * P2 + k0 + k, sWtp[k * (FC1 + 1) + jn], sWtm[k * (FC1 + 1) + jn]);
+        estk_form_pm(p.theta, nz, sigma, oF1W + (int64_t)jn * P2 + k0 + k, sWtp[k * (FC1 + 1) + jn],
+                     sWtm[k * (FC1 + 1) + jn]);
       }
       __syncthreads();
 #pragma unroll 4
@@ -393,7 +364,7 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
     }
     {
       float bp, bm;
-      form(oF1B + tid, bp, bm);
+      estk_form_pm(p.theta, nz, sigma, oF1B + tid, bp, bm);
 #pragma unroll
       for (int i = 0; i < NB; ++i) {
         sH[i * FC1 + tid] = fmaxf(accp[i] + bp, 0.f);
@@ -405,12 +376,13 @@ __global__ void __launch_bounds__(kT, 1) conv_act_kernel(const ActParams p) {
     for (int a0 = 0; a0 < A; a0 += FC2_AT) {
       const int na = min(FC2_AT, A - a0);
       __syncthreads();   // fc1 tiles / the previous fc2 tile consumed, sH written
-      for (int e = tid; e < na * FC1; e += kT) form(oF2W + (int64_t)a0 * FC1 + e, sV[e], sV[FC2_AT * FC1 + e]);
+      for (int e = tid; e < na * FC1; e += kT)
+        estk_form_pm(p.theta, nz, sigma, oF2W + (int64_t)a0 * FC1 + e, sV[e], sV[FC2_AT * FC1 + e]);
       __syncthreads();
       for (int e = tid; e < signs * nb * na; e += kT) {
         const int a = e % na, r = e / na, s = r / nb, bl = r % nb;
         float bp, bm;
-        form(oF2B + a0 + a, bp, bm);
+        estk_form_pm(p.theta, nz, sigma, oF2B + a0 + a, bp, bm);
         float y = s ? bm : bp;
         const float* const h = sH + (s * NB + bl) * FC1;
         const float* const w = sV + s * FC2_AT * FC1 + a * FC1;
@@ -474,7 +446,7 @@ int eval_conv_actions(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream)
                  "%s: scratch %lld < %lld bytes (members * ESTK_CONV_VBN_STATS_FLOATS * 4)", who,
                  (long long)c.scratch_bytes, (long long)need);
 
-  const int B = c.B, nb = !c.obs ? 1 : B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
+  const int B = c.B, nb = c.obs ? estk_chunk_rows(B) : 1;
   const int stats_grid = std::min(ctx->sm_count, members);
   const int64_t chunks = c.obs ? (B + nb - 1) / nb : 1;
   const int act_grid = (int)std::min<int64_t>((centre ? 1 : c.pairs) * chunks, ctx->sm_count);

@@ -24,9 +24,6 @@
 // Algorithmic bytes per launch = 4*n*pairs (noise rows; 2*n*pairs from table16) + 4*n (theta)
 // + 4*P*B*(in+out+2S) (observations, state and outputs).
 #include "estk_common.cuh"
-#include <cuda_fp16.h>
-#include <algorithm>
-#include <climits>
 
 namespace {
 
@@ -59,12 +56,6 @@ struct RnnParams {
 // floats of one work item's activations per row: x|h, the gate buffer (GRU: + b_n), h'
 __host__ __device__ inline int rnn_act_width(int cell, int in, int H) {
   return in + H + cell_gates(cell) * H + (cell == ESTK_CELL_GRU ? H : 0) + H;
-}
-
-__device__ __forceinline__ float ld_noise1h(const uint16_t* p) {
-  unsigned short v;
-  asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(v) : "l"(p));
-  return __half2float(__ushort_as_half(v));
 }
 
 template <int BC, int CELL, bool OUT_TANH, bool SLAB>
@@ -100,17 +91,8 @@ __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p)
   for (; slot < (unsigned)p.pairs; chunk += gridDim.x, slot += chunk / p.chunks, chunk %= p.chunks) {
     const int j = p.order ? p.order[slot] : (int)slot;
     const int64_t toff = centre ? 0 : p.offsets[j];
-    const float* const trow = centre ? p.theta : p.table + toff;
-    const uint16_t* const trow16 = (centre || !p.table16) ? nullptr : p.table16 + toff;
+    const NoiseRow nz{centre ? p.theta : p.table + toff, (centre || !p.table16) ? nullptr : p.table16 + toff};
     const int b0 = chunk * BC;
-    // W+ / W- of parameter idx: theta +- (sigma*t), two roundings
-    auto wpm = [&](int64_t idx, float& wp, float& wm) {
-      const float th = __ldg(p.theta + idx);
-      const float t = trow16 ? ld_noise1h(trow16 + idx) : ld_noise1(trow + idx);
-      const float ep = __fmul_rn(sigma, t);
-      wp = __fadd_rn(th, ep);
-      wm = __fsub_rn(th, ep);
-    };
     // acc[i] = fmaf chain over k < K of Xs[k][row_i] * W[o0+c][k], W = this sign's weights at wbase ([nout][K])
     auto chain = [&](float (&acc)[NB], const float* Xs, int K, int64_t wbase, int o0, int nout) {
       for (int k0 = 0; k0 < K; k0 += KT) {
@@ -118,7 +100,8 @@ __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p)
         for (int e = tid; e < OT * KT; e += kThreads) {
           const int k = e % KT, o = e / KT;
           float wp = 0.f, wm = 0.f;
-          if (o0 + o < nout && k0 + k < K) wpm(wbase + (int64_t)(o0 + o) * K + k0 + k, wp, wm);
+          if (o0 + o < nout && k0 + k < K)
+            estk_form_pm(p.theta, nz, sigma, wbase + (int64_t)(o0 + o) * K + k0 + k, wp, wm);
           Wp[k * OTP + o] = wp;
           Wm[k * OTP + o] = wm;
         }
@@ -155,8 +138,8 @@ __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p)
       const int o = o0 + c;
       if (o < GH) {
         float bp, bm, hp, hm;
-        wpm(b_ih + o, bp, bm);
-        wpm(b_hh + o, hp, hm);
+        estk_form_pm(p.theta, nz, sigma, b_ih + o, bp, bm);
+        estk_form_pm(p.theta, nz, sigma, b_hh + o, hp, hm);
         const float bi = minus ? bm : bp, bh = minus ? hm : hp;
 #pragma unroll
         for (int i = 0; i < NB; ++i) {
@@ -215,7 +198,7 @@ __global__ void __launch_bounds__(kThreads, 3) act_rnn_kernel(const RnnParams p)
       const int o = o0 + c;
       if (o < out) {
         float bp, bm;
-        wpm(b_head + o, bp, bm);
+        estk_form_pm(p.theta, nz, sigma, b_head + o, bp, bm);
         const float bias = minus ? bm : bp;
         float* const bc = minus ? p.bc_minus : p.bc_plus;
 #pragma unroll
@@ -237,28 +220,14 @@ size_t tile_bytes(int bc) { return sizeof(float) * 2 * KT * (rnn_ot(bc) + 1); }
 
 template <int BC, int CELL, bool OUT_TANH>
 int launch_rnn(estk_ctx* ctx, RnnParams& p, cudaStream_t stream, const char* who) {
-  const int64_t items = (int64_t)p.pairs * p.chunks;
-  const int64_t act_floats = (int64_t)rnn_act_width(CELL, p.in, p.H) * 2 * BC;
-  const size_t smem_all = tile_bytes(BC) + sizeof(float) * (size_t)act_floats;
-  if (smem_all <= kSmemBudget) {
-    auto kern = act_rnn_kernel<BC, CELL, OUT_TANH, false>;
-    ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_all));
-    const int grid = (int)std::min<int64_t>(items, INT_MAX);
-    kern<<<grid, kThreads, smem_all, stream>>>(p);
-  } else {
-    auto kern = act_rnn_kernel<BC, CELL, OUT_TANH, true>;
-    const size_t smem = tile_bytes(BC);
-    ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-    const int grid = (int)std::min<int64_t>(items, (int64_t)ctx->sm_count * std::max(per_sm, 1));
-    const int rc = estk_ctx_reserve(ctx, 0, 0, stream, who, (int64_t)grid * act_floats);
-    if (rc) return rc;
-    p.slab = ctx->eval_slab;
-    kern<<<grid, kThreads, smem, stream>>>(p);
-  }
-  ESTK_CUDA(cudaGetLastError());
-  return ESTK_OK;
+  SlabLaunch l = {};
+  l.items = (int64_t)p.pairs * p.chunks;
+  l.slab_per_cta = (int64_t)rnn_act_width(CELL, p.in, p.H) * 2 * BC;
+  l.smem_slab = tile_bytes(BC);
+  l.smem_shared = l.smem_slab + sizeof(float) * (size_t)l.slab_per_cta;
+  l.slab = l.smem_shared > kSmemBudget;
+  return estk_launch_eval(ctx, act_rnn_kernel<BC, CELL, OUT_TANH, false>, act_rnn_kernel<BC, CELL, OUT_TANH, true>, p,
+                          l, kThreads, stream, who, [] {});
 }
 
 template <int BC>
@@ -290,8 +259,8 @@ int eval_rnn_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   p.theta = c.theta; p.table = c.table; p.table16 = c.table16; p.offsets = c.offsets; p.order = c.order;
   p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.B = c.B;
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
-  const int B = c.B, bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
-  p.chunks = (B + bc - 1) / bc;
+  const int bc = estk_chunk_rows(c.B);
+  p.chunks = (c.B + bc - 1) / bc;
   switch (bc) {
     case 1: return launch_bc<1>(ctx, p, d.activation, stream, who);
     case 2: return launch_bc<2>(ctx, p, d.activation, stream, who);

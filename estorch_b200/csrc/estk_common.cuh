@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <algorithm>
+#include <climits>
 #include "estk.h"
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
@@ -55,6 +57,15 @@ static inline EvalRoute estk_eval_route(int a) {
   if ((a & 0xff0000) == ESTK_ACTIONS) return cell ? kRouteActionsCell : kRouteActions;
   return cell ? kRouteSequence : kRouteDense;
 }
+// The output head of a code with a return, a compile-time parameter of the sequence and convolutional
+// evaluates: identity, tanhf, or the logits of the cross-entropy (which takes precedence over the Tanh bit)
+constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2;
+static inline int estk_head(int code) {
+  return (code & ESTK_LOSS_XENT) ? kHeadXent : (code & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
+}
+// Rows per sign in one work item of the fp32 act kernels (an environment population): B itself up to 2, then
+// 4, then 8 -- one instantiation per value.
+static inline int estk_chunk_rows(int B) { return B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8; }
 
 #ifdef __CUDACC__
 // y / d rounded to nearest-even in fp32 -- the bits of the IEEE divide y / d -- for d >= 1 or d = +inf,
@@ -134,6 +145,45 @@ static inline unsigned int* estk_member_counters(estk_ctx* c) { return c->counte
 int estk_ctx_reserve(estk_ctx* c, int64_t members, int64_t eval_floats, cudaStream_t stream, const char* who,
                      int64_t slab_floats = 0);
 
+#ifdef __CUDACC__
+// The launch of an fp32 evaluate whose per-item activations live in shared memory when they fit, else in a
+// per-CTA slab of the context workspace (the same kernel code with slab = true, P::slab pointing there).
+struct SlabLaunch {
+  bool slab;                   // the activations are in the slab
+  int64_t items;               // work items; in shared memory each has its own CTA
+  size_t smem_shared;          // dynamic shared memory of the shared-memory kernel
+  size_t smem_slab;            // ... and of the slab kernel
+  int64_t slab_per_cta;        // slab floats of one CTA
+  int64_t members, eval_floats;  // estk_ctx_reserve's; both 0: the call reserves on the slab path only
+  int64_t slab_cap;            // > 0: the grid's slab stays within this many floats, down to one CTA
+};
+// The slab grid is persistent: the resident CTAs (by the occupancy of the slab kernel), at most `items`, and
+// at most slab_cap / slab_per_cta.  `bind` runs after the reservation, so it can take workspace pointers.
+template <class P, class Bind>
+int estk_launch_eval(estk_ctx* ctx, void (*shared_kern)(P), void (*slab_kern)(P), P& p, const SlabLaunch& l,
+                     int threads, cudaStream_t stream, const char* who, Bind bind) {
+  void (*const kern)(P) = l.slab ? slab_kern : shared_kern;
+  const size_t smem = l.slab ? l.smem_slab : l.smem_shared;
+  ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int64_t grid = l.items < INT_MAX ? l.items : INT_MAX;
+  if (l.slab) {
+    int per_sm = 0;
+    ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    grid = std::min<int64_t>(l.items, (int64_t)ctx->sm_count * std::max(per_sm, 1));
+    if (l.slab_cap > 0) grid = std::min<int64_t>(grid, std::max<int64_t>(1, l.slab_cap / l.slab_per_cta));
+  }
+  if (l.members || l.eval_floats || l.slab) {
+    const int rc = estk_ctx_reserve(ctx, l.members, l.eval_floats, stream, who, l.slab ? grid * l.slab_per_cta : 0);
+    if (rc) return rc;
+  }
+  p.slab = l.slab ? ctx->eval_slab : nullptr;
+  bind();
+  kern<<<(int)grid, threads, smem, stream>>>(p);
+  ESTK_CUDA(cudaGetLastError());
+  return ESTK_OK;
+}
+#endif
+
 // ---------------------------------------------------------------- evaluate back ends
 // estk_eval_mlp checks the precision code, builds this record once and hands it to the back end of the
 // activation code (estk_eval_route), which makes its own argument checks.  A centre call (offsets == NULL)
@@ -165,6 +215,12 @@ int eval_mlp_tc(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);     /
 // the first checks of both ESTK_ACTIONS back ends: fp32 only, the pointers, the bc layout, no
 // centre_return_out (target and the returns are not part of the call; estk_eval_mlp_act.cu)
 int eval_actions_check(estk_ctx* ctx, const EvalMlpCall& c);
+// the checks of both back ends that return a loss (the sequence and the convolutional evaluate), in two
+// groups so that each back end's own ESTK_ERR_UNSUPPORTED checks can run between them (estk_eval_rnn_seq.cu):
+// eval_returns_supported: fp32 only, no centre_return_out (ESTK_ERR_UNSUPPORTED);
+// eval_returns_check: the pointers, the bc layout, B and pairs (ESTK_ERR_INVALID)
+int eval_returns_supported(const EvalMlpCall& c, const char* who);
+int eval_returns_check(estk_ctx* ctx, const EvalMlpCall& c, const char* who);
 // kRouteActions: eval_actions_check, its own checks, then the act-mode kernel (estk_eval_mlp_act.cu)
 int eval_mlp_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
 // kRouteActionsCell: eval_actions_check, then one step of the cell + head kernel (estk_act_rnn.cu)
@@ -216,6 +272,7 @@ __host__ __device__ __forceinline__ uint64_t estk_mix64(uint64_t z) {
 
 // ---------------------------------------------------------------- loads
 #ifdef __CUDACC__
+#include <cuda_fp16.h>
 // streaming 128-bit read of the noise table: read-only path, do not pollute L1
 // (every byte is used exactly once per CTA); default L2 policy on purpose --
 // table rows of one generation overlap and are re-read by other CTAs.
@@ -243,6 +300,64 @@ __device__ __forceinline__ float ld_noise1(const float* p) {
   asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p));
   return v;
 }
+__device__ __forceinline__ float ld_noise1h(const uint16_t* p) {
+  unsigned short v;
+  asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(v) : "l"(p));
+  return __half2float(__ushort_as_half(v));
+}
+
+// One pair's noise row: the fp32 table, its exact fp16 copy, or theta itself for the centre (sigma 0).
+// A kernel that reads the fp32 table only passes table16 = nullptr, and the fp16 branch folds away.
+struct NoiseRow {
+  const float* t32;
+  const uint16_t* t16;
+  __device__ __forceinline__ float operator()(int64_t i) const { return t16 ? ld_noise1h(t16 + i) : ld_noise1(t32 + i); }
+};
+__device__ __forceinline__ NoiseRow noise_row(const float* theta, const float* table, const uint16_t* table16,
+                                              const int64_t* offsets, int j) {
+  if (offsets == nullptr) return NoiseRow{theta, nullptr};
+  const int64_t toff = offsets[j];
+  return table16 ? NoiseRow{nullptr, table16 + toff} : NoiseRow{table + toff, nullptr};
+}
+// Parameter idx of both members of a pair: W+ = theta + (sigma*t) and W- = theta - (sigma*t), each with the
+// evaluate's two roundings, so W- has the bits of theta + (-sigma)*t (estk.h)
+__device__ __forceinline__ void estk_form_pm(const float* theta, const NoiseRow& row, float sigma, int64_t idx,
+                                             float& wp, float& wm) {
+  const float th = __ldg(theta + idx);
+  const float ep = __fmul_rn(sigma, row(idx));
+  wp = __fadd_rn(th, ep);
+  wm = __fsub_rn(th, ep);
+}
+// ... and of one member, for a thread that serves one sign
+__device__ __forceinline__ float estk_form_sign(const float* theta, const NoiseRow& row, float sigma, int64_t idx,
+                                                bool minus) {
+  const float th = __ldg(theta + idx);
+  const float ep = __fmul_rn(sigma, row(idx));
+  return minus ? __fsub_rn(th, ep) : __fadd_rn(th, ep);
+}
+
+// The return of a pair whose loss is split over `items` work items (CTAs, or chunks of a persistent CTA).
+// part = [2][n] partials of the pair (+ then -); each is stored and __threadfence'd by its writer before a
+// barrier, after which one thread of the work item arrives on the pair's counter.  The last arrival finishes:
+// a fence that orders its reads of the other work items' partials, the in-order fold of each sign (include/
+// estk.h states it: the bits do not depend on the schedule), ret = -(sum / denom), and the counter back to 0
+// for the next launch.  The finish is a macro, not a function: the fold loop then stays the kernel's own loop,
+// which nvcc unrolls as it did before the finish was shared (an inlined function's loop is unrolled
+// differently, and the kernel's SASS would change).
+__device__ __forceinline__ bool estk_pair_arrive(unsigned int* counter, int items) {
+  return atomicAdd(counter, 1u) == (unsigned int)items - 1;
+}
+#define ESTK_PAIR_FINISH(part, n, denom, ret_plus, ret_minus, j, counter)                                   \
+  do {                                                                                                      \
+    __threadfence();                                                                                        \
+    const float* const pf_ = (part);                                                                        \
+    float sp_ = 0.f, sm_ = 0.f;                                                                             \
+    for (int i_ = 0; i_ < (n); ++i_) { sp_ += __ldcg(pf_ + i_); sm_ += __ldcg(pf_ + (n) + i_); }          \
+    const float d_ = (denom);                                                                               \
+    (ret_plus)[j] = -(sp_ / d_);                                                                            \
+    if (ret_minus) (ret_minus)[j] = -(sm_ / d_);                                                            \
+    *(counter) = 0u;                                                                                        \
+  } while (0)
 __device__ __forceinline__ int warp_sum_i(int v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

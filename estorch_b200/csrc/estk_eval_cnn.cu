@@ -23,8 +23,6 @@
 // below; otherwise they live in a per-CTA slab of the context workspace and a persistent grid loops over the
 // work items (the same code, global instead of shared addresses).  Layer 0 reads the images from `obs`.
 #include "estk_common.cuh"
-#include <algorithm>
-#include <climits>
 
 namespace {
 
@@ -34,7 +32,6 @@ constexpr int kMaxKT = 256;                  // taps per tile
 constexpr size_t kSmemBudget = 220 * 1024;   // up to the 227 KB a CTA may hold
 constexpr size_t kSmemPreferred = 110 * 1024;  // two CTAs per SM
 constexpr int64_t kSlabBudgetFloats = (int64_t)1 << 28;  // 1 GB of slab for the whole grid (at least one CTA's)
-constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2;
 
 struct CnnLayer {
   int cin, hin, win, cout, k, s, pad, ho, wo;
@@ -91,7 +88,7 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
   unsigned int slot = blockIdx.x / (unsigned)p.chunks, chunk = blockIdx.x % (unsigned)p.chunks;
   for (; slot < (unsigned)p.pairs; chunk += gridDim.x, slot += chunk / p.chunks, chunk %= p.chunks) {
     const int j = p.order ? p.order[slot] : (int)slot;
-    const float* const trow = centre ? p.theta : p.table + p.offsets[j];
+    const NoiseRow nz{centre ? p.theta : p.table + p.offsets[j], nullptr};   // the fp32 table only
     const int b0 = chunk * BC;
     const int nb = min(BC, p.B - b0);                // images of this chunk (rows past it read zeros)
 
@@ -113,7 +110,7 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
             const int og = e / kt, t = e % kt;
             const int64_t idx = ly.wbase + (int64_t)(oc0 + og) * ly.K + k0 + t;
             const float th = __ldg(p.theta + idx);
-            const float ep = __fmul_rn(sigma, ld_noise1(trow + idx));
+            const float ep = __fmul_rn(sigma, nz(idx));
             Wp[og * kt + t] = __fadd_rn(th, ep);
             Wm[og * kt + t] = __fsub_rn(th, ep);
           }
@@ -155,9 +152,7 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
             }
             if (fin) {
               const int64_t bidx = ly.wbase + (int64_t)ly.cout * ly.K + oc0 + og;
-              const float th = __ldg(p.theta + bidx);
-              const float ep = __fmul_rn(sigma, ld_noise1(trow + bidx));
-              float y = acc + (minus ? __fsub_rn(th, ep) : __fadd_rn(th, ep));
+              float y = acc + estk_form_sign(p.theta, nz, sigma, bidx, minus);
               if (!last) y = estk_hidden_act<HID, true>(y);   // SiLU without the div.rn call: the same bits
               else if (HEAD == kHeadTanh) y = tanhf(y);
               acc = y;
@@ -203,19 +198,10 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
       __threadfence();
     }
     __syncthreads();
-    if (tid == 0) {
-      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
-      if (arrived == (unsigned int)p.chunks - 1) {
-        __threadfence();
-        const float* const part = p.partial + (size_t)slot * 2 * p.B;
-        float sp = 0.f, sm = 0.f;
-        for (int i = 0; i < p.B; ++i) { sp += __ldcg(part + i); sm += __ldcg(part + p.B + i); }
-        const float denom = (float)((int64_t)p.B * (HEAD == kHeadXent ? 1 : p.out));
-        p.ret_plus[j] = -(sp / denom);
-        if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
-        p.counters[slot] = 0u;  // ready for the next launch
-      }
-    }
+    if (tid == 0 && estk_pair_arrive(p.counters + slot, p.chunks))
+      ESTK_PAIR_FINISH(p.partial + (size_t)slot * 2 * p.B, p.B,
+                       (float)((int64_t)p.B * (HEAD == kHeadXent ? 1 : p.out)), p.ret_plus, p.ret_minus, j,
+                       p.counters + slot);
   }
 }
 
@@ -233,33 +219,25 @@ int launch_cnn(estk_ctx* ctx, CnnParams& p, cudaStream_t stream, const char* who
     }
     if (bc) break;
   }
-  const bool slab = bc == 0;
-  if (slab) bc = 1;
+  SlabLaunch l = {};
+  l.slab = bc == 0;
+  if (l.slab) bc = 1;
   p.BC = bc;
   p.chunks = (p.B + bc - 1) / bc;
-  const int64_t items = (int64_t)p.pairs * p.chunks;
-  const int64_t act_floats = (int64_t)2 * p.maxact * 2 * bc;
-  auto kern = slab ? eval_cnn_kernel<HID, HEAD, true> : eval_cnn_kernel<HID, HEAD, false>;
-  const size_t smem = slab ? fixed_smem() : smem_all;
-  ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int grid = (int)std::min<int64_t>(items, INT_MAX);
-  if (slab) {
-    // resident CTAs, but never more slab than kSlabBudgetFloats (down to one CTA): the persistent loop serves any
-    // grid, so a large image costs the memory of a few CTAs' buffers, not of every resident CTA's
-    int per_sm = 0;
-    ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-    const int64_t by_memory = std::max<int64_t>(1, kSlabBudgetFloats / act_floats);
-    grid = (int)std::min<int64_t>({items, (int64_t)ctx->sm_count * std::max(per_sm, 1), by_memory});
-  }
-  const int rc = estk_ctx_reserve(ctx, p.pairs, (int64_t)p.pairs * 2 * p.B, stream, who,
-                                  slab ? (int64_t)grid * act_floats : 0);
-  if (rc) return rc;
-  p.partial = ctx->eval_partial;
-  p.counters = estk_member_counters(ctx);
-  p.slab = slab ? ctx->eval_slab : nullptr;
-  kern<<<grid, kThreads, smem, stream>>>(p);
-  ESTK_CUDA(cudaGetLastError());
-  return ESTK_OK;
+  l.items = (int64_t)p.pairs * p.chunks;
+  l.smem_shared = smem_all;
+  l.smem_slab = fixed_smem();
+  l.slab_per_cta = (int64_t)2 * p.maxact * 2 * bc;
+  l.members = p.pairs;
+  l.eval_floats = (int64_t)p.pairs * 2 * p.B;
+  // the persistent loop serves any grid, so a large image costs the memory of a few CTAs' buffers, not of
+  // every resident CTA's
+  l.slab_cap = kSlabBudgetFloats;
+  return estk_launch_eval(ctx, eval_cnn_kernel<HID, HEAD, false>, eval_cnn_kernel<HID, HEAD, true>, p, l, kThreads,
+                          stream, who, [&] {
+                            p.partial = ctx->eval_partial;
+                            p.counters = estk_member_counters(ctx);
+                          });
 }
 
 template <int HID>
@@ -273,16 +251,7 @@ int launch_hid(estk_ctx* ctx, CnnParams& p, int head, cudaStream_t stream, const
 
 int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   const char* who = "estk_eval_mlp[convolutional]";
-  const bool centre = call.offsets == nullptr;
-  if (call.precision != ESTK_PREC_FP32) {
-    estk_set_error("%s: precision %d is not supported: a convolutional policy is computed with ESTK_PREC_FP32 "
-                   "only", who, call.precision);
-    return ESTK_ERR_UNSUPPORTED;
-  }
-  if (call.centre_out) {
-    estk_set_error("%s: centre_return_out (folded centre rollout) needs a tensor-core precision", who);
-    return ESTK_ERR_UNSUPPORTED;
-  }
+  if (const int rc = eval_returns_supported(call, who)) return rc;
   const estk_mlp_desc& d = call.desc;
   const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
   ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
@@ -297,16 +266,7 @@ int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   ESTK_CHECK_ARG(d.n_layers > n_conv && d.n_layers <= ESTK_MAX_LAYERS,
                  "%s: n_layers=%d must exceed n_conv=%d (at least one Linear) and be at most %d", who, d.n_layers,
                  n_conv, ESTK_MAX_LAYERS);
-  ESTK_CHECK_ARG(ctx && call.theta && call.obs && call.target && call.ret_plus &&
-                 (centre || (call.table && call.ret_minus)),
-                 "%s: null argument (theta, obs, target, returns_plus, and for a population table and "
-                 "returns_minus)", who);
-  ESTK_CHECK_ARG(centre || (call.bc_plus == nullptr) == (call.bc_minus == nullptr),
-                 "%s: bc_plus/bc_minus must both be set or both null", who);
-  ESTK_CHECK_ARG(!call.bc_plus || (call.bc_obs > 0 && call.bc_dim > 0),
-                 "%s: bc_obs/bc_dim must be positive with bc outputs", who);
-  ESTK_CHECK_ARG(call.B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(call.pairs >= 1 && call.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, call.pairs);
+  if (const int rc = eval_returns_check(ctx, call, who)) return rc;
 
   CnnParams p = {};
   const uint32_t in = (uint32_t)d.dims[0];
@@ -350,7 +310,7 @@ int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   p.pairs = call.pairs; p.sigma = call.sigma; p.obs = call.obs; p.target = call.target; p.B = call.B;
   p.ret_plus = call.ret_plus; p.ret_minus = call.ret_minus;
   p.bc_plus = call.bc_plus; p.bc_minus = call.bc_minus; p.bc_obs = call.bc_obs; p.bc_dim = call.bc_dim;
-  const int head = (low & ESTK_LOSS_XENT) ? kHeadXent : (low & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
+  const int head = estk_head(low);
   switch (low & 0xff) {
     case ESTK_ACT_TANH: return launch_hid<ESTK_ACT_TANH>(ctx, p, head, stream, who);
     case ESTK_ACT_ELU: return launch_hid<ESTK_ACT_ELU>(ctx, p, head, stream, who);

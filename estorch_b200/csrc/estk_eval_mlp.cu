@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
   const int chunk = blockIdx.x % p.chunks;
   const int j = p.order ? p.order[slot] : slot;
   const bool centre = (p.offsets == nullptr);
-  const float* trow = centre ? p.theta : p.table + p.offsets[j];
+  const NoiseRow nz{centre ? p.theta : p.table + p.offsets[j], nullptr};   // the fp32 table only
   const float sigma = centre ? 0.f : p.sigma;
   const int b0 = chunk * BC;
   const int L = p.desc.n_layers;
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
           if (o0 + o < out && k0 + k < in) {
             const int64_t idx = wbase + (int64_t)(o0 + o) * in + k0 + k;
             const float th = __ldg(p.theta + idx);
-            const float ep = __fmul_rn(sigma, ld_noise1(trow + idx));
+            const float ep = __fmul_rn(sigma, nz(idx));
             wp = __fadd_rn(th, ep);
             wm = __fsub_rn(th, ep);
           }
@@ -146,9 +146,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
       for (int c = 0; c < 4; ++c) {
         const int o = o0 + tc * 4 + c;
         if (o >= out) continue;
-        const float th = __ldg(p.theta + bbase + o);
-        const float ep = __fmul_rn(sigma, ld_noise1(trow + bbase + o));
-        const float bias = minus ? __fsub_rn(th, ep) : __fadd_rn(th, ep);
+        const float bias = estk_form_sign(p.theta, nz, sigma, bbase + o, minus);
         float y[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
@@ -225,20 +223,13 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
       part[chunk] = sp;
       part[p.chunks + chunk] = sm;
       __threadfence();
-      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
-      s_last = (arrived == (unsigned int)p.chunks - 1);
+      s_last = estk_pair_arrive(p.counters + slot, p.chunks);
     }
     __syncthreads();
-    if (s_last && tid == 0) {
-      __threadfence();
-      const float* part = p.partial + ((size_t)slot * 2) * p.chunks;
-      float sp = 0.f, sm = 0.f;
-      for (int c = 0; c < p.chunks; ++c) { sp += __ldcg(part + c); sm += __ldcg(part + p.chunks + c); }
-      const float denom = XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L];
-      p.ret_plus[j] = -(sp / denom);
-      if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
-      p.counters[slot] = 0u;  // ready for the next launch
-    }
+    if (s_last && tid == 0)
+      ESTK_PAIR_FINISH(p.partial + ((size_t)slot * 2) * p.chunks, p.chunks,
+                       XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus, p.ret_minus, j,
+                       p.counters + slot);
   }
 }
 
@@ -331,7 +322,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
     const int slot = (int)(item / p.chunks);
     const int chunk = (int)(item % p.chunks);
     const int j = p.order ? p.order[slot] : slot;
-    const float* trow = centre ? p.theta : p.table + p.offsets[j];
+    const NoiseRow nz{centre ? p.theta : p.table + p.offsets[j], nullptr};   // the fp32 table only
     const int b0 = chunk * BC;
     float loss = 0.f;
     int64_t pbase = 0;
@@ -371,7 +362,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
             if (o0 + o < out && k0 + k < in) {
               const int64_t idx = wbase + (int64_t)(o0 + o) * in + k0 + k;
               th[i] = __ldg(p.theta + idx);
-              tv[i] = ld_noise1(trow + idx);
+              tv[i] = nz(idx);
             }
           }
         };
@@ -414,9 +405,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
         for (int c = 0; c < 8; ++c) {
           const int o = o0 + (c >> 2) * 32 + tc * 4 + (c & 3);
           if (o >= out) continue;
-          const float th0 = __ldg(p.theta + bbase + o);
-          const float ep = __fmul_rn(sigma, ld_noise1(trow + bbase + o));
-          const float bias = minus ? __fsub_rn(th0, ep) : __fadd_rn(th0, ep);
+          const float bias = estk_form_sign(p.theta, nz, sigma, bbase + o, minus);
           float y[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i) y[i] = acc[i][c] + bias;
@@ -489,16 +478,9 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
       part[chunk] = sp;
       part[p.chunks + chunk] = sm;
       __threadfence();
-      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
-      if (arrived == (unsigned int)p.chunks - 1) {
-        __threadfence();
-        sp = sm = 0.f;
-        for (int c = 0; c < p.chunks; ++c) { sp += __ldcg(part + c); sm += __ldcg(part + p.chunks + c); }
-        const float denom = XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L];
-        p.ret_plus[j] = -(sp / denom);
-        if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
-        p.counters[slot] = 0u;  // ready for the next launch
-      }
+      if (estk_pair_arrive(p.counters + slot, p.chunks))
+        ESTK_PAIR_FINISH(part, p.chunks, XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus,
+                         p.ret_minus, j, p.counters + slot);
     }
   }
 }

@@ -24,9 +24,6 @@
 // Algorithmic bytes per launch = 4*n*pairs (noise rows; 2*n*pairs from table16) + 4*n (theta)
 // + 4*P*B*(in+out) (observations and outputs).
 #include "estk_common.cuh"
-#include <cuda_fp16.h>
-#include <algorithm>
-#include <climits>
 
 namespace {
 
@@ -54,12 +51,6 @@ struct ActParams {
   int bc_obs, bc_dim;
   float* slab;               // SLAB: [gridDim.x][2][maxw][ROWS]
 };
-
-__device__ __forceinline__ float ld_noise1h(const uint16_t* p) {
-  unsigned short v;
-  asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(v) : "l"(p));
-  return __half2float(__ushort_as_half(v));
-}
 
 template <int BC, int ACT, bool SLAB>
 __global__ void __launch_bounds__(kThreads, 4) eval_mlp_act_kernel(const ActParams p) {
@@ -91,8 +82,7 @@ __global__ void __launch_bounds__(kThreads, 4) eval_mlp_act_kernel(const ActPara
   for (; slot < (unsigned)p.pairs; chunk += gridDim.x, slot += chunk / p.chunks, chunk %= p.chunks) {
     const int j = p.order ? p.order[slot] : (int)slot;
     const int64_t toff = centre ? 0 : p.offsets[j];
-    const float* const trow = centre ? p.theta : p.table + toff;
-    const uint16_t* const trow16 = (centre || !p.table16) ? nullptr : p.table16 + toff;
+    const NoiseRow nz{centre ? p.theta : p.table + toff, (centre || !p.table16) ? nullptr : p.table16 + toff};
     const int b0 = chunk * BC;
     float* X = act0;
     float* Y = act1;
@@ -122,14 +112,8 @@ __global__ void __launch_bounds__(kThreads, 4) eval_mlp_act_kernel(const ActPara
           for (int e = tid; e < OT * KT; e += kThreads) {
             const int k = e % KT, o = e / KT;
             float wp = 0.f, wm = 0.f;
-            if (o0 + o < out && k0 + k < in) {
-              const int64_t idx = wbase + (int64_t)(o0 + o) * in + k0 + k;
-              const float th = __ldg(p.theta + idx);
-              const float t = trow16 ? ld_noise1h(trow16 + idx) : ld_noise1(trow + idx);
-              const float ep = __fmul_rn(sigma, t);
-              wp = __fadd_rn(th, ep);
-              wm = __fsub_rn(th, ep);
-            }
+            if (o0 + o < out && k0 + k < in)
+              estk_form_pm(p.theta, nz, sigma, wbase + (int64_t)(o0 + o) * in + k0 + k, wp, wm);
             Wp[k * OTP + o] = wp;
             Wm[k * OTP + o] = wm;
           }
@@ -147,10 +131,7 @@ __global__ void __launch_bounds__(kThreads, 4) eval_mlp_act_kernel(const ActPara
         // ---- tile epilogue: bias (+-), hidden activation into Y, or the output activation into bc
         const int o = o0 + c;
         if (o < out) {
-          const float th = __ldg(p.theta + bbase + o);
-          const float t = trow16 ? ld_noise1h(trow16 + bbase + o) : ld_noise1(trow + bbase + o);
-          const float ep = __fmul_rn(sigma, t);
-          const float bias = minus ? __fsub_rn(th, ep) : __fadd_rn(th, ep);
+          const float bias = estk_form_sign(p.theta, nz, sigma, bbase + o, minus);
           float* const bc = minus ? p.bc_minus : p.bc_plus;
 #pragma unroll
           for (int i = 0; i < NB; ++i) {
@@ -181,27 +162,14 @@ size_t act_bytes(int bc, int maxw) { return sizeof(float) * 2 * (size_t)maxw * 2
 
 template <int BC, int ACT>
 int launch_act(estk_ctx* ctx, ActParams& p, cudaStream_t stream, const char* who) {
-  const int64_t items = (int64_t)p.pairs * p.chunks;
-  const size_t smem_all = tile_bytes(BC) + act_bytes(BC, p.maxw);
-  if (smem_all <= kSmemBudget) {
-    auto kern = eval_mlp_act_kernel<BC, ACT, false>;
-    ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_all));
-    const int grid = (int)std::min<int64_t>(items, INT_MAX);
-    kern<<<grid, kThreads, smem_all, stream>>>(p);
-  } else {
-    auto kern = eval_mlp_act_kernel<BC, ACT, true>;
-    const size_t smem = tile_bytes(BC);
-    ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-    const int grid = (int)std::min<int64_t>(items, (int64_t)ctx->sm_count * std::max(per_sm, 1));
-    const int rc = estk_ctx_reserve(ctx, 0, 0, stream, who, (int64_t)grid * 2 * p.maxw * 2 * BC);
-    if (rc) return rc;
-    p.slab = ctx->eval_slab;
-    kern<<<grid, kThreads, smem, stream>>>(p);
-  }
-  ESTK_CUDA(cudaGetLastError());
-  return ESTK_OK;
+  SlabLaunch l = {};
+  l.items = (int64_t)p.pairs * p.chunks;
+  l.smem_slab = tile_bytes(BC);
+  l.smem_shared = l.smem_slab + act_bytes(BC, p.maxw);
+  l.slab = l.smem_shared > kSmemBudget;
+  l.slab_per_cta = (int64_t)2 * p.maxw * 2 * BC;
+  return estk_launch_eval(ctx, eval_mlp_act_kernel<BC, ACT, false>, eval_mlp_act_kernel<BC, ACT, true>, p, l,
+                          kThreads, stream, who, [] {});
 }
 
 template <int BC>
@@ -252,8 +220,8 @@ int eval_mlp_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   p.desc = d; p.theta = c.theta; p.table = c.table; p.table16 = c.table16; p.offsets = c.offsets; p.order = c.order;
   p.pairs = c.pairs; p.sigma = c.sigma; p.obs = c.obs; p.B = c.B; p.maxw = maxw;
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
-  const int B = c.B, bc = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
-  p.chunks = (B + bc - 1) / bc;
+  const int bc = estk_chunk_rows(c.B);
+  p.chunks = (c.B + bc - 1) / bc;
   switch (bc) {
     case 1: return launch_bc<1>(ctx, p, stream, who);
     case 2: return launch_bc<2>(ctx, p, stream, who);

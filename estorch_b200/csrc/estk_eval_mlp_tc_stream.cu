@@ -338,16 +338,9 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
       part[chunk] = sp;
       part[p.chunks + chunk] = sm;
       __threadfence();
-      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
-      if (arrived == (unsigned int)p.chunks - 1) {
-        __threadfence();
-        float tp = 0.f, tm = 0.f;
-        for (int c = 0; c < p.chunks; ++c) { tp += __ldcg(part + c); tm += __ldcg(part + p.chunks + c); }
-        const float denom = XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L];
-        p.ret_plus[j] = -(tp / denom);
-        if (p.ret_minus) p.ret_minus[j] = -(tm / denom);
-        p.counters[slot] = 0u;  // ready for the next launch
-      }
+      if (estk_pair_arrive(p.counters + slot, p.chunks))
+        ESTK_PAIR_FINISH(part, p.chunks, XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus,
+                         p.ret_minus, j, p.counters + slot);
     }
   }
 }

@@ -22,8 +22,6 @@
 // Algorithmic bytes per launch = 4*n*pairs (noise rows) + 4*n (theta) + 4*B*T*(in+out) (observations and
 // targets) + 4*P (returns); the weights are re-formed T times per work item from L1 / L2.
 #include "estk_common.cuh"
-#include <algorithm>
-#include <climits>
 
 namespace {
 
@@ -32,7 +30,6 @@ constexpr int KT = 32;                       // k-chunk of the weight tile
 // activations + tiles in shared memory, up to the 227 KB a CTA may hold; above it the activations stream
 // through the slab (DESIGN §9 has this budget against 96 KB at H = 128 - 256)
 constexpr size_t kSmemBudget = 220 * 1024;
-constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2;
 
 // row groups per CTA: 2 (one per sign) for a single row per sign, else 4
 __host__ __device__ constexpr int seq_groups(int bc) { return bc == 1 ? 2 : 4; }
@@ -97,15 +94,8 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
   unsigned int slot = blockIdx.x / (unsigned)p.chunks, chunk = blockIdx.x % (unsigned)p.chunks;
   for (; slot < (unsigned)p.pairs; chunk += gridDim.x, slot += chunk / p.chunks, chunk %= p.chunks) {
     const int j = p.order ? p.order[slot] : (int)slot;
-    const float* const trow = centre ? p.theta : p.table + p.offsets[j];
+    const NoiseRow nz{centre ? p.theta : p.table + p.offsets[j], nullptr};   // the fp32 table only
     const int b0 = chunk * BC;
-    // W+ / W- of parameter idx: theta +- (sigma*t), two roundings
-    auto wpm = [&](int64_t idx, float& wp, float& wm) {
-      const float th = __ldg(p.theta + idx);
-      const float ep = __fmul_rn(sigma, ld_noise1(trow + idx));
-      wp = __fadd_rn(th, ep);
-      wm = __fsub_rn(th, ep);
-    };
     // acc[i] = fmaf chain over k < K of Xs[k][row_i] * W[o0+c][k], W = this sign's weights at wbase ([nout][K])
     auto chain = [&](float (&acc)[NB], const float* Xs, int K, int64_t wbase, int o0, int nout) {
       for (int k0 = 0; k0 < K; k0 += KT) {
@@ -113,7 +103,8 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
         for (int e = tid; e < OT * KT; e += kThreads) {
           const int k = e % KT, o = e / KT;
           float wp = 0.f, wm = 0.f;
-          if (o0 + o < nout && k0 + k < K) wpm(wbase + (int64_t)(o0 + o) * K + k0 + k, wp, wm);
+          if (o0 + o < nout && k0 + k < K)
+            estk_form_pm(p.theta, nz, sigma, wbase + (int64_t)(o0 + o) * K + k0 + k, wp, wm);
           Wp[k * OTP + o] = wp;
           Wm[k * OTP + o] = wm;
         }
@@ -157,8 +148,8 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
         const int o = o0 + c;
         if (o < GH) {
           float bp, bm, hp, hm;
-          wpm(b_ih + o, bp, bm);
-          wpm(b_hh + o, hp, hm);
+          estk_form_pm(p.theta, nz, sigma, b_ih + o, bp, bm);
+          estk_form_pm(p.theta, nz, sigma, b_hh + o, hp, hm);
           const float bi = minus ? bm : bp, bh = minus ? hm : hp;
 #pragma unroll
           for (int i = 0; i < NB; ++i) {
@@ -209,7 +200,7 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
         const int o = o0 + c;
         if (o < out) {
           float bp, bm;
-          wpm(b_head + o, bp, bm);
+          estk_form_pm(p.theta, nz, sigma, b_head + o, bp, bm);
           const float bias = minus ? bm : bp;
           float* const bc = minus ? p.bc_minus : p.bc_plus;
 #pragma unroll
@@ -263,20 +254,10 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
       __threadfence();
     }
     __syncthreads();
-    if (tid == 0) {
-      const unsigned int arrived = atomicAdd(p.counters + slot, 1u);
-      if (arrived == (unsigned int)p.chunks - 1) {
-        __threadfence();
-        const float* const part = p.partial + (size_t)slot * 2 * p.B;
-        float sp = 0.f, sm = 0.f;
-        for (int s = 0; s < p.B; ++s) { sp += __ldcg(part + s); sm += __ldcg(part + p.B + s); }
-        const int64_t cnt = (int64_t)p.B * T * (HEAD == kHeadXent ? 1 : out);
-        const float denom = (float)cnt;
-        p.ret_plus[j] = -(sp / denom);
-        if (p.ret_minus) p.ret_minus[j] = -(sm / denom);
-        p.counters[slot] = 0u;  // ready for the next launch
-      }
-    }
+    if (tid == 0 && estk_pair_arrive(p.counters + slot, p.chunks))
+      ESTK_PAIR_FINISH(p.partial + (size_t)slot * 2 * p.B, p.B,
+                       (float)((int64_t)p.B * T * (HEAD == kHeadXent ? 1 : out)), p.ret_plus, p.ret_minus, j,
+                       p.counters + slot);
   }
 }
 
@@ -285,33 +266,24 @@ size_t tile_bytes(int bc) { return sizeof(float) * 2 * KT * (seq_ot(bc) + 1); }
 template <int BC, int CELL, int HEAD>
 int launch_seq(estk_ctx* ctx, SeqParams& p, cudaStream_t stream, const char* who) {
   p.chunks = (p.B + BC - 1) / BC;
-  const int64_t items = (int64_t)p.pairs * p.chunks;
-  const int64_t act_floats = (int64_t)seq_act_width(CELL, p.in, p.H, p.out) * 2 * BC;
-  const size_t smem_all = tile_bytes(BC) + sizeof(float) * (size_t)act_floats;
-  const bool slab = smem_all > kSmemBudget;
-  auto kern = slab ? eval_rnn_seq_kernel<BC, CELL, HEAD, true> : eval_rnn_seq_kernel<BC, CELL, HEAD, false>;
-  const size_t smem = slab ? tile_bytes(BC) : smem_all;
-  ESTK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int grid = (int)std::min<int64_t>(items, INT_MAX);
-  if (slab) {
-    int per_sm = 0;
-    ESTK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-    grid = (int)std::min<int64_t>(items, (int64_t)ctx->sm_count * std::max(per_sm, 1));
-  }
-  const int rc = estk_ctx_reserve(ctx, p.pairs, (int64_t)p.pairs * 2 * p.B, stream, who,
-                                  slab ? (int64_t)grid * act_floats : 0);
-  if (rc) return rc;
-  p.partial = ctx->eval_partial;
-  p.counters = estk_member_counters(ctx);
-  p.slab = slab ? ctx->eval_slab : nullptr;
-  kern<<<grid, kThreads, smem, stream>>>(p);
-  ESTK_CUDA(cudaGetLastError());
-  return ESTK_OK;
+  SlabLaunch l = {};
+  l.items = (int64_t)p.pairs * p.chunks;
+  l.slab_per_cta = (int64_t)seq_act_width(CELL, p.in, p.H, p.out) * 2 * BC;
+  l.smem_slab = tile_bytes(BC);
+  l.smem_shared = l.smem_slab + sizeof(float) * (size_t)l.slab_per_cta;
+  l.slab = l.smem_shared > kSmemBudget;
+  l.members = p.pairs;
+  l.eval_floats = (int64_t)p.pairs * 2 * p.B;
+  return estk_launch_eval(ctx, eval_rnn_seq_kernel<BC, CELL, HEAD, false>, eval_rnn_seq_kernel<BC, CELL, HEAD, true>,
+                          p, l, kThreads, stream, who, [&] {
+                            p.partial = ctx->eval_partial;
+                            p.counters = estk_member_counters(ctx);
+                          });
 }
 
 template <int BC>
 int launch_bc(estk_ctx* ctx, SeqParams& p, int code, cudaStream_t stream, const char* who) {
-  const int head = (code & ESTK_LOSS_XENT) ? kHeadXent : (code & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
+  const int head = estk_head(code);
   if ((code & 0xff) == ESTK_CELL_GRU) {
     if (head == kHeadXent) return launch_seq<BC, ESTK_CELL_GRU, kHeadXent>(ctx, p, stream, who);
     if (head == kHeadTanh) return launch_seq<BC, ESTK_CELL_GRU, kHeadTanh>(ctx, p, stream, who);
@@ -324,11 +296,9 @@ int launch_bc(estk_ctx* ctx, SeqParams& p, int code, cudaStream_t stream, const 
 
 }  // namespace
 
-int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
-  const char* who = "estk_eval_mlp[recurrent cell, sequence]";
-  const bool centre = c.offsets == nullptr;
+int eval_returns_supported(const EvalMlpCall& c, const char* who) {
   if (c.precision != ESTK_PREC_FP32) {
-    estk_set_error("%s: the sequence evaluate is computed with ESTK_PREC_FP32 only (precision %d)", who,
+    estk_set_error("%s: precision %d is not supported: this evaluate is computed with ESTK_PREC_FP32 only", who,
                    c.precision);
     return ESTK_ERR_UNSUPPORTED;
   }
@@ -336,6 +306,11 @@ int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) 
     estk_set_error("%s: centre_return_out (folded centre rollout) needs a tensor-core precision", who);
     return ESTK_ERR_UNSUPPORTED;
   }
+  return ESTK_OK;
+}
+
+int eval_returns_check(estk_ctx* ctx, const EvalMlpCall& c, const char* who) {
+  const bool centre = c.offsets == nullptr;
   ESTK_CHECK_ARG(ctx && c.theta && c.obs && c.target && c.ret_plus && (centre || (c.table && c.ret_minus)),
                  "%s: null argument (theta, obs, target, returns_plus, and for a population table and "
                  "returns_minus)", who);
@@ -343,6 +318,15 @@ int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) 
                  "%s: bc_plus/bc_minus must both be set or both null", who);
   ESTK_CHECK_ARG(!c.bc_plus || (c.bc_obs > 0 && c.bc_dim > 0), "%s: bc_obs/bc_dim must be positive with bc outputs",
                  who);
+  ESTK_CHECK_ARG(c.B >= 1, "%s: B must be positive", who);
+  ESTK_CHECK_ARG(c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, c.pairs);
+  return ESTK_OK;
+}
+
+int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
+  const char* who = "estk_eval_mlp[recurrent cell, sequence]";
+  if (const int rc = eval_returns_supported(c, who)) return rc;
+  if (const int rc = eval_returns_check(ctx, c, who)) return rc;
   const estk_mlp_desc& d = c.desc;
   ESTK_CHECK_ARG(d.n_layers == 2, "%s: a recurrent cell is n_layers = 2, dims = (in, H, out, T) (n_layers=%d)", who,
                  d.n_layers);
@@ -351,8 +335,6 @@ int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) 
   // the parameter count and every row width fit comfortably in 32 bits for the widths accepted here
   ESTK_CHECK_ARG(d.dims[0] <= (1 << 16) && d.dims[1] <= (1 << 13) && d.dims[2] <= (1 << 16),
                  "%s: dims (%d, %d, %d) exceed (65536, 8192, 65536)", who, d.dims[0], d.dims[1], d.dims[2]);
-  ESTK_CHECK_ARG(c.B >= 1, "%s: B must be positive", who);
-  ESTK_CHECK_ARG(c.pairs >= 1 && c.pairs <= ESTK_MAX_POPULATION / 2, "%s: pairs=%d", who, c.pairs);
   SeqParams p = {};
   p.in = d.dims[0]; p.H = d.dims[1]; p.out = d.dims[2]; p.T = d.dims[3];
   p.theta = c.theta; p.table = c.table; p.offsets = c.offsets; p.order = c.order; p.pairs = c.pairs;

@@ -335,6 +335,10 @@ code=N_CONV(1)|GRU|ACTIONS precision=1                              | UU
 code=N_CONV(8)|ACTIONS                                              | II
 code=N_CONV(8)|ACTIONS B=0                                          | II
 code=N_CONV(8)|ACTIONS precision=1                                  | UU
+code=N_CONV(1)|ACTIONS theta=NULL                                   | UU
+code=N_CONV(1)|ACTIONS ctx=NULL                                     | UU
+code=N_CONV(1)|ACTIONS bc_plus=NULL bc_minus=FAKE                   | UU
+code=N_CONV(8)|ACTIONS theta=NULL                                   | II
 code=N_CONV(1)|XENT|OUT_TANH                                        | II
 code=N_CONV(1)|XENT|OUT_TANH B=0                                    | II
 code=N_CONV(1)|XENT|OUT_TANH precision=1                            | UU
