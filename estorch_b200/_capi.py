@@ -1,4 +1,5 @@
-"""ctypes binding of libestk.so (the C ABI declared in include/estk.h and include/estk_batch.h).
+"""ctypes binding of libestk.so (the C ABI declared in include/estk.h, include/estk_batch.h and
+include/estk_act_cnn.h).
 
 The library is built in-tree by ``estorch_b200/csrc/build.sh`` (or
 ``__graft_entry__.build()``).  There is NO fallback: if the shared object is
@@ -114,6 +115,11 @@ BATCH_SIGNATURES = {
     "estk_sample_batch": [_P, _U64, _P, _I64, _I64, _I32, _P, _I64, _P, _P, _I64, _P, _P, _P],
 }
 
+# include/estk_act_cnn.h: population mode for convolutional policies, declared beside the core of estk.h
+ACT_CNN_SIGNATURES = {
+    "estk_act_cnn": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _P],
+}
+
 _lib = None
 
 
@@ -128,7 +134,7 @@ def load():
             "`bash estorch_b200/csrc/build.sh` (or `python -c 'import __graft_entry__ as g; "
             "g.build()'`). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in {**SIGNATURES, **BATCH_SIGNATURES}.items():
+    for name, argtypes in {**SIGNATURES, **BATCH_SIGNATURES, **ACT_CNN_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = (C.c_char_p if name == "estk_last_error" else

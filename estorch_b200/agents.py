@@ -205,6 +205,16 @@ class PopulationAgent:
     torch.  In population mode one fused launch computes every member's cell step and head; the returned
     state is the next call's ``state``, and the agent owns it (resetting it where an episode ends, say).
 
+    A generic convolutional policy -- a Conv2d stack, a flatten and Linear layers, as ``DeviceAgent``'s
+    convolutional evaluate recognises it -- runs in population mode when the subclass sets ``obs_shape`` to
+    ``(c, h, w)``, the shape of one observation: a Conv2d stack does not fix H and W, and the agent has no
+    observations to read them from before its episodes.  ``act`` then takes images ``[members, c, h, w]`` or
+    ``[members, B, c, h, w]`` and returns ``[members, out]`` or ``[members, B, out]``, every member's forward on
+    its own images in one fused launch.  Without ``obs_shape`` such a policy runs in hooks mode; a value that is
+    not three positive ints is a ``ValueError`` when ``ES`` is built.  A plain ``Conv2d`` takes ``[1, c, h, w]``
+    but not ``[1, B, c, h, w]``, so an agent that plays B > 1 games per member overrides ``rollout`` to fold B
+    into the batch (examples/cnn_catch.py), and then also runs in hooks mode and under the reference.
+
     ``rollout(policy)`` -- the reference protocol -- is ``rollout_population`` with ``members == 1`` and
     ``act = policy`` (with the state passed through for a recurrent policy), so the same object also runs
     in hooks mode and under the reference itself.
@@ -213,6 +223,7 @@ class PopulationAgent:
 
     device = torch.device("cpu")
     bc_dim = 0
+    obs_shape = None
 
     def rollout_population(self, act, members: int):
         raise NotImplementedError

@@ -354,6 +354,27 @@ class CudaBackend:
         self.eval_cnn(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
                       bc_dim, precision=precision, act=act)
 
+    def act_cnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act):
+        """Every perturbed convolutional policy's outputs on its own images (estk_act_cnn, fp32).  ``dims`` the
+        packed descriptor (``CNNSpec.dims``, or the spec itself); ``act`` the hidden | output | n_conv code
+        (ESTK_ACTIONS is added here).  Population: ``obs`` ``[2*pairs, B, c, h, w]`` -> ``out``
+        ``[2*pairs, B, out]``, rows ``< pairs`` the + members of the local pairs, the rest their mirrors.
+        ``offsets`` None = the centre: ``obs`` / ``out`` ``[1, B, ...]`` for theta."""
+        d = cnn_desc(dims, (int(act) & 0xff00ffff) | _capi.ESTK_ACTIONS)
+        (c, h, w), n_out = cnn_shapes([d.dims[i] for i in range(d.n_layers + 1)], act)
+        M = 1 if offsets is None else 2 * int(pairs)
+        B = int(obs.shape[1]) if obs.dim() == 5 else -1
+        if obs.dim() != 5 or tuple(obs.shape) != (M, B, c, h, w) or tuple(out.shape) != (M, B, n_out):
+            raise ValueError(f"obs {tuple(obs.shape)} / out {tuple(out.shape)} do not match the convolutional policy "
+                             f"for {M} members: expected [{M}, B, {c}, {h}, {w}] / [{M}, B, {n_out}]")
+        minus = None if offsets is None else C.c_void_p(out.data_ptr() + int(pairs) * B * n_out * out.element_size())
+        _capi.check(self.lib.estk_act_cnn(
+            self._ctx, C.byref(d), self._ptr(theta, torch.float32, "theta"), self._ptr(table, torch.float32, "table"),
+            self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+            float(sigma), self._ptr(obs, torch.float32, "obs"), B, self._ptr(out, torch.float32, "out"), minus,
+            self._stream()), "estk_act_cnn")
+        self.launches += 1
+
     def conv_scratch_bytes(self, ref_batch, B, precision="fp32") -> int:
         return int(self.lib.estk_eval_conv_vbn_scratch_bytes(self._ctx, self._precision(precision)[0], int(ref_batch),
                                                              int(B)))

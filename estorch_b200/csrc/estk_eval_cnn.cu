@@ -22,7 +22,13 @@
 // The two activation buffers ([2][max layer output][ROWS]) stay in shared memory when they fit the budget
 // below; otherwise they live in a per-CTA slab of the context workspace and a persistent grid loops over the
 // work items (the same code, global instead of shared addresses).  Layer 0 reads the images from `obs`.
+//
+// estk_act_cnn (include/estk_act_cnn.h) runs the same kernel with kHeadAct in HEAD: layer 0 reads each member's
+// own images, the epilogue writes the last layer's outputs instead of scoring them, and there are no partials
+// and no arrival counters.  The layer walk is shared, so a member's outputs are the bits the evaluate writes to
+// its behaviour characteristic for the same images.
 #include "estk_common.cuh"
+#include "estk_act_cnn.h"
 
 namespace {
 
@@ -32,6 +38,9 @@ constexpr int kMaxKT = 256;                  // taps per tile
 constexpr size_t kSmemBudget = 220 * 1024;   // up to the 227 KB a CTA may hold
 constexpr size_t kSmemPreferred = 110 * 1024;  // two CTAs per SM
 constexpr int64_t kSlabBudgetFloats = (int64_t)1 << 28;  // 1 GB of slab for the whole grid (at least one CTA's)
+// HEAD = kHeadAct | kHeadIdentity or kHeadTanh: the act variant (estk_act_cnn); the evaluate's HEAD values
+// (kHeadIdentity, kHeadTanh, kHeadXent) name the same kernels as before the act variant existed
+constexpr int kHeadAct = 4;
 
 struct CnnLayer {
   int cin, hin, win, cout, k, s, pad, ho, wo;
@@ -59,6 +68,11 @@ struct CnnParams {
   float* partial;            // [pairs][2][B] per-image loss values
   unsigned int* counters;    // [pairs], zero on entry, zero on exit
   float* slab;               // SLAB: [gridDim.x][2][maxact][ROWS]
+  // the act variant: obs is [2*pairs][B][c][h][w] (block j the + member of local pair j, pairs + j its mirror)
+  // or, for the centre, [B][c][h][w]; the outputs are [pairs][B][out] per sign (after every field above, so
+  // the evaluate kernels read their parameters at the same offsets)
+  float* out_plus;
+  float* out_minus;
 };
 
 // OG x KT of a layer's weight tile
@@ -70,6 +84,8 @@ __host__ __device__ inline int cnn_og(int K, int cout) {
 
 template <int HID, int HEAD, bool SLAB>
 __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
+  constexpr bool ACT = (HEAD & kHeadAct) != 0;
+  constexpr int OUT_HEAD = HEAD & ~kHeadAct;
   extern __shared__ __align__(16) float smem[];
   const int ROWS = 2 * p.BC, BC = p.BC;
   float* const Wp = smem;                          // [OG][KT]
@@ -132,8 +148,11 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
             float* const yp = Y + ((size_t)(oc0 + og) * P + pos) * ROWS + r;
             float acc = first ? 0.f : *yp;
             if (l == 0) {
-              if (b < nb) {
-                const float* const xb = p.obs + (size_t)(b0 + b) * HWin * ly.cin + (ih0 * ly.win + iw0);
+              // the act variant's centre has no - members: its - rows read nothing and are never written out
+              if (b < nb && !(ACT && centre && minus)) {
+                size_t img = b0 + b;
+                if constexpr (ACT) img += (size_t)(minus ? p.pairs + j : j) * p.B;   // the member's own images
+                const float* const xb = p.obs + img * HWin * ly.cin + (ih0 * ly.win + iw0);
 #pragma unroll 4
                 for (int t = 0; t < kt; ++t) {
                   const int kh = tkhw[t] >> 8, kw = tkhw[t] & 0xff;
@@ -154,7 +173,7 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
               const int64_t bidx = ly.wbase + (int64_t)ly.cout * ly.K + oc0 + og;
               float y = acc + estk_form_sign(p.theta, nz, sigma, bidx, minus);
               if (!last) y = estk_hidden_act<HID, true>(y);   // SiLU without the div.rn call: the same bits
-              else if (HEAD == kHeadTanh) y = tanhf(y);
+              else if (OUT_HEAD == kHeadTanh) y = tanhf(y);
               acc = y;
             }
             *yp = acc;
@@ -166,6 +185,15 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
     // ---- thread r < ROWS scores image r in column order; the outputs are in the last layer's buffer
     __syncthreads();
     const float* const Yo = ((L - 1) & 1) ? buf1 : buf0;
+    if constexpr (ACT) {   // thread r < ROWS writes image r's outputs themselves to out[j][b] of its sign
+      const int bl = tid % BC;
+      const bool minus = tid >= BC;
+      if (tid < ROWS && bl < nb && !(centre && minus)) {
+        float* const y = (minus ? p.out_minus : p.out_plus) + ((size_t)j * p.B + b0 + bl) * p.out;
+        for (int o = 0; o < p.out; ++o) y[o] = Yo[(size_t)o * ROWS + tid];
+      }
+      continue;
+    }
     const int r = tid, bl = tid % BC, b = b0 + bl;
     if (tid < ROWS && bl < nb) {
       const bool minus = r >= BC;
@@ -209,6 +237,7 @@ size_t fixed_smem() { return sizeof(float) * 2 * kTile + sizeof(int) * 2 * kMaxK
 
 template <int HID, int HEAD>
 int launch_cnn(estk_ctx* ctx, CnnParams& p, cudaStream_t stream, const char* who) {
+  constexpr bool ACT = (HEAD & kHeadAct) != 0;
   // the largest chunk of images whose activations fit in shared memory, preferring two CTAs per SM
   int bc = 0;
   size_t smem_all = 0;
@@ -228,13 +257,15 @@ int launch_cnn(estk_ctx* ctx, CnnParams& p, cudaStream_t stream, const char* who
   l.smem_shared = smem_all;
   l.smem_slab = fixed_smem();
   l.slab_per_cta = (int64_t)2 * p.maxact * 2 * bc;
-  l.members = p.pairs;
-  l.eval_floats = (int64_t)p.pairs * 2 * p.B;
+  // the act variant keeps no partials and no counters: it reserves on the slab path only
+  l.members = ACT ? 0 : p.pairs;
+  l.eval_floats = ACT ? 0 : (int64_t)p.pairs * 2 * p.B;
   // the persistent loop serves any grid, so a large image costs the memory of a few CTAs' buffers, not of
   // every resident CTA's
   l.slab_cap = kSlabBudgetFloats;
   return estk_launch_eval(ctx, eval_cnn_kernel<HID, HEAD, false>, eval_cnn_kernel<HID, HEAD, true>, p, l, kThreads,
                           stream, who, [&] {
+                            if (ACT) return;
                             p.partial = ctx->eval_partial;
                             p.counters = estk_member_counters(ctx);
                           });
@@ -244,31 +275,28 @@ template <int HID>
 int launch_hid(estk_ctx* ctx, CnnParams& p, int head, cudaStream_t stream, const char* who) {
   if (head == kHeadXent) return launch_cnn<HID, kHeadXent>(ctx, p, stream, who);
   if (head == kHeadTanh) return launch_cnn<HID, kHeadTanh>(ctx, p, stream, who);
+  if (head == (kHeadAct | kHeadTanh)) return launch_cnn<HID, kHeadAct | kHeadTanh>(ctx, p, stream, who);
+  if (head == (kHeadAct | kHeadIdentity)) return launch_cnn<HID, kHeadAct | kHeadIdentity>(ctx, p, stream, who);
   return launch_cnn<HID, kHeadIdentity>(ctx, p, stream, who);
 }
 
-}  // namespace
-
-int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
-  const char* who = "estk_eval_mlp[convolutional]";
-  if (const int rc = eval_returns_supported(call, who)) return rc;
-  const estk_mlp_desc& d = call.desc;
-  const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
-  ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
-                 n_conv, code);
-  if (estk_eval_route(low) != kRouteDense) {
-    estk_set_error("%s: ESTK_ACTIONS and the recurrent cells are not supported with a conv stack (code 0x%x)", who,
-                   code);
-    return ESTK_ERR_UNSUPPORTED;
+int launch_code(estk_ctx* ctx, CnnParams& p, int code, int head, cudaStream_t stream, const char* who) {
+  switch (code & 0xff) {
+    case ESTK_ACT_TANH: return launch_hid<ESTK_ACT_TANH>(ctx, p, head, stream, who);
+    case ESTK_ACT_ELU: return launch_hid<ESTK_ACT_ELU>(ctx, p, head, stream, who);
+    case ESTK_ACT_SILU: return launch_hid<ESTK_ACT_SILU>(ctx, p, head, stream, who);
+    case ESTK_ACT_LEAKY_RELU: return launch_hid<ESTK_ACT_LEAKY_RELU>(ctx, p, head, stream, who);
+    default: return launch_hid<ESTK_ACT_RELU>(ctx, p, head, stream, who);
   }
-  ESTK_CHECK_ARG(estk_act_valid(low), "%s: activation=0x%x: bits 0-23 are not a defined hidden | output | loss "
-                 "combination", who, code);
+}
+
+// The layers of a packed descriptor (include/estk.h, convolutional evaluate) into p.layer, p.n_layers, p.in_size,
+// p.out and p.maxact; n_conv (1..7) is bits 24-31 of d.activation, checked by the caller.  Every malformed
+// field is ESTK_ERR_INVALID.
+int cnn_parse(const estk_mlp_desc& d, int n_conv, CnnParams& p, const char* who) {
   ESTK_CHECK_ARG(d.n_layers > n_conv && d.n_layers <= ESTK_MAX_LAYERS,
                  "%s: n_layers=%d must exceed n_conv=%d (at least one Linear) and be at most %d", who, d.n_layers,
                  n_conv, ESTK_MAX_LAYERS);
-  if (const int rc = eval_returns_check(ctx, call, who)) return rc;
-
-  CnnParams p = {};
   const uint32_t in = (uint32_t)d.dims[0];
   int c = in & 1023, h = (in >> 10) & 1023, w = (in >> 20) & 1023;
   ESTK_CHECK_ARG((in >> 30) == 0 && c >= 1 && h >= 1 && w >= 1,
@@ -306,16 +334,63 @@ int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   p.n_layers = d.n_layers;
   p.out = c;
   p.maxact = (int)maxact;
+  return ESTK_OK;
+}
+
+}  // namespace
+
+int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
+  const char* who = "estk_eval_mlp[convolutional]";
+  if (const int rc = eval_returns_supported(call, who)) return rc;
+  const estk_mlp_desc& d = call.desc;
+  const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
+  ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
+                 n_conv, code);
+  if (estk_eval_route(low) != kRouteDense) {
+    estk_set_error("%s: ESTK_ACTIONS and the recurrent cells are not supported with a conv stack (code 0x%x)", who,
+                   code);
+    return ESTK_ERR_UNSUPPORTED;
+  }
+  ESTK_CHECK_ARG(estk_act_valid(low), "%s: activation=0x%x: bits 0-23 are not a defined hidden | output | loss "
+                 "combination", who, code);
+  if (const int rc = eval_returns_check(ctx, call, who)) return rc;
+
+  CnnParams p = {};
+  if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;
   p.theta = call.theta; p.table = call.table; p.offsets = call.offsets; p.order = call.order;
   p.pairs = call.pairs; p.sigma = call.sigma; p.obs = call.obs; p.target = call.target; p.B = call.B;
   p.ret_plus = call.ret_plus; p.ret_minus = call.ret_minus;
   p.bc_plus = call.bc_plus; p.bc_minus = call.bc_minus; p.bc_obs = call.bc_obs; p.bc_dim = call.bc_dim;
-  const int head = estk_head(low);
-  switch (low & 0xff) {
-    case ESTK_ACT_TANH: return launch_hid<ESTK_ACT_TANH>(ctx, p, head, stream, who);
-    case ESTK_ACT_ELU: return launch_hid<ESTK_ACT_ELU>(ctx, p, head, stream, who);
-    case ESTK_ACT_SILU: return launch_hid<ESTK_ACT_SILU>(ctx, p, head, stream, who);
-    case ESTK_ACT_LEAKY_RELU: return launch_hid<ESTK_ACT_LEAKY_RELU>(ctx, p, head, stream, who);
-    default: return launch_hid<ESTK_ACT_RELU>(ctx, p, head, stream, who);
+  return launch_code(ctx, p, low, estk_head(low), stream, who);
+}
+
+extern "C" int estk_act_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, const float* theta, const float* table,
+                            const int64_t* offsets, const int32_t* order, int32_t pairs, float sigma,
+                            const float* obs, int32_t B, float* out_plus, float* out_minus, void* stream) {
+  const char* who = "estk_act_cnn";
+  const bool centre = offsets == nullptr;
+  ESTK_CHECK_ARG(ctx && desc && theta && obs && out_plus, "%s: null context, desc, theta, obs or out_plus", who);
+  ESTK_CHECK_ARG(centre || (table && out_minus), "%s: a population needs table and out_minus", who);
+  ESTK_CHECK_ARG(B >= 1, "%s: B=%d must be positive", who, B);
+  ESTK_CHECK_ARG(centre || (pairs >= 1 && pairs <= ESTK_MAX_POPULATION / 2), "%s: pairs=%d is outside 1..%d", who,
+                 pairs, ESTK_MAX_POPULATION / 2);
+  const estk_mlp_desc& d = *desc;
+  const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff, hid = low & 0xff;
+  ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
+                 n_conv, code);
+  ESTK_CHECK_ARG((low & ~0xff) == ESTK_ACTIONS || (low & ~0xff) == (ESTK_ACTIONS | ESTK_ACT_OUT_TANH),
+                 "%s: activation=0x%x: bits 8-23 must be ESTK_ACTIONS, optionally with ESTK_ACT_OUT_TANH", who, code);
+  ESTK_CHECK_ARG(hid == ESTK_ACT_RELU || hid == ESTK_ACT_TANH || hid == ESTK_ACT_ELU || hid == ESTK_ACT_SILU ||
+                 hid == ESTK_ACT_LEAKY_RELU, "%s: activation=0x%x: bits 0-7 are not a hidden kind", who, code);
+
+  CnnParams p = {};
+  if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;
+  p.theta = theta; p.obs = obs; p.B = B; p.out_plus = out_plus;
+  if (centre) {
+    p.pairs = 1;
+  } else {
+    p.table = table; p.offsets = offsets; p.order = order; p.pairs = pairs; p.sigma = sigma; p.out_minus = out_minus;
   }
+  const int head = kHeadAct | ((low & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity);
+  return launch_code(ctx, p, low, head, (cudaStream_t)stream, who);
 }

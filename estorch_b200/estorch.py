@@ -301,6 +301,11 @@ class ES:
 
         self.agent = agent(**agent_kwargs)
         self._device_agent = isinstance(self.agent, DeviceAgent)
+        obs_shape = getattr(self.agent, "obs_shape", None) if isinstance(self.agent, PopulationAgent) else None
+        if obs_shape is not None and not (isinstance(obs_shape, (tuple, list)) and len(obs_shape) == 3 and all(
+                isinstance(d, int) and not isinstance(d, bool) and d > 0 for d in obs_shape)):
+            raise ValueError(f"PopulationAgent.obs_shape must be None or (c, h, w), three positive ints; got "
+                             f"{obs_shape!r}")
         # a device agent with batch_size: every generation evaluates a fresh minibatch of its dataset
         self._sampling = self._device_agent and self.agent.batch_size is not None
         if self._sampling and type(self.agent).next_batch is not DeviceAgent.next_batch:
@@ -318,6 +323,9 @@ class ES:
         if self._spec is None and type(self.agent) is not SequenceAgent and isinstance(self.agent, DeviceAgent) \
                 and self.agent.obs.dim() == 4:
             self._spec = cnn_spec_from_module(self.target, tuple(self.agent.obs.shape[1:]))
+        # ... and for a population agent, the shape of one observation it declares
+        if self._spec is None and obs_shape is not None:
+            self._spec = cnn_spec_from_module(self.target, tuple(obs_shape))
         self._is_conv = isinstance(self._spec, ConvVBNSpec)
         self._is_rnn = isinstance(self._spec, RNNSpec)
         self._is_cnn = isinstance(self._spec, CNNSpec)
@@ -428,9 +436,10 @@ class ES:
     def _decide_fused(self, optimizer_cls):
         """Fused mode for a DeviceAgent (an MLP, conv + VirtualBatchNorm or generic Conv2d + Linear policy) or a
         SequenceAgent (a recurrent policy), population mode for a PopulationAgent (a recognised MLP, conv +
-        VirtualBatchNorm or recurrent policy on one GPU: the multi-GPU population generation is not
-        implemented, hooks mode serves it).  A generic CNN with a PopulationAgent stays in hooks mode: it is
-        recognised for a DeviceAgent's images only (there is no population-mode CNN kernel)."""
+        VirtualBatchNorm, recurrent or generic Conv2d + Linear policy on one GPU: the multi-GPU population
+        generation is not implemented, hooks mode serves it).  A generic CNN is recognised for a DeviceAgent's
+        images, and for a PopulationAgent that declares ``obs_shape``; a SequenceAgent with a CNN stays in hooks
+        mode."""
         population = isinstance(self.agent, PopulationAgent)
         if not (self._device_agent or population) or self._spec is None:
             return False
@@ -439,7 +448,7 @@ class ES:
         # a recurrent policy is evaluated over sequences, other policies over a batch of observations
         if not population and self._is_rnn != isinstance(self.agent, SequenceAgent):
             return False
-        if self._is_cnn and (population or isinstance(self.agent, SequenceAgent)):
+        if self._is_cnn and isinstance(self.agent, SequenceAgent):
             return False
         if optimizer_cls is not torch.optim.Adam:
             return False
@@ -1104,6 +1113,8 @@ class ES:
             return self._population_act_conv(slot, centre)
         if self._is_rnn:
             return self._population_act_rnn(slot, centre)
+        if self._is_cnn:
+            return self._population_act_cnn(slot, centre)
         be, dims, dev, code = self._be, self._spec.dims, self._dev, self._spec.act
         M = 1 if centre else self.population_size
         t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
@@ -1165,6 +1176,29 @@ class ES:
                 out = out[:, 0]
             y, h = out[..., :dout], out[..., dout:dout + H]
             return y, ((h, out[..., dout + H:]) if lstm else h)
+        return act
+
+    def _population_act_cnn(self, slot, centre):
+        """``act`` for a Conv2d stack + Linear head policy (CNNSpec): images ``[M, c, h, w]`` or
+        ``[M, B, c, h, w]`` -> outputs ``[M, out]`` or ``[M, B, out]``, one estk_act_cnn launch per call."""
+        be, dev, spec = self._be, self._dev, self._spec
+        M = 1 if centre else self.population_size
+        shape = tuple(spec.input_shape)
+
+        def act(obs):
+            x = torch.as_tensor(obs).to(device=dev, dtype=torch.float32).contiguous()
+            single = x.dim() == 4
+            x5 = x.unsqueeze(1) if single else x
+            if x5.dim() != 5 or x5.shape[0] != M or tuple(x5.shape[2:]) != shape:
+                dims = ", ".join(map(str, shape))
+                raise ValueError(f"act: images {tuple(x.shape)}, expected [{M}, {dims}] or [{M}, B, {dims}]")
+            out = torch.empty(M, x5.shape[1], spec.out, dtype=torch.float32, device=dev)
+            if centre:
+                be.act_cnn(spec.dims, slot.theta, None, None, None, 1, 0.0, x5, out, spec.act)
+            else:
+                be.act_cnn(spec.dims, slot.theta_prev, self._table, self._offsets, self._order, self._pairs_local,
+                           self.sigma, x5, out, spec.act)
+            return out[:, 0] if single else out
         return act
 
     def _population_act_conv(self, slot, centre):
