@@ -29,6 +29,8 @@ ESTK_CELL_LSTM = 9
 ESTK_ACT_OUT_TANH = 1 << 8
 ESTK_LOSS_XENT = 1 << 16
 ESTK_ACTIONS = 3 << 16
+# the return is the fraction of rows whose logits' first argmax is the target's first argmax (fp32)
+ESTK_LOSS_ACCURACY = 6 << 16
 # bits 24-31: n_conv, the number of leading Conv2d layers of a convolutional policy (the CNN evaluate, fp32);
 # its dims[0] is ESTK_CNN_INPUT(c, h, w) and dims[1..n_conv] ESTK_CNN_CONV(out_c, k, stride, pad)
 ESTK_CNN_SHIFT = 24

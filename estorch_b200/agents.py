@@ -8,7 +8,8 @@ an agent that *declares* its computation:
 ``DeviceAgent`` -- rollout is "run the policy over a fixed observation batch
 and reduce": ``return = -mean((policy(obs) - target)**2)`` (``loss="mse"``) or the
 soft-target cross-entropy ``return = mean_b sum_c target_bc * log_softmax(policy(obs))_bc``
-(``loss="cross_entropy"``: the policy's output is the logits) and (NS family)
+(``loss="cross_entropy"``: the policy's output is the logits), or the classification accuracy
+``return = mean_b [argmax policy(obs)_b == argmax target_b]`` (``loss="accuracy"``) and (NS family)
 ``bc = policy(obs[:bc_obs]).flatten()[:bc_dim]`` (the 256-float behaviour
 characteristic shape of examples/nsra_es.py:45-49).  It still implements the
 reference protocol (``rollout``) with plain torch, so the very same object
@@ -32,7 +33,9 @@ import torch
 from .batches import batch_indices
 
 
-LOSSES = ("mse", "cross_entropy")
+LOSSES = ("mse", "cross_entropy", "accuracy")
+# the accuracy counts correct rows in fp32: exact for batches below 2^24 rows
+ACCURACY_MAX_BATCH = (1 << 24) - 1
 
 
 class DeviceAgent:
@@ -42,6 +45,11 @@ class DeviceAgent:
     ``loss="cross_entropy"``: ``target`` is ``[B, C]`` class weights per observation (one-hot or
     soft labels, finite and >= 0) and the return is minus the mean over the batch of the
     cross-entropy between those weights and the softmax of the policy's output.
+    ``loss="accuracy"``: ``target`` as for the cross-entropy; the return is the fraction of the batch whose
+    prediction (the first index of the maximum of the policy's output, ``torch.argmax``'s rule: a NaN counts
+    as the maximum) is the label (the first index of the maximum of the target row): count / B in fp32,
+    bit for bit.  The batch (``batch_size``, else N) must be below 2^24 rows.  Not available for
+    ``SequenceAgent``.
 
     ``batch_size=B``: ``obs`` / ``target`` are a whole dataset of N rows (``dataset_obs`` / ``dataset_target``)
     and every generation is scored on a minibatch of B of them, the same minibatch for every member.
@@ -65,11 +73,14 @@ class DeviceAgent:
             raise ValueError(f"loss must be one of {LOSSES}, got {loss!r}")
         if batch_size is not None:      # before the dataset is copied
             _check_batches(obs.shape[0], batch_size, bc_obs, bc_dim)
+        if loss == "accuracy" and (batch_size if batch_size is not None else obs.shape[0]) > ACCURACY_MAX_BATCH:
+            raise ValueError("loss='accuracy' counts correct rows exactly in fp32 only for batches below 2^24 rows")
         self.obs = obs.detach().to(torch.float32).contiguous()
         self.target = target.detach().to(torch.float32).contiguous()
-        if loss == "cross_entropy" and not (target.is_floating_point() and bool(torch.isfinite(self.target).all())
-                                            and bool((self.target >= 0).all())):
-            raise ValueError("loss='cross_entropy' needs target class weights that are finite and >= 0")
+        if loss in ("cross_entropy", "accuracy") and not (
+                target.is_floating_point() and bool(torch.isfinite(self.target).all())
+                and bool((self.target >= 0).all())):
+            raise ValueError(f"loss={loss!r} needs target class weights that are finite and >= 0")
         self.loss = loss
         self.bc_obs = int(bc_obs)
         self.bc_dim = int(bc_dim)
@@ -100,6 +111,9 @@ class DeviceAgent:
             tgt = self.target.to(p.device)
             if self.loss == "cross_entropy":
                 reward = float((tgt * torch.log_softmax(out, 1)).sum(1).mean())
+            elif self.loss == "accuracy":
+                # the mean on the CPU: an exact count and one IEEE divide (a CUDA mean multiplies by 1 / B)
+                reward = float((out.argmax(1) == tgt.argmax(1)).float().cpu().mean())
             else:
                 reward = float(-((out - tgt) ** 2).mean())
             if self.bc_dim:
@@ -143,6 +157,8 @@ class SequenceAgent(DeviceAgent):
 
     def __init__(self, obs: torch.Tensor, target: torch.Tensor, bc_obs: int = 0, bc_dim: int = 0, *,
                  loss: str = "mse", batch_size: Optional[int] = None, batch_seed: int = 0):
+        if loss == "accuracy":
+            raise ValueError("loss='accuracy' is not available for SequenceAgent: use 'mse' or 'cross_entropy'")
         if obs.dim() != 3 or target.dim() != 3 or tuple(obs.shape[:2]) != tuple(target.shape[:2]) or \
                 obs.shape[1] < 1:
             raise ValueError("obs must be [B, T, in] and target [B, T, out] with the same B and T >= 1")

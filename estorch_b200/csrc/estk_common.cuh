@@ -35,16 +35,22 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
-// estk_mlp_desc.activation: the thirty-five defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
+// estk_mlp_desc.activation: the forty defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
 // LeakyReLU and each recurrent cell GRU / LSTM x output identity / Tanh with the squared error, x identity
-// output with the cross-entropy, and x output identity / Tanh with ESTK_ACTIONS)
+// output with the cross-entropy, and x output identity / Tanh with ESTK_ACTIONS; each hidden kind, not a
+// cell, x identity output with the accuracy)
 static inline bool estk_act_valid(int a) {
   const int h = a & 0xff, rest = a & ~0xff;
   const bool actions = rest == ESTK_ACTIONS || rest == (ESTK_ACT_OUT_TANH | ESTK_ACTIONS);
+  const bool cell = h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM;
   const bool known = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
-                     h == ESTK_ACT_LEAKY_RELU || h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM;
-  return known && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions);
+                     h == ESTK_ACT_LEAKY_RELU || cell;
+  return known && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions ||
+                   (rest == ESTK_LOSS_ACCURACY && !cell));
 }
+// the loss field is ESTK_LOSS_ACCURACY: the count of correct rows needs B < 2^24 to stay exact in fp32
+static inline bool estk_loss_accuracy(int code) { return (code & 0xff0000) == ESTK_LOSS_ACCURACY; }
+static const int kAccuracyMaxB = (1 << 24) - 1;
 // The estk_eval_mlp back end of an activation code: n_conv != 0 in bits 24-31 the convolutional evaluate;
 // a defined code whose loss field is ESTK_ACTIONS (no return, the outputs themselves) one step of the MLP or
 // of the recurrent cell in bits 0-7; a defined recurrent cell code with a return the sequence evaluate;
@@ -59,9 +65,10 @@ static inline EvalRoute estk_eval_route(int a) {
 }
 // The output head of a code with a return, a compile-time parameter of the sequence and convolutional
 // evaluates: identity, tanhf, or the logits of the cross-entropy (which takes precedence over the Tanh bit)
-constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2;
+constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2, kHeadAccuracy = 3;
 static inline int estk_head(int code) {
-  return (code & ESTK_LOSS_XENT) ? kHeadXent : (code & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
+  return estk_loss_accuracy(code) ? kHeadAccuracy : (code & ESTK_LOSS_XENT) ? kHeadXent
+       : (code & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
 }
 // Rows per sign in one work item of the fp32 act kernels (an environment population): B itself up to 2, then
 // 4, then 8 -- one instantiation per value.
@@ -358,6 +365,35 @@ __device__ __forceinline__ bool estk_pair_arrive(unsigned int* counter, int item
     if (ret_minus) (ret_minus)[j] = -(sm_ / d_);                                                            \
     *(counter) = 0u;                                                                                        \
   } while (0)
+// The order of torch.argmax on (value, index) pairs: a NaN is above every number (the lower index wins between
+// two NaNs) and the lower index wins a tie.  It is a total order, so folding the pairs of a row in any order
+// and any grouping, from (-INFINITY, INT_MAX), leaves the first index of the maximum (ESTK_LOSS_ACCURACY).
+__device__ __forceinline__ void estk_argmax_fold(float& m, int& i, float v, int k) {
+  const bool better = v != v ? (m == m || k < i) : (m == m && (v > m || (v == m && k < i)));
+  if (better) { m = v; i = k; }
+}
+// The fold across the four lanes of a quad (lane distance 1, then 2): every lane ends with the quad's result.
+// All 32 lanes of the warp take part.
+__device__ __forceinline__ void estk_argmax_quad(float& m, int& i) {
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+    estk_argmax_fold(m, i, om, oi);
+  }
+}
+// The label of a target row t[0..C) for the four lanes of a quad (q = lane & 3): lane q folds its quarter of the
+// columns, four loads in flight; every lane returns the first index of the row's maximum.  C = 0 reads nothing
+// (a row past the batch).
+__device__ __forceinline__ int estk_quad_label(const float* t, int C, int q) {
+  const int qs = (C + 3) / 4, c1 = min(C, (q + 1) * qs);
+  float m = -INFINITY;
+  int i = INT_MAX;
+#pragma unroll 4
+  for (int c = q * qs; c < c1; ++c) estk_argmax_fold(m, i, __ldg(t + c), c);
+  estk_argmax_quad(m, i);
+  return i;
+}
 __device__ __forceinline__ int warp_sum_i(int v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

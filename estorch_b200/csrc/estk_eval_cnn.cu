@@ -39,7 +39,8 @@ constexpr size_t kSmemBudget = 220 * 1024;   // up to the 227 KB a CTA may hold
 constexpr size_t kSmemPreferred = 110 * 1024;  // two CTAs per SM
 constexpr int64_t kSlabBudgetFloats = (int64_t)1 << 28;  // 1 GB of slab for the whole grid (at least one CTA's)
 // HEAD = kHeadAct | kHeadIdentity or kHeadTanh: the act variant (estk_act_cnn); the evaluate's HEAD values
-// (kHeadIdentity, kHeadTanh, kHeadXent) name the same kernels as before the act variant existed
+// (kHeadIdentity, kHeadTanh, kHeadXent) name the same kernels as before the act variant existed; kHeadAccuracy
+// is the evaluate only
 constexpr int kHeadAct = 4;
 
 struct CnnLayer {
@@ -210,6 +211,14 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
           sty = fmaf(tv, y, sty);
         }
         s = fmaf(m + logf(se), st, -sty);
+      } else if constexpr (HEAD == kHeadAccuracy) {   // 1 where the first argmaxes of logits and target agree
+        float ym = -INFINITY, tm = -INFINITY;
+        int yi = INT_MAX, ti = INT_MAX;
+        for (int o = 0; o < p.out; ++o) {
+          estk_argmax_fold(ym, yi, Yo[(size_t)o * ROWS + r], o);
+          estk_argmax_fold(tm, ti, __ldg(tg + o), o);
+        }
+        s = yi == ti ? 1.f : 0.f;
       } else {
         for (int o = 0; o < p.out; ++o) {
           const float d = Yo[(size_t)o * ROWS + r] - __ldg(tg + o);
@@ -228,8 +237,9 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
     __syncthreads();
     if (tid == 0 && estk_pair_arrive(p.counters + slot, p.chunks))
       ESTK_PAIR_FINISH(p.partial + (size_t)slot * 2 * p.B, p.B,
-                       (float)((int64_t)p.B * (HEAD == kHeadXent ? 1 : p.out)), p.ret_plus, p.ret_minus, j,
-                       p.counters + slot);
+                       HEAD == kHeadAccuracy ? -(float)p.B
+                                             : (float)((int64_t)p.B * (HEAD == kHeadXent ? 1 : p.out)),
+                       p.ret_plus, p.ret_minus, j, p.counters + slot);
   }
 }
 
@@ -274,6 +284,7 @@ int launch_cnn(estk_ctx* ctx, CnnParams& p, cudaStream_t stream, const char* who
 template <int HID>
 int launch_hid(estk_ctx* ctx, CnnParams& p, int head, cudaStream_t stream, const char* who) {
   if (head == kHeadXent) return launch_cnn<HID, kHeadXent>(ctx, p, stream, who);
+  if (head == kHeadAccuracy) return launch_cnn<HID, kHeadAccuracy>(ctx, p, stream, who);
   if (head == kHeadTanh) return launch_cnn<HID, kHeadTanh>(ctx, p, stream, who);
   if (head == (kHeadAct | kHeadTanh)) return launch_cnn<HID, kHeadAct | kHeadTanh>(ctx, p, stream, who);
   if (head == (kHeadAct | kHeadIdentity)) return launch_cnn<HID, kHeadAct | kHeadIdentity>(ctx, p, stream, who);
@@ -354,6 +365,8 @@ int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
   ESTK_CHECK_ARG(estk_act_valid(low), "%s: activation=0x%x: bits 0-23 are not a defined hidden | output | loss "
                  "combination", who, code);
   if (const int rc = eval_returns_check(ctx, call, who)) return rc;
+  ESTK_CHECK_ARG(!estk_loss_accuracy(low) || call.B <= kAccuracyMaxB,
+                 "%s: B=%d: the accuracy's count is exact in fp32 for B < 2^24 only", who, call.B);
 
   CnnParams p = {};
   if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;

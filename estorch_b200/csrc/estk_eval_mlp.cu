@@ -7,7 +7,8 @@
 //   Policy.forward           examples/cartpole_es.py:14-20 (Linear-ReLU-Linear-ReLU-Linear; or Tanh
 //                            hidden and / or output activations, estk.h ESTK_ACT_*)
 //   Agent.rollout            synthetic agent of SURVEY 8d: -mean((policy(obs)-y)^2), or the
-//                            soft-target cross-entropy (ESTK_LOSS_XENT)
+//                            soft-target cross-entropy (ESTK_LOSS_XENT), or the accuracy
+//                            (ESTK_LOSS_ACCURACY)
 //                            (+ behaviour characteristic, examples/nsra_es.py:45-49)
 //
 // One CTA = one antithetic pair x one chunk of BC observations.  The pair's
@@ -18,7 +19,8 @@
 // layers (k-major [width][ROWS], ROWS = 2*BC rows = sign-major), register tile
 // 4 rows x 4 outputs per thread.  The last layer is fused with the squared
 // error; with the cross-entropy it writes the logits to shared memory like a hidden
-// layer, and one thread per row then reduces its row in column order.  Chunk partial sums are combined in fixed order by the last-arriving
+// layer, and one thread per row then reduces its row in column order (the accuracy likewise: the
+// first argmax of the logits and of the target row, 1 per row where they agree).  Chunk partial sums are combined in fixed order by the last-arriving
 // chunk CTA (deterministic, no float atomics).
 //
 // This is the exact-fp32 path used for parity and for small policies; algorithmic
@@ -58,6 +60,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
   constexpr int HID = ACT & 0xff;
   constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
+  constexpr bool ACC = (ACT & 0xff0000) == ESTK_LOSS_ACCURACY;
   constexpr int OT = 4096 / ROWS;  // output features per tile
   constexpr int OTP = OT + 4;      // padded row of the weight tile (keeps float4 alignment)
   constexpr int TC = OT / 4;       // thread columns
@@ -154,7 +157,7 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
 #pragma unroll
           for (int i = 0; i < 4; ++i) y[i] = estk_hidden_act<HID>(y[i]);
           *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
-        } else if constexpr (XENT) {
+        } else if constexpr (XENT || ACC) {
           // the logits stay in shared memory for the row pass below
           *reinterpret_cast<float4*>(Y + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
           float* bc = minus ? p.bc_minus : p.bc_plus;
@@ -208,10 +211,26 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
       loss = fmaf(m + logf(s), st, -sty);
     }
   }
+  // ---- accuracy: thread r < ROWS compares the first argmax of row r of the logits with its target's
+  if constexpr (ACC) {
+    __syncthreads();
+    const int C = p.desc.dims[L];
+    const int b = b0 + (tid % BC);
+    if (tid < ROWS && b < p.B) {
+      const float* t = p.target + (size_t)b * C;
+      float ym = -INFINITY, tm = -INFINITY;
+      int yi = INT_MAX, ti = INT_MAX;
+      for (int c = 0; c < C; ++c) {
+        estk_argmax_fold(ym, yi, X[(size_t)c * ROWS + tid], c);
+        estk_argmax_fold(tm, ti, __ldg(t + c), c);
+      }
+      loss = yi == ti ? 1.f : 0.f;
+    }
+  }
 
   // ---- block reduction of the loss, per sign
   {
-    const bool lminus = XENT ? tid >= BC : minus;   // cross-entropy: the sign of row tid
+    const bool lminus = (XENT || ACC) ? tid >= BC : minus;   // cross-entropy, accuracy: the sign of row tid
     const float lp = warp_sum_f(lminus ? 0.f : loss);
     const float lm = warp_sum_f(lminus ? loss : 0.f);
     if ((tid & 31) == 0) { s_red[0][tid >> 5] = lp; s_red[1][tid >> 5] = lm; }
@@ -228,8 +247,8 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
     __syncthreads();
     if (s_last && tid == 0)
       ESTK_PAIR_FINISH(p.partial + ((size_t)slot * 2) * p.chunks, p.chunks,
-                       XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus, p.ret_minus, j,
-                       p.counters + slot);
+                       ACC ? -(float)p.B : XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus,
+                       p.ret_minus, j, p.counters + slot);
   }
 }
 
@@ -263,6 +282,11 @@ int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
     case ESTK_ACT_LEAKY_RELU: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU>(p, smem, stream);
     case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, smem, stream);
     case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, smem, stream);
+    case ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_LOSS_ACCURACY>(p, smem, stream);
+    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>(p, smem, stream);
+    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>(p, smem, stream);
+    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>(p, smem, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>(p, smem, stream);
     default: return launch_act<ROWS, ESTK_ACT_RELU>(p, smem, stream);
   }
 }
@@ -302,6 +326,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
   constexpr int HID = ACT & 0xff;
   constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
+  constexpr bool ACC = (ACT & 0xff0000) == ESTK_LOSS_ACCURACY;
   constexpr int ROWS = kWideRows, BC = kWideBC, OT = kWideOT, OTP = kWideOTP, KT = kWideKT;
   extern __shared__ __align__(16) float smem[];
   float* const Xs = smem;                     // [2][KT][ROWS]; layer 0 fills the first BC rows only
@@ -413,7 +438,7 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
 #pragma unroll
             for (int i = 0; i < 4; ++i) y[i] = estk_hidden_act<HID>(y[i]);
             *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
-          } else if constexpr (XENT) {
+          } else if constexpr (XENT || ACC) {
             *reinterpret_cast<float4*>(yout + (size_t)o * ROWS + r0) = make_float4(y[0], y[1], y[2], y[3]);
             float* bc = minus ? p.bc_minus : p.bc_plus;
 #pragma unroll
@@ -464,9 +489,26 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
         loss = fmaf(m + logf(s), st, -sty);
       }
     }
+    // ---- accuracy: thread r < ROWS compares the first argmax of row r of the logits with its target's
+    if constexpr (ACC) {
+      __syncthreads();
+      const float* Y = ((L - 1) & 1) ? act1 : act0;
+      const int C = p.desc.dims[L];
+      const int b = b0 + (tid % BC);
+      if (tid < ROWS && b < p.B) {
+        const float* t = p.target + (size_t)b * C;
+        float ym = -INFINITY, tm = -INFINITY;
+        int yi = INT_MAX, ti = INT_MAX;
+        for (int c = 0; c < C; ++c) {
+          estk_argmax_fold(ym, yi, __ldcg(Y + (size_t)c * ROWS + tid), c);
+          estk_argmax_fold(tm, ti, __ldg(t + c), c);
+        }
+        loss = yi == ti ? 1.f : 0.f;
+      }
+    }
 
     // ---- block reduction of the loss per sign, chunk partials combined in chunk order by the last arrival
-    const bool lminus = XENT ? tid >= BC : minus;
+    const bool lminus = (XENT || ACC) ? tid >= BC : minus;
     const float lp = warp_sum_f(lminus ? 0.f : loss);
     const float lm = warp_sum_f(lminus ? loss : 0.f);
     if ((tid & 31) == 0) { s_red[0][tid >> 5] = lp; s_red[1][tid >> 5] = lm; }
@@ -479,8 +521,8 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
       part[p.chunks + chunk] = sm;
       __threadfence();
       if (estk_pair_arrive(p.counters + slot, p.chunks))
-        ESTK_PAIR_FINISH(part, p.chunks, XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus,
-                         p.ret_minus, j, p.counters + slot);
+        ESTK_PAIR_FINISH(part, p.chunks, ACC ? -(float)p.B : XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L],
+                         p.ret_plus, p.ret_minus, j, p.counters + slot);
     }
   }
 }
@@ -503,15 +545,21 @@ WideKernel wide_kernel(int act) {
     case ESTK_ACT_LEAKY_RELU: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU>;
     case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
     case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
+    case ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>;
     default: return eval_mlp_wide_kernel<ESTK_ACT_RELU>;
   }
 }
 
 // The streamed kernel for a checked call: a persistent grid of at most (resident CTAs per SM) x SMs,
-// each with its slab of 2 x (widest hidden layer, or the logits of the cross-entropy) x kWideRows floats.
+// each with its slab of 2 x (widest hidden layer, or the logits of the cross-entropy or the accuracy) x
+// kWideRows floats.
 int run_wide(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who) {
   const estk_mlp_desc& d = p.desc;
-  int slab_w = (d.activation & ESTK_LOSS_XENT) ? d.dims[d.n_layers] : 0;
+  int slab_w = ((d.activation & ESTK_LOSS_XENT) || estk_loss_accuracy(d.activation)) ? d.dims[d.n_layers] : 0;
   for (int l = 1; l < d.n_layers; ++l) slab_w = max(slab_w, d.dims[l]);
   p.BC = kWideBC;
   p.chunks = (p.B + kWideBC - 1) / kWideBC;
@@ -612,6 +660,8 @@ extern "C" int estk_eval_mlp(estk_ctx* ctx, const estk_mlp_desc* desc, int32_t p
                  "estk_eval_mlp: bc_plus/bc_minus must both be set or both null");
   ESTK_CHECK_ARG(!bc_plus || (bc_obs > 0 && bc_dim > 0), "estk_eval_mlp: bc_obs/bc_dim must be positive with bc outputs");
   ESTK_CHECK_ARG(!centre_return_out || !centre, "estk_eval_mlp: centre_return_out needs a population (offsets)");
+  ESTK_CHECK_ARG(!estk_loss_accuracy(desc->activation) || B <= kAccuracyMaxB,
+                 "estk_eval_mlp: B=%d: the accuracy's count is exact in fp32 for B < 2^24 only", B);
   ESTK_CHECK_ARG(!tc || (ESTK_ALIGNED16(theta) && ESTK_ALIGNED16(obs) && ESTK_ALIGNED16(target) &&
                          (!shadows || ESTK_ALIGNED16(theta16)) &&
                          (centre || (ESTK_ALIGNED16(table) && (!t16 || ESTK_ALIGNED16(table16))))),

@@ -23,7 +23,9 @@
 //      the squared-error reduction and the behaviour characterisation; with the cross-entropy
 //      (ESTK_LOSS_XENT) each thread carries an online softmax of its two rows over its columns
 //      (running max, rescaled sum of exponentials, sum t*y, sum t) from tile to tile, and the
-//      warpgroup that drains the last tile combines the four lanes of each quad.
+//      warpgroup that drains the last tile combines the four lanes of each quad; with the accuracy
+//      (ESTK_LOSS_ACCURACY) the chain is the (max, first index) of the row's logits, carried the same
+//      way, and the quad's merge leaves 1 per row where it is the first index of the target row's max.
 // Operand modes (template MODE):
 //   kModeBF16   bf16 operands formed from fp32 theta + fp32 table (one FMA in fp32, one rounding)
 //   kModeBF16S  bf16 operands formed from bf16 shadows of theta and table (fma.rn.bf16x2)
@@ -154,6 +156,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   constexpr int HID = ACT & 0xff;
   constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
+  constexpr bool ACC = (ACT & 0xff0000) == ESTK_LOSS_ACCURACY;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sH = smem;                                  // 2 activation buffers x 8 k-blocks x 8 KB
@@ -163,7 +166,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   uint64_t* bar_empty = bar_full + kStages;                             // [kStages] stage consumed
   float* s_loss = reinterpret_cast<float*>(bar_empty + kStages);        // [4]
   float* s_chain = s_loss + 4;                                          // [128] loss chain handoff
-                                                                        // ([8][128] with the cross-entropy)
+                                                                        // ([8][128] with the cross-entropy
+                                                                        // or the accuracy)
   __shared__ Layer lay[ESTK_MAX_LAYERS];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -398,6 +402,62 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
               if ((lane & 3) == 0)
                 loss = fmaf(tm[0] + logf(ts[0]), tst[0], -tsty[0]) + fmaf(tm[1] + logf(ts[1]), tst[1], -tsty[1]);
             }
+          } else if (ACC && last) {
+            // Accuracy.  Per thread and row h (r0 + 8h): the (max, first index) of the logits over the
+            // thread's columns, in the fold of estk_argmax_fold (a total order, so the tiles, the handoff and
+            // the quad merge may combine them in any grouping); the target's label is read at the last tile.
+            float am[2] = {-INFINITY, -INFINITY};
+            int ai[2] = {INT_MAX, INT_MAX}, label[2] = {0, 0};
+#pragma unroll
+            for (int jb = 0; jb < kTileN / 8; ++jb) {
+              if (jb * 8 < width) {
+                const int col = n0 + jb * 8 + cq;
+                const float2 bv = *reinterpret_cast<const float2*>(bias + col);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int b = chunk * kRows + r0 + 8 * h;
+                  const float y0 = d[jb * 4 + 2 * h] + bv.x, y1 = d[jb * 4 + 2 * h + 1] + bv.y;
+                  estk_argmax_fold(am[h], ai[h], y0, col);
+                  estk_argmax_fold(am[h], ai[h], y1, col + 1);
+                  if (with_bc && b < p.bc_obs) {
+                    float* bc = sgn ? p.bc_minus : p.bc_plus;
+                    const int64_t idx = (int64_t)b * N + col;
+                    if (idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y0;
+                    if (idx + 1 < p.bc_dim) bc[(size_t)j * p.bc_dim + idx + 1] = y1;
+                  }
+                }
+              }
+            }
+            if (last_tile) {                 // the rows' labels, before the wait on the chain, which they overlap
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                label[h] = estk_quad_label(p.target + (size_t)(chunk * kRows + r0 + 8 * h) * N, N, lane & 3);
+            }
+            // the chain continues from the previous tile, which the other warpgroup drained; thread tid of
+            // both warpgroups holds the same rows and columns
+            if (n0 > 0) {
+              ESTK_PROF(kPrDrain);
+              named_bar_sync(kBarLoss + cw, kConsThreads);
+              ESTK_PROF(kPrOther);
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                estk_argmax_fold(am[h], ai[h], s_chain[(2 * h) * 128 + tid], __float_as_int(s_chain[(2 * h + 1) * 128 + tid]));
+            }
+            if (!last_tile) {                // hand the chain to the warpgroup of the next tile
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                s_chain[(2 * h) * 128 + tid] = am[h];
+                s_chain[(2 * h + 1) * 128 + tid] = __int_as_float(ai[h]);
+              }
+              named_bar_arrive(kBarLoss + (cw ^ 1), kConsThreads);
+            } else {
+              // the row's four lanes (the quad) hold disjoint columns: merge them, then 1 per correct row
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                estk_argmax_quad(am[h], ai[h]);
+                if ((lane & 3) == 0 && ai[h] == label[h]) loss += 1.f;
+              }
+            }
           } else if (last) {
             // the targets of kTgtBatch column blocks are loaded before any is used: the behaviour-
             // characterisation stores would otherwise hold each load until the one before returned
@@ -489,7 +549,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           __threadfence();
           float s = 0.f;
           for (int c = 0; c < parts; ++c) s += __ldcg(part + c);
-          const float r = XENT ? -(s / (float)p.B) : -(s / ((float)p.B * (float)lay[L - 1].N));
+          const float r = ACC ? s / (float)p.B : XENT ? -(s / (float)p.B) : -(s / ((float)p.B * (float)lay[L - 1].N));
           if (folded) p.centre_out[0] = r;
           else if (sgn) p.ret_minus[j] = r;
           else p.ret_plus[j] = r;
@@ -642,7 +702,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
   cluster_sync();
 }
 
-// the cross-entropy's loss chain carries 8 floats per consumer thread instead of 1
+// the loss chain carries 8 floats per consumer thread with the cross-entropy (4 with the accuracy, which takes
+// the same space) instead of 1
 size_t tc_smem_bytes(bool xent) {
   return 1024 + 2 * (size_t)kHBytes + (size_t)kStages * kStageBytes + 2 * kMaxW * sizeof(float) +
          2 * kStages * sizeof(uint64_t) + (4 + (xent ? 8 : 1) * 128) * sizeof(float);
@@ -653,7 +714,7 @@ size_t tc_smem_bytes(bool xent) {
 // kCluster, so it can be less than sm_count / kCluster.
 template <int MODE, int ACT>
 int launch_tc(const EvalTCParams& p, cudaStream_t stream) {
-  const size_t smem = tc_smem_bytes((ACT & ESTK_LOSS_XENT) != 0);
+  const size_t smem = tc_smem_bytes((ACT & ESTK_LOSS_XENT) != 0 || (ACT & 0xff0000) == ESTK_LOSS_ACCURACY);
   ESTK_CUDA(cudaFuncSetAttribute(eval_mlp_tc_kernel<MODE, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -711,6 +772,11 @@ int launch_tc_act(const EvalTCParams& p, cudaStream_t stream) {
     case ESTK_ACT_LEAKY_RELU: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU>(p, stream);
     case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, stream);
     case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, stream);
+    case ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_LOSS_ACCURACY>(p, stream);
+    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>(p, stream);
+    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>(p, stream);
+    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>(p, stream);
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>(p, stream);
     default: return launch_tc<MODE, ESTK_ACT_RELU>(p, stream);
   }
 }

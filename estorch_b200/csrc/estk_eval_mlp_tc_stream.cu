@@ -112,6 +112,7 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
   constexpr int HID = ACT & 0xff;
   constexpr bool OUT_TANH = (ACT & ESTK_ACT_OUT_TANH) != 0;
   constexpr bool XENT = (ACT & ESTK_LOSS_XENT) != 0;
+  constexpr bool ACC = (ACT & 0xff0000) == ESTK_LOSS_ACCURACY;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* sBias = reinterpret_cast<float*>(smem + 2 * kStageBytesS);   // [sign][kTileNS]
@@ -138,6 +139,9 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
     float* const bc = sg ? p.bc_minus : p.bc_plus;
     float loss = 0.f;
     float xm[2] = {-INFINITY, -INFINITY}, xs[2] = {0.f, 0.f}, xsty[2] = {0.f, 0.f}, xst[2] = {0.f, 0.f};
+    // accuracy: per row h the (max, first index) of the logits over this thread's columns
+    float am[2] = {-INFINITY, -INFINITY};
+    int ai[2] = {INT_MAX, INT_MAX};
     int64_t wbase = 0;
 
     for (int l = 0; l < L; ++l) {
@@ -283,6 +287,24 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
                   ts[h] += expf(d[jb * 4 + 2 * h + e] - tm[h]);
 #pragma unroll
           for (int h = 0; h < 2; ++h) lse_merge(xm[h], xs[h], tm[h], ts[h]);
+        } else if constexpr (ACC) {
+#pragma unroll
+          for (int jb = 0; jb < kTileNS / 8; ++jb) {
+            const int c = jb * 8 + cq, col = n0 + c;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int b = chunk * kRowsS + r0 + 8 * h;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                if (b < p.B && col + e < N) {
+                  const float y = d[jb * 4 + 2 * h + e] + bias[c + e];
+                  estk_argmax_fold(am[h], ai[h], y, col + e);
+                  const int64_t idx = (int64_t)b * N + col + e;
+                  if (bc && b < p.bc_obs && idx < p.bc_dim) bc[(size_t)j * p.bc_dim + idx] = y;
+                }
+              }
+            }
+          }
         } else {
 #pragma unroll
           for (int jb = 0; jb < kTileNS / 8; ++jb) {
@@ -326,6 +348,17 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
         if ((lane & 3) == 0 && chunk * kRowsS + r0 + 8 * h < p.B)
           loss += fmaf(xm[h] + logf(xs[h]), xst[h], -xsty[h]);
     }
+    if constexpr (ACC) {
+      // the quad's lanes hold disjoint columns of the row; the target's label is read here, once per row
+      const int C = p.desc.dims[L];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int b = chunk * kRowsS + r0 + 8 * h;
+        estk_argmax_quad(am[h], ai[h]);
+        const int label = estk_quad_label(p.target + (size_t)b * C, b < p.B ? C : 0, lane & 3);
+        if ((lane & 3) == 0 && b < p.B && ai[h] == label) loss += 1.f;
+      }
+    }
 
     // ---- loss of each sign over the chunk; the last arriving chunk combines the partials in chunk order
     loss = warp_sum_f(loss);
@@ -339,8 +372,8 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
       part[p.chunks + chunk] = sm;
       __threadfence();
       if (estk_pair_arrive(p.counters + slot, p.chunks))
-        ESTK_PAIR_FINISH(part, p.chunks, XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L], p.ret_plus,
-                         p.ret_minus, j, p.counters + slot);
+        ESTK_PAIR_FINISH(part, p.chunks, ACC ? -(float)p.B : XENT ? (float)p.B : (float)p.B * (float)p.desc.dims[L],
+                         p.ret_plus, p.ret_minus, j, p.counters + slot);
     }
   }
 }
@@ -363,6 +396,11 @@ StreamKernel stream_kernel(int act) {
     case ESTK_ACT_LEAKY_RELU: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU>;
     case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
     case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
+    case ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>;
+    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>;
     default: return eval_mlp_tc_stream_kernel<ESTK_ACT_RELU>;
   }
 }

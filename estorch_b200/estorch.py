@@ -45,7 +45,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
+from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_ACCURACY, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
 from .agents import DeviceAgent, PopulationAgent, SequenceAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import (CNNSpec, ConvVBNSpec, RNNSpec, cnn_spec_from_module, conv_vbn_spec_from_module,
@@ -253,8 +253,8 @@ class ES:
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
             ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
-                        (ReLU, Tanh, ELU, SiLU and LeakyReLU MLPs alike, with the squared error or the
-                        cross-entropy of ``DeviceAgent(loss=...)``; always ``"fp32"`` for
+                        (ReLU, Tanh, ELU, SiLU and LeakyReLU MLPs alike, with the squared error, the
+                        cross-entropy or the accuracy of ``DeviceAgent(loss=...)``; always ``"fp32"`` for
                         the conv policy);
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
                         ``bf16s`` additionally reads bf16 shadows of theta and the table);
@@ -459,8 +459,9 @@ class ES:
             return False                        # any k (estorch.py:413) -> hooks mode (host novelty) serves it
         if population:
             pass                                # its episodes are user code: no shape of the agent to check
-        elif getattr(self.agent, "loss", "mse") == "cross_entropy" and (self._is_conv or self._spec.output != "identity"):
-            return False                        # the softmax is the output map: identity-output MLPs only
+        elif getattr(self.agent, "loss", "mse") in ("cross_entropy", "accuracy") and \
+                (self._is_conv or self._spec.output != "identity"):
+            return False                        # the logits are the output: identity-output MLPs and CNNs only
         elif self._is_conv:
             if self._ALGORITHM_TYPE != _Algorithm.classic:      # no behaviour characteristic on the conv kernel yet
                 return False
@@ -909,8 +910,10 @@ class ES:
 
     def _act_code(self):
         """``estk_mlp_desc.activation`` of the MLP evaluate: the policy's activations (include/estk.h
-        ESTK_ACT_*) and the agent's loss (ESTK_LOSS_XENT for ``loss="cross_entropy"``)."""
-        return self._spec.act | (ESTK_LOSS_XENT if getattr(self.agent, "loss", "mse") == "cross_entropy" else 0)
+        ESTK_ACT_*) and the agent's loss (ESTK_LOSS_XENT for ``loss="cross_entropy"``, ESTK_LOSS_ACCURACY for
+        ``loss="accuracy"``)."""
+        loss = getattr(self.agent, "loss", "mse")
+        return self._spec.act | {"cross_entropy": ESTK_LOSS_XENT, "accuracy": ESTK_LOSS_ACCURACY}.get(loss, 0)
 
     def _mlp_kw(self, slot, centre=False):
         """``_eval_kw`` plus the code of ``_act_code``.  It is left out for ReLU hidden + identity

@@ -101,6 +101,19 @@ typedef struct {
  *              bits from run to run); the max shift keeps it finite for finite logits and a
  *              NaN logit gives a NaN return.  The behaviour characteristic stays the logits.
  *              Valid with the identity output only (the softmax is the output map).
+ *              ESTK_LOSS_ACCURACY classification accuracy on the logits y (acc + bias), target rows
+ *              t_b = class weights as for ESTK_LOSS_XENT:
+ *                label_b = the first index of the maximum of t_b,
+ *                pred_b  = the first index of the maximum of y_b (torch.argmax's rule: ties go to the
+ *                          lowest index and a NaN counts as the maximum, so the first NaN wins),
+ *                return  = (float)count / (float)B, count = #{b : pred_b == label_b}, an IEEE divide.
+ *              count is an exact integer (per-row 0 / 1 values summed without float atomics), so the
+ *              return is the same bits from run to run and, on the same logits, those of
+ *              torch's (y.argmax(1) == t.argmax(1)).float().mean() on the CPU.  B < 2^24 keeps the
+ *              count exact (a larger B is ESTK_ERR_INVALID with this loss).  The behaviour
+ *              characteristic stays the logits.  Valid with the identity output only, for the hidden
+ *              kinds of bits 0-7 (not with a recurrent cell), in the dense MLP evaluate (every
+ *              precision, under the shape rules of the cross-entropy) and in the convolutional evaluate.
  *              ESTK_ACTIONS: no return at all -- the outputs themselves, on each member's OWN
  *              observations (one forward of every perturbed policy per environment step):
  *                population (offsets != NULL): obs is [2*pairs][B][dims[0]]; block j holds the
@@ -198,6 +211,7 @@ typedef struct {
  * ESTK_CELL_LSTM}: c | ESTK_ACTIONS and c | ESTK_ACT_OUT_TANH | ESTK_ACTIONS (4 codes; the MLP and step
  * codes, 29 in all; the sequence codes add 6: c, c | ESTK_ACT_OUT_TANH and c | ESTK_LOSS_XENT, 35 in all).
  * Loss value 2 (0x20000) is undefined.
+ * ESTK_LOSS_ACCURACY (6 << 16) adds 5 codes beside them: h | ESTK_LOSS_ACCURACY for each hidden kind h.
  * 0 is ReLU hidden + identity output + squared error.  Any other value is ESTK_ERR_INVALID in
  * estk_eval_mlp with ESTK_PREC_FP32, ESTK_ERR_UNSUPPORTED with a tensor-core precision,
  * and makes estk_eval_mlp_supported return 0.
@@ -221,6 +235,7 @@ typedef struct {
 #define ESTK_ACT_OUT_TANH (1 << 8)
 #define ESTK_LOSS_XENT (1 << 16)
 #define ESTK_ACTIONS (3 << 16)
+#define ESTK_LOSS_ACCURACY (6 << 16)
 /* the convolutional evaluate (above): n_conv in bits 24-31 of the activation code, packed dims */
 #define ESTK_CNN_N_CONV(n) ((int32_t)((uint32_t)(n) << 24))
 #define ESTK_CNN_INPUT(c, h, w) ((int32_t)((uint32_t)(c) | (uint32_t)(h) << 10 | (uint32_t)(w) << 20))
