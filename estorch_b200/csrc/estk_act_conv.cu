@@ -482,10 +482,5 @@ int eval_conv_actions(estk_ctx* ctx, const EvalConvCall& c, cudaStream_t stream)
     a.table = c.table; a.table16 = c.table16; a.order = c.order; a.pairs = c.pairs; a.sigma = c.sigma;
     a.out_minus = c.ret_minus;
   }
-  switch (nb) {
-    case 1: return launch_act<1>(ctx, a, stream);
-    case 2: return launch_act<2>(ctx, a, stream);
-    case 4: return launch_act<4>(ctx, a, stream);
-    default: return launch_act<8>(ctx, a, stream);
-  }
+  return estk_dispatch(EstkChunkRows{}, nb, [&](auto NB) { return launch_act<NB>(ctx, a, stream); });
 }

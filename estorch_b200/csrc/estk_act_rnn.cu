@@ -230,15 +230,6 @@ int launch_rnn(estk_ctx* ctx, RnnParams& p, cudaStream_t stream, const char* who
                           l, kThreads, stream, who, [] {});
 }
 
-template <int BC>
-int launch_bc(estk_ctx* ctx, RnnParams& p, int code, cudaStream_t stream, const char* who) {
-  const bool out_tanh = (code & ESTK_ACT_OUT_TANH) != 0;
-  if ((code & 0xff) == ESTK_CELL_GRU)
-    return out_tanh ? launch_rnn<BC, ESTK_CELL_GRU, true>(ctx, p, stream, who)
-                    : launch_rnn<BC, ESTK_CELL_GRU, false>(ctx, p, stream, who);
-  return out_tanh ? launch_rnn<BC, ESTK_CELL_LSTM, true>(ctx, p, stream, who)
-                  : launch_rnn<BC, ESTK_CELL_LSTM, false>(ctx, p, stream, who);
-}
 
 }  // namespace
 
@@ -261,10 +252,10 @@ int eval_rnn_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
   const int bc = estk_chunk_rows(c.B);
   p.chunks = (c.B + bc - 1) / bc;
-  switch (bc) {
-    case 1: return launch_bc<1>(ctx, p, d.activation, stream, who);
-    case 2: return launch_bc<2>(ctx, p, d.activation, stream, who);
-    case 4: return launch_bc<4>(ctx, p, d.activation, stream, who);
-    default: return launch_bc<8>(ctx, p, d.activation, stream, who);
-  }
+  return estk_dispatch(EstkChunkRows{}, bc, [&](auto BC) {
+    return estk_dispatch(EstkCells{}, d.activation & 0xff, [&](auto CELL) {
+      return estk_dispatch(EstkActionOutputs{}, d.activation & ESTK_ACT_OUT_TANH,
+                           [&](auto O) { return launch_rnn<BC, CELL, O != 0>(ctx, p, stream, who); });
+    });
+  });
 }

@@ -6,6 +6,7 @@
 #include <stdarg.h>
 #include <algorithm>
 #include <climits>
+#include <type_traits>
 #include "estk.h"
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
@@ -35,16 +36,35 @@ void estk_set_error(const char* fmt, ...);
 
 #define ESTK_ALIGNED16(p) ((((uintptr_t)(p)) & 15u) == 0)
 
-// estk_mlp_desc.activation: the forty defined codes (each hidden kind ReLU / Tanh / ELU / SiLU /
-// LeakyReLU and each recurrent cell GRU / LSTM x output identity / Tanh with the squared error, x identity
-// output with the cross-entropy, and x output identity / Tanh with ESTK_ACTIONS; each hidden kind, not a
-// cell, x identity output with the accuracy)
+// ---------------------------------------------------------------- compile-time value lists
+// The values a kernel template parameter is instantiated over.  estk_dispatch(list, v, f) calls the generic
+// lambda f with std::integral_constant<int, V> for the V of the list that equals v, and with the first value
+// of the list (the default) when none does.  f is instantiated for every value of its list, so a kernel with
+// two such parameters nests two dispatches over the two lists, and the instantiations are exactly their product.
+template <int... V> struct EstkValues {};
+template <int... V> __host__ __device__ constexpr bool estk_in(EstkValues<V...>, int v) { return ((v == V) || ...); }
+template <int D, int... V, class F> auto estk_dispatch(EstkValues<D, V...>, int v, F&& f) {
+  decltype(f(std::integral_constant<int, D>{})) r{};
+  const bool hit = ((v == V ? (r = f(std::integral_constant<int, V>{}), true) : false) || ...);
+  return hit ? r : f(std::integral_constant<int, D>{});
+}
+// bits 0-7 of estk_mlp_desc.activation: the hidden kinds (ReLU, the default, first) and the recurrent cells
+using EstkHiddenKinds = EstkValues<ESTK_ACT_RELU, ESTK_ACT_TANH, ESTK_ACT_ELU, ESTK_ACT_SILU, ESTK_ACT_LEAKY_RELU>;
+using EstkCells = EstkValues<ESTK_CELL_GRU, ESTK_CELL_LSTM>;
+// bits 8-23 of a dense MLP code with a return (output activation | loss), and the output bits alone of an
+// ESTK_ACTIONS code (an MLP or a recurrent cell step)
+using EstkDenseOutLoss = EstkValues<0, ESTK_ACT_OUT_TANH, ESTK_LOSS_XENT, ESTK_LOSS_ACCURACY>;
+using EstkActionOutputs = EstkValues<0, ESTK_ACT_OUT_TANH>;
+
+// estk_mlp_desc.activation: the forty defined codes (each hidden kind of EstkHiddenKinds and each recurrent
+// cell of EstkCells x output identity / Tanh with the squared error, x identity output with the cross-entropy,
+// and x output identity / Tanh with ESTK_ACTIONS; each hidden kind, not a cell, x identity output with the
+// accuracy)
 static inline bool estk_act_valid(int a) {
   const int h = a & 0xff, rest = a & ~0xff;
   const bool actions = rest == ESTK_ACTIONS || rest == (ESTK_ACT_OUT_TANH | ESTK_ACTIONS);
-  const bool cell = h == ESTK_CELL_GRU || h == ESTK_CELL_LSTM;
-  const bool known = h == ESTK_ACT_RELU || h == ESTK_ACT_TANH || h == ESTK_ACT_ELU || h == ESTK_ACT_SILU ||
-                     h == ESTK_ACT_LEAKY_RELU || cell;
+  const bool cell = estk_in(EstkCells{}, h);
+  const bool known = estk_in(EstkHiddenKinds{}, h) || cell;
   return known && (rest == 0 || rest == ESTK_ACT_OUT_TANH || rest == ESTK_LOSS_XENT || actions ||
                    (rest == ESTK_LOSS_ACCURACY && !cell));
 }
@@ -59,20 +79,26 @@ enum EvalRoute { kRouteDense, kRouteCnn, kRouteActions, kRouteActionsCell, kRout
 static inline EvalRoute estk_eval_route(int a) {
   if ((a >> 24) & 0xff) return kRouteCnn;
   if (!estk_act_valid(a)) return kRouteDense;
-  const bool cell = (a & 0xff) == ESTK_CELL_GRU || (a & 0xff) == ESTK_CELL_LSTM;
+  const bool cell = estk_in(EstkCells{}, a & 0xff);
   if ((a & 0xff0000) == ESTK_ACTIONS) return cell ? kRouteActionsCell : kRouteActions;
   return cell ? kRouteSequence : kRouteDense;
 }
 // The output head of a code with a return, a compile-time parameter of the sequence and convolutional
 // evaluates: identity, tanhf, or the logits of the cross-entropy (which takes precedence over the Tanh bit)
-constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2, kHeadAccuracy = 3;
+// or of the accuracy.  kHeadAct | kHeadIdentity or kHeadTanh: the act variant of the convolutional kernel
+// (estk_act_cnn), which writes the outputs instead of scoring them.
+constexpr int kHeadIdentity = 0, kHeadTanh = 1, kHeadXent = 2, kHeadAccuracy = 3, kHeadAct = 4;
 static inline int estk_head(int code) {
   return estk_loss_accuracy(code) ? kHeadAccuracy : (code & ESTK_LOSS_XENT) ? kHeadXent
        : (code & ESTK_ACT_OUT_TANH) ? kHeadTanh : kHeadIdentity;
 }
+using EstkSeqHeads = EstkValues<kHeadIdentity, kHeadXent, kHeadTanh>;
+using EstkCnnHeads = EstkValues<kHeadIdentity, kHeadXent, kHeadAccuracy, kHeadTanh, kHeadAct | kHeadTanh,
+                                kHeadAct | kHeadIdentity>;
 // Rows per sign in one work item of the fp32 act kernels (an environment population): B itself up to 2, then
-// 4, then 8 -- one instantiation per value.
+// 4, then 8 -- one instantiation per value of EstkChunkRows.
 static inline int estk_chunk_rows(int B) { return B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8; }
+using EstkChunkRows = EstkValues<1, 2, 4, 8>;
 
 #ifdef __CUDACC__
 // y / d rounded to nearest-even in fp32 -- the bits of the IEEE divide y / d -- for d >= 1 or d = +inf,
@@ -96,8 +122,7 @@ __device__ __forceinline__ float estk_div_rn_ge1(float y, float d) {
 // SiLU divides with estk_div_rn_ge1 instead of div.rn -- the same bits, another register footprint.
 template <int H, bool CALL_FREE_DIV = false>
 __device__ __forceinline__ float estk_hidden_act(float y) {
-  static_assert(H == ESTK_ACT_RELU || H == ESTK_ACT_TANH || H == ESTK_ACT_ELU || H == ESTK_ACT_SILU ||
-                H == ESTK_ACT_LEAKY_RELU, "undefined hidden activation");
+  static_assert(estk_in(EstkHiddenKinds{}, H), "undefined hidden activation");
   if constexpr (H == ESTK_ACT_TANH) return tanhf(y);
   else if constexpr (H == ESTK_ACT_ELU) return y > 0.f ? y : expm1f(y);
   else if constexpr (H == ESTK_ACT_SILU) {
@@ -371,6 +396,33 @@ __device__ __forceinline__ bool estk_pair_arrive(unsigned int* counter, int item
 __device__ __forceinline__ void estk_argmax_fold(float& m, int& i, float v, int k) {
   const bool better = v != v ? (m == m || k < i) : (m == m && (v > m || (v == m && k < i)));
   if (better) { m = v; i = k; }
+}
+// The loss of one row of an fp32 evaluate's row pass: the outputs y(0 .. C) (a loader of the row's columns from
+// shared memory or the slab) against the target row t[0 .. C), in column order.  kHeadXent: the cross-entropy
+// m + log sum exp(y - m) times sum t, minus sum t*y; any other head: the squared error sum (y - t)^2.  Only
+// where the kernel keeps its SASS: the dense and streamed MLP kernels' accuracy and the convolutional kernel's
+// scores are their own lines (with this helper inlined, their registers are allocated differently).
+template <int HEAD, class Y>
+__device__ __forceinline__ float estk_row_loss(Y y, const float* t, int C) {
+  if constexpr (HEAD == kHeadXent) {
+    float m = -INFINITY;
+    for (int c = 0; c < C; ++c) m = fmaxf(m, y(c));
+    float s = 0.f, st = 0.f, sty = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float v = y(c), tv = __ldg(t + c);
+      s += expf(v - m);
+      st += tv;
+      sty = fmaf(tv, v, sty);
+    }
+    return fmaf(m + logf(s), st, -sty);
+  } else {
+    float s = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float d = y(c) - __ldg(t + c);
+      s = fmaf(d, d, s);
+    }
+    return s;
+  }
 }
 // The fold across the four lanes of a quad (lane distance 1, then 2): every lane ends with the quad's result.
 // All 32 lanes of the warp take part.

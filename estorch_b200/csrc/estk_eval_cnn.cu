@@ -38,10 +38,6 @@ constexpr int kMaxKT = 256;                  // taps per tile
 constexpr size_t kSmemBudget = 220 * 1024;   // up to the 227 KB a CTA may hold
 constexpr size_t kSmemPreferred = 110 * 1024;  // two CTAs per SM
 constexpr int64_t kSlabBudgetFloats = (int64_t)1 << 28;  // 1 GB of slab for the whole grid (at least one CTA's)
-// HEAD = kHeadAct | kHeadIdentity or kHeadTanh: the act variant (estk_act_cnn); the evaluate's HEAD values
-// (kHeadIdentity, kHeadTanh, kHeadXent) name the same kernels as before the act variant existed; kHeadAccuracy
-// is the evaluate only
-constexpr int kHeadAct = 4;
 
 struct CnnLayer {
   int cin, hin, win, cout, k, s, pad, ho, wo;
@@ -199,7 +195,7 @@ __global__ void __launch_bounds__(kThreads) eval_cnn_kernel(const CnnParams p) {
     if (tid < ROWS && bl < nb) {
       const bool minus = r >= BC;
       const float* const tg = p.target + (size_t)b * p.out;
-      float s = 0.f;
+      float s = 0.f;   // the kernel's own lines, not estk_row_loss: the inlined helper changes its SASS
       if constexpr (HEAD == kHeadXent) {
         float m = -INFINITY;
         for (int o = 0; o < p.out; ++o) m = fmaxf(m, Yo[(size_t)o * ROWS + r]);
@@ -281,24 +277,11 @@ int launch_cnn(estk_ctx* ctx, CnnParams& p, cudaStream_t stream, const char* who
                           });
 }
 
-template <int HID>
-int launch_hid(estk_ctx* ctx, CnnParams& p, int head, cudaStream_t stream, const char* who) {
-  if (head == kHeadXent) return launch_cnn<HID, kHeadXent>(ctx, p, stream, who);
-  if (head == kHeadAccuracy) return launch_cnn<HID, kHeadAccuracy>(ctx, p, stream, who);
-  if (head == kHeadTanh) return launch_cnn<HID, kHeadTanh>(ctx, p, stream, who);
-  if (head == (kHeadAct | kHeadTanh)) return launch_cnn<HID, kHeadAct | kHeadTanh>(ctx, p, stream, who);
-  if (head == (kHeadAct | kHeadIdentity)) return launch_cnn<HID, kHeadAct | kHeadIdentity>(ctx, p, stream, who);
-  return launch_cnn<HID, kHeadIdentity>(ctx, p, stream, who);
-}
-
+// The kernel of hidden kind code & 0xff and head `head` (estk_head, or kHeadAct | the output of an act call)
 int launch_code(estk_ctx* ctx, CnnParams& p, int code, int head, cudaStream_t stream, const char* who) {
-  switch (code & 0xff) {
-    case ESTK_ACT_TANH: return launch_hid<ESTK_ACT_TANH>(ctx, p, head, stream, who);
-    case ESTK_ACT_ELU: return launch_hid<ESTK_ACT_ELU>(ctx, p, head, stream, who);
-    case ESTK_ACT_SILU: return launch_hid<ESTK_ACT_SILU>(ctx, p, head, stream, who);
-    case ESTK_ACT_LEAKY_RELU: return launch_hid<ESTK_ACT_LEAKY_RELU>(ctx, p, head, stream, who);
-    default: return launch_hid<ESTK_ACT_RELU>(ctx, p, head, stream, who);
-  }
+  return estk_dispatch(EstkHiddenKinds{}, code & 0xff, [&](auto HID) {
+    return estk_dispatch(EstkCnnHeads{}, head, [&](auto HEAD) { return launch_cnn<HID, HEAD>(ctx, p, stream, who); });
+  });
 }
 
 // The layers of a packed descriptor (include/estk.h, convolutional evaluate) into p.layer, p.n_layers, p.in_size,
@@ -393,8 +376,7 @@ extern "C" int estk_act_cnn(estk_ctx* ctx, const estk_mlp_desc* desc, const floa
                  n_conv, code);
   ESTK_CHECK_ARG((low & ~0xff) == ESTK_ACTIONS || (low & ~0xff) == (ESTK_ACTIONS | ESTK_ACT_OUT_TANH),
                  "%s: activation=0x%x: bits 8-23 must be ESTK_ACTIONS, optionally with ESTK_ACT_OUT_TANH", who, code);
-  ESTK_CHECK_ARG(hid == ESTK_ACT_RELU || hid == ESTK_ACT_TANH || hid == ESTK_ACT_ELU || hid == ESTK_ACT_SILU ||
-                 hid == ESTK_ACT_LEAKY_RELU, "%s: activation=0x%x: bits 0-7 are not a hidden kind", who, code);
+  ESTK_CHECK_ARG(estk_in(EstkHiddenKinds{}, hid), "%s: activation=0x%x: bits 0-7 are not a hidden kind", who, code);
 
   CnnParams p = {};
   if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;

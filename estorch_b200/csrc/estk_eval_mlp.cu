@@ -197,21 +197,11 @@ __global__ void __launch_bounds__(kThreads) eval_mlp_kernel(const EvalParams p) 
     __syncthreads();
     const int C = p.desc.dims[L];
     const int b = b0 + (tid % BC);
-    if (tid < ROWS && b < p.B) {
-      const float* t = p.target + (size_t)b * C;
-      float m = -INFINITY;
-      for (int c = 0; c < C; ++c) m = fmaxf(m, X[(size_t)c * ROWS + tid]);
-      float s = 0.f, st = 0.f, sty = 0.f;
-      for (int c = 0; c < C; ++c) {
-        const float y = X[(size_t)c * ROWS + tid], tv = __ldg(t + c);
-        s += expf(y - m);
-        st += tv;
-        sty = fmaf(tv, y, sty);
-      }
-      loss = fmaf(m + logf(s), st, -sty);
-    }
+    if (tid < ROWS && b < p.B)
+      loss = estk_row_loss<kHeadXent>([=](int c) { return X[(size_t)c * ROWS + tid]; }, p.target + (size_t)b * C, C);
   }
-  // ---- accuracy: thread r < ROWS compares the first argmax of row r of the logits with its target's
+  // ---- accuracy: thread r < ROWS compares the first argmax of row r of the logits with its target's (here, not
+  // estk_row_loss: the inlined helper allocates this kernel's registers differently)
   if constexpr (ACC) {
     __syncthreads();
     const int C = p.desc.dims[L];
@@ -263,32 +253,6 @@ int launch_act(const EvalParams& p, size_t smem, cudaStream_t stream) {
   eval_mlp_kernel<ROWS, ACT><<<p.pairs * p.chunks, kThreads, smem, stream>>>(p);
   ESTK_CUDA(cudaGetLastError());
   return ESTK_OK;
-}
-
-template <int ROWS>
-int launch(const EvalParams& p, size_t smem, cudaStream_t stream) {
-  switch (p.desc.activation) {
-    case ESTK_ACT_TANH: return launch_act<ROWS, ESTK_ACT_TANH>(p, smem, stream);
-    case ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_OUT_TANH>(p, smem, stream);
-    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, smem, stream);
-    case ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_LOSS_XENT>(p, smem, stream);
-    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_act<ROWS, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, smem, stream);
-    case ESTK_ACT_ELU: return launch_act<ROWS, ESTK_ACT_ELU>(p, smem, stream);
-    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>(p, smem, stream);
-    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_LOSS_XENT>(p, smem, stream);
-    case ESTK_ACT_SILU: return launch_act<ROWS, ESTK_ACT_SILU>(p, smem, stream);
-    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>(p, smem, stream);
-    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_LOSS_XENT>(p, smem, stream);
-    case ESTK_ACT_LEAKY_RELU: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU>(p, smem, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, smem, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, smem, stream);
-    case ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_LOSS_ACCURACY>(p, smem, stream);
-    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>(p, smem, stream);
-    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>(p, smem, stream);
-    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>(p, smem, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return launch_act<ROWS, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>(p, smem, stream);
-    default: return launch_act<ROWS, ESTK_ACT_RELU>(p, smem, stream);
-  }
 }
 
 // ---------------------------------------------------------------- streamed kernel
@@ -475,21 +439,11 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
       const float* Y = ((L - 1) & 1) ? act1 : act0;
       const int C = p.desc.dims[L];
       const int b = b0 + (tid % BC);
-      if (tid < ROWS && b < p.B) {
-        const float* t = p.target + (size_t)b * C;
-        float m = -INFINITY;
-        for (int c = 0; c < C; ++c) m = fmaxf(m, __ldcg(Y + (size_t)c * ROWS + tid));
-        float s = 0.f, st = 0.f, sty = 0.f;
-        for (int c = 0; c < C; ++c) {
-          const float y = __ldcg(Y + (size_t)c * ROWS + tid), tv = __ldg(t + c);
-          s += expf(y - m);
-          st += tv;
-          sty = fmaf(tv, y, sty);
-        }
-        loss = fmaf(m + logf(s), st, -sty);
-      }
+      if (tid < ROWS && b < p.B)
+        loss = estk_row_loss<kHeadXent>([=](int c) { return __ldcg(Y + (size_t)c * ROWS + tid); },
+                                        p.target + (size_t)b * C, C);
     }
-    // ---- accuracy: thread r < ROWS compares the first argmax of row r of the logits with its target's
+    // ---- accuracy: as in eval_mlp_kernel, the kernel's own lines
     if constexpr (ACC) {
       __syncthreads();
       const float* Y = ((L - 1) & 1) ? act1 : act0;
@@ -529,29 +483,13 @@ __global__ void __launch_bounds__(kThreads, 1) eval_mlp_wide_kernel(const EvalPa
 
 using WideKernel = void (*)(const EvalParams, float*, int);
 
+// The kernel of a defined code: hidden kind x output / loss
 WideKernel wide_kernel(int act) {
-  switch (act) {
-    case ESTK_ACT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_TANH>;
-    case ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>;
-    case ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_LOSS_XENT>;
-    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return eval_mlp_wide_kernel<ESTK_LOSS_XENT | ESTK_ACT_TANH>;
-    case ESTK_ACT_ELU: return eval_mlp_wide_kernel<ESTK_ACT_ELU>;
-    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_LOSS_XENT>;
-    case ESTK_ACT_SILU: return eval_mlp_wide_kernel<ESTK_ACT_SILU>;
-    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_LOSS_XENT>;
-    case ESTK_ACT_LEAKY_RELU: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
-    case ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return eval_mlp_wide_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>;
-    default: return eval_mlp_wide_kernel<ESTK_ACT_RELU>;
-  }
+  return estk_dispatch(EstkHiddenKinds{}, act & 0xff, [&](auto H) {
+    return estk_dispatch(EstkDenseOutLoss{}, act & ~0xff, [&](auto O) -> WideKernel {
+      return eval_mlp_wide_kernel<H | O>;
+    });
+  });
 }
 
 // The streamed kernel for a checked call: a persistent grid of at most (resident CTAs per SM) x SMs,
@@ -609,13 +547,13 @@ int run_eval(estk_ctx* ctx, EvalParams& p, cudaStream_t stream, const char* who)
   p.partial = ctx->eval_partial;
   p.counters = estk_member_counters(ctx);
   const size_t smem = smem_bytes(rows, maxw);
-  switch (rows) {
-    case 256: return launch<256>(p, smem, stream);
-    case 128: return launch<128>(p, smem, stream);
-    case 64: return launch<64>(p, smem, stream);
-    case 32: return launch<32>(p, smem, stream);
-    default: return launch<16>(p, smem, stream);
-  }
+  return estk_dispatch(EstkValues<16, 32, 64, 128, 256>{}, rows, [&](auto R) {
+    return estk_dispatch(EstkHiddenKinds{}, d.activation & 0xff, [&](auto H) {
+      return estk_dispatch(EstkDenseOutLoss{}, d.activation & ~0xff, [&](auto O) {
+        return launch_act<R, H | O>(p, smem, stream);
+      });
+    });
+  });
 }
 
 }  // namespace

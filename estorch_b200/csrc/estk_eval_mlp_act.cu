@@ -172,22 +172,6 @@ int launch_act(estk_ctx* ctx, ActParams& p, cudaStream_t stream, const char* who
                           kThreads, stream, who, [] {});
 }
 
-template <int BC>
-int launch_bc(estk_ctx* ctx, ActParams& p, cudaStream_t stream, const char* who) {
-  switch (p.desc.activation & 0xffff) {   // the loss field is ESTK_ACTIONS here
-    case ESTK_ACT_TANH: return launch_act<BC, ESTK_ACT_TANH>(ctx, p, stream, who);
-    case ESTK_ACT_ELU: return launch_act<BC, ESTK_ACT_ELU>(ctx, p, stream, who);
-    case ESTK_ACT_SILU: return launch_act<BC, ESTK_ACT_SILU>(ctx, p, stream, who);
-    case ESTK_ACT_LEAKY_RELU: return launch_act<BC, ESTK_ACT_LEAKY_RELU>(ctx, p, stream, who);
-    case ESTK_ACT_OUT_TANH: return launch_act<BC, ESTK_ACT_OUT_TANH>(ctx, p, stream, who);
-    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_act<BC, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(ctx, p, stream, who);
-    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return launch_act<BC, ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>(ctx, p, stream, who);
-    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return launch_act<BC, ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>(ctx, p, stream, who);
-    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH:
-      return launch_act<BC, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(ctx, p, stream, who);
-    default: return launch_act<BC, ESTK_ACT_RELU>(ctx, p, stream, who);
-  }
-}
 
 }  // namespace
 
@@ -222,10 +206,11 @@ int eval_mlp_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) {
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
   const int bc = estk_chunk_rows(c.B);
   p.chunks = (c.B + bc - 1) / bc;
-  switch (bc) {
-    case 1: return launch_bc<1>(ctx, p, stream, who);
-    case 2: return launch_bc<2>(ctx, p, stream, who);
-    case 4: return launch_bc<4>(ctx, p, stream, who);
-    default: return launch_bc<8>(ctx, p, stream, who);
-  }
+  // the loss field is ESTK_ACTIONS here
+  return estk_dispatch(EstkChunkRows{}, bc, [&](auto BC) {
+    return estk_dispatch(EstkHiddenKinds{}, d.activation & 0xff, [&](auto H) {
+      return estk_dispatch(EstkActionOutputs{}, d.activation & ESTK_ACT_OUT_TANH,
+                           [&](auto O) { return launch_act<BC, H | O>(ctx, p, stream, who); });
+    });
+  });
 }

@@ -757,28 +757,10 @@ int tc_supported(const estk_mlp_desc& d, int B, const char** why, int mode) {
 
 template <int MODE>
 int launch_tc_act(const EvalTCParams& p, cudaStream_t stream) {
-  switch (p.desc.activation) {
-    case ESTK_ACT_TANH: return launch_tc<MODE, ESTK_ACT_TANH>(p, stream);
-    case ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_OUT_TANH>(p, stream);
-    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>(p, stream);
-    case ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_LOSS_XENT>(p, stream);
-    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return launch_tc<MODE, ESTK_LOSS_XENT | ESTK_ACT_TANH>(p, stream);
-    case ESTK_ACT_ELU: return launch_tc<MODE, ESTK_ACT_ELU>(p, stream);
-    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>(p, stream);
-    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_LOSS_XENT>(p, stream);
-    case ESTK_ACT_SILU: return launch_tc<MODE, ESTK_ACT_SILU>(p, stream);
-    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>(p, stream);
-    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_LOSS_XENT>(p, stream);
-    case ESTK_ACT_LEAKY_RELU: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU>(p, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>(p, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>(p, stream);
-    case ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_LOSS_ACCURACY>(p, stream);
-    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>(p, stream);
-    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>(p, stream);
-    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>(p, stream);
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return launch_tc<MODE, ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>(p, stream);
-    default: return launch_tc<MODE, ESTK_ACT_RELU>(p, stream);
-  }
+  return estk_dispatch(EstkHiddenKinds{}, p.desc.activation & 0xff, [&](auto H) {
+    return estk_dispatch(EstkDenseOutLoss{}, p.desc.activation & ~0xff,
+                         [&](auto O) { return launch_tc<MODE, H | O>(p, stream); });
+  });
 }
 
 int run_tc(estk_ctx* ctx, EvalTCParams& p, cudaStream_t stream, const char* who) {

@@ -381,28 +381,10 @@ __global__ void __launch_bounds__(kThreadsS, 1) eval_mlp_tc_stream_kernel(const 
 using StreamKernel = void (*)(const StreamParams);
 
 StreamKernel stream_kernel(int act) {
-  switch (act) {
-    case ESTK_ACT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_TANH>;
-    case ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_TANH | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_TANH | ESTK_ACT_OUT_TANH>;
-    case ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_LOSS_XENT>;
-    case ESTK_LOSS_XENT | ESTK_ACT_TANH: return eval_mlp_tc_stream_kernel<ESTK_LOSS_XENT | ESTK_ACT_TANH>;
-    case ESTK_ACT_ELU: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU>;
-    case ESTK_ACT_ELU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_ELU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_LOSS_XENT>;
-    case ESTK_ACT_SILU: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU>;
-    case ESTK_ACT_SILU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_SILU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_LOSS_XENT>;
-    case ESTK_ACT_LEAKY_RELU: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_ACT_OUT_TANH>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_XENT>;
-    case ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_TANH | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_TANH | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_ELU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_ELU | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_SILU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_SILU | ESTK_LOSS_ACCURACY>;
-    case ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY: return eval_mlp_tc_stream_kernel<ESTK_ACT_LEAKY_RELU | ESTK_LOSS_ACCURACY>;
-    default: return eval_mlp_tc_stream_kernel<ESTK_ACT_RELU>;
-  }
+  return estk_dispatch(EstkHiddenKinds{}, act & 0xff, [&](auto H) {
+    return estk_dispatch(EstkDenseOutLoss{}, act & ~0xff,
+                         [&](auto O) -> StreamKernel { return eval_mlp_tc_stream_kernel<H | O>; });
+  });
 }
 
 }  // namespace

@@ -221,27 +221,8 @@ __global__ void __launch_bounds__(kThreads, SLAB ? 1 : 2) eval_rnn_seq_kernel(co
       // ---- 4. thread r < ROWS scores step t of row r in column order
       const int b = b0 + tid % BC;
       if (tid < ROWS && b < p.B) {
-        const float* const tg = p.target + ((size_t)b * T + t) * out;
-        float s;
-        if constexpr (HEAD == kHeadXent) {
-          float m = -INFINITY;
-          for (int o = 0; o < out; ++o) m = fmaxf(m, Y[(size_t)o * ROWS + tid]);
-          float se = 0.f, st = 0.f, sty = 0.f;
-          for (int o = 0; o < out; ++o) {
-            const float y = Y[(size_t)o * ROWS + tid], tv = __ldg(tg + o);
-            se += expf(y - m);
-            st += tv;
-            sty = fmaf(tv, y, sty);
-          }
-          s = fmaf(m + logf(se), st, -sty);
-        } else {
-          s = 0.f;
-          for (int o = 0; o < out; ++o) {
-            const float d = Y[(size_t)o * ROWS + tid] - __ldg(tg + o);
-            s = fmaf(d, d, s);
-          }
-        }
-        rloss += s;
+        rloss += estk_row_loss<HEAD>([&](int o) { return Y[(size_t)o * ROWS + tid]; },
+                                     p.target + ((size_t)b * T + t) * out, out);
       }
       // the next step's first writes (x_t) are ordered after this step's readers of X by the barriers above;
       // Y and Gt are next written only after the next step's first chain barrier
@@ -281,18 +262,6 @@ int launch_seq(estk_ctx* ctx, SeqParams& p, cudaStream_t stream, const char* who
                           });
 }
 
-template <int BC>
-int launch_bc(estk_ctx* ctx, SeqParams& p, int code, cudaStream_t stream, const char* who) {
-  const int head = estk_head(code);
-  if ((code & 0xff) == ESTK_CELL_GRU) {
-    if (head == kHeadXent) return launch_seq<BC, ESTK_CELL_GRU, kHeadXent>(ctx, p, stream, who);
-    if (head == kHeadTanh) return launch_seq<BC, ESTK_CELL_GRU, kHeadTanh>(ctx, p, stream, who);
-    return launch_seq<BC, ESTK_CELL_GRU, kHeadIdentity>(ctx, p, stream, who);
-  }
-  if (head == kHeadXent) return launch_seq<BC, ESTK_CELL_LSTM, kHeadXent>(ctx, p, stream, who);
-  if (head == kHeadTanh) return launch_seq<BC, ESTK_CELL_LSTM, kHeadTanh>(ctx, p, stream, who);
-  return launch_seq<BC, ESTK_CELL_LSTM, kHeadIdentity>(ctx, p, stream, who);
-}
 
 }  // namespace
 
@@ -342,7 +311,10 @@ int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream) 
   p.ret_plus = c.ret_plus; p.ret_minus = c.ret_minus;
   p.bc_plus = c.bc_plus; p.bc_minus = c.bc_minus; p.bc_obs = c.bc_obs; p.bc_dim = c.bc_dim;
   // chunk of sequences per work item: the bits do not depend on it (the returns are summed per sequence)
-  if (c.B == 1) return launch_bc<1>(ctx, p, d.activation, stream, who);
-  if (c.B <= 4) return launch_bc<4>(ctx, p, d.activation, stream, who);
-  return launch_bc<16>(ctx, p, d.activation, stream, who);
+  return estk_dispatch(EstkValues<16, 1, 4>{}, c.B == 1 ? 1 : c.B <= 4 ? 4 : 16, [&](auto BC) {
+    return estk_dispatch(EstkCells{}, d.activation & 0xff, [&](auto CELL) {
+      return estk_dispatch(EstkSeqHeads{}, estk_head(d.activation),
+                           [&](auto HEAD) { return launch_seq<BC, CELL, HEAD>(ctx, p, stream, who); });
+    });
+  });
 }
