@@ -55,6 +55,14 @@ from .population import LazyPopulation, NoiseHandle
 __all__ = ["ES", "NS_ES", "NSR_ES", "NSRA_ES", "rank_transformation"]
 
 DEFAULT_NOISE_TABLE_SIZE = 1 << 28   # fp32 unit normals = 1 GiB per GPU (SURVEY 8d)
+# Smallest sigma at which eval_precision="auto" evaluates an MLP in "f16".  f16 rounds each formed weight
+# theta +- sigma*eps to 11 bits, about 2^-11 |theta|: once sigma*eps is not much larger than that, the
+# antithetic differences that order the population turn to noise.  Measured on an H100 80GB HBM3 (700 W)
+# against a float64 evaluate (tests/test_signal_fidelity_gpu.py, DESIGN.md 4.3): at sigma >= 0.02 the f16
+# gradient is within 3e-2 (rel-L2) of the float64-return gradient for weights up to 8x their initial scale;
+# at sigma = 5e-3 it reaches 3.3e-2 at 4x, at sigma = 1e-3 4.4e-2.  Below the threshold "auto" evaluates
+# in fp32, whose ranks are the float64 ranks up to near-ties within fp32 rounding.
+AUTO_F16_MIN_SIGMA = 0.02
 _UNFUSED_ADAM_FLAGS = ("amsgrad", "maximize", "differentiable", "decoupled_weight_decay")
 
 
@@ -252,10 +260,19 @@ class ES:
                         For the conv + VirtualBatchNorm policy (examples/atari.py) ``"f16"``
                         is an opt-in mma.sync kernel whose weights, inputs and normalised
                         activations all enter as hi + lo fp16 pairs (22-bit operands);
-            ``"auto"``  (default) ``"f16"`` when the MLP shape supports it, else ``"fp32"``
-                        (ReLU, Tanh, ELU, SiLU and LeakyReLU MLPs alike, with the squared error, the
-                        cross-entropy or the accuracy of ``DeviceAgent(loss=...)``; always ``"fp32"`` for
-                        the conv policy);
+            ``"auto"``  (default) ``"f16"`` when the MLP shape supports it and ``sigma >=
+                        AUTO_F16_MIN_SIGMA`` (0.02), else ``"fp32"`` (ReLU, Tanh, ELU, SiLU and
+                        LeakyReLU MLPs alike, with the squared error, the cross-entropy or the accuracy
+                        of ``DeviceAgent(loss=...)``; always ``"fp32"`` for the conv policy).
+                        Accuracy of "f16" against a float64 evaluate, on what ES consumes (H100 at 700 W,
+                        P = 64): at sigma >= 0.02 and weights up to 8x their initial scale the gradient
+                        is within 3e-2 (rel-L2) of the float64-return gradient and the returns within
+                        about 2e-4 (max-norm relative; 1e-5 only at init-scale weights).  Below, the
+                        11-bit rounding of each formed weight, about 2^-11 |theta|, reorders members:
+                        gradient error up to 3.3e-2 at sigma = 5e-3 and 4x init, 4.4e-2 at 1e-3, and at
+                        sigma = 2e-4 up to a quarter of the antithetic differences change sign.  There
+                        "auto" evaluates in fp32, whose ranks are the float64 ranks up to near-ties
+                        within fp32 rounding; an explicit ``"f16"`` is still honoured;
             ``"bf16"`` / ``"bf16s"``  explicit opt-in, lower precision (8-bit significand;
                         ``bf16s`` additionally reads bf16 shadows of theta and the table);
                         MLP policies only.
@@ -366,6 +383,8 @@ class ES:
                                  "is a multiple of 256")
             self._precision = ("f16_any" if any_shape else
                                ("f16" if eval_precision == "auto" else eval_precision) if supported else "fp32")
+            if eval_precision == "auto" and float(sigma) < AUTO_F16_MIN_SIGMA:
+                self._precision = "fp32"
 
         # ---- noise table (replicated on every GPU, identical by construction)
         n_pad = (self.n_parameters + 31) // 32 * 32

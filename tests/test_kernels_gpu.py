@@ -591,7 +591,9 @@ def test_north_star_all_returns_ranks_and_gradient_f16_vs_fp32(be):
     CUDA-core kernel; then what the difference does to the rank indices, to the gradient
     estimate and to theta' (estorch.py:174-179, :236-245) -- next to the same figures for the
     fp32 kernel itself (two fp32 implementations also disagree in the last bits, and at this
-    size neighbouring returns are ~1e-7 apart) and for the opt-in bf16 modes."""
+    size neighbouring returns are ~1e-7 apart) and for the opt-in bf16 modes.  The 1e-5 return bar
+    holds at init-scale weights and sigma = 0.02, where "auto" picks f16; at grown weights the returns
+    drift to ~2e-4 and, at smaller sigma, the ranks with them (test_signal_fidelity_gpu.py)."""
     import json, os, time
     dims = [128, 512, 512, 512, 512, 288]
     n, P, pairs, sigma = orc.mlp_param_count(dims), 4096, 2048, 0.02
@@ -667,8 +669,9 @@ def test_north_star_all_returns_ranks_and_gradient_f16_vs_fp32(be):
         json.dump(report, open(os.path.join(out_dir, "north_star_precision.json"), "w"), indent=1)
     m = report["modes"]
     assert m["fp32"]["returns_max_rel_err_vs_cpu_fp32"] < 2e-6
-    # the parity bar of the default mode: every one of the 4096 returns within 1e-5 (max-norm relative)
-    # of the reference's fp32 CPU arithmetic
+    # the default mode at init-scale weights and sigma = 0.02: every one of the 4096 returns within 1e-5
+    # (max-norm relative) of the reference's fp32 CPU arithmetic.  It is not a bar for grown weights or a
+    # smaller sigma: there the measure is the gradient against a float64 evaluate (test_signal_fidelity_gpu.py)
     assert m["f16"]["returns_max_rel_err_vs_cpu_fp32"] < 1e-5
     # rank agreement and its effect on the update, as measured bounds (fp32-vs-fp32 is the floor)
     assert m["f16"]["rank_mean_displacement"] < 8 * max(1.0, m["fp32"]["rank_mean_displacement"])
