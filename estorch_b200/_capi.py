@@ -1,5 +1,5 @@
-"""ctypes binding of libestk.so (the C ABI declared in include/estk.h, include/estk_batch.h and
-include/estk_act_cnn.h).
+"""ctypes binding of libestk.so (the C ABI declared in include/estk.h, include/estk_batch.h,
+include/estk_act_cnn.h and include/estk_eval_cnn_tf32.h).
 
 The library is built in-tree by ``estorch_b200/csrc/build.sh`` (or
 ``__graft_entry__.build()``).  There is NO fallback: if the shared object is
@@ -122,6 +122,13 @@ ACT_CNN_SIGNATURES = {
     "estk_act_cnn": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _F32, _P, _I32, _P, _P, _P],
 }
 
+# include/estk_eval_cnn_tf32.h: the convolutional evaluate on TF32 tensor cores, declared beside the core of estk.h
+EVAL_CNN_TF32_SIGNATURES = {
+    "estk_eval_cnn_tf32": [_P, C.POINTER(EstkMlpDesc), _P, _P, _P, _P, _I32, _F32, _P, _P, _I32, _P, _P, _P, _P,
+                           _I32, _I32, _P],
+    "estk_eval_cnn_tf32_supported": [C.POINTER(EstkMlpDesc), _I32],
+}
+
 _lib = None
 
 
@@ -136,7 +143,8 @@ def load():
             "`bash estorch_b200/csrc/build.sh` (or `python -c 'import __graft_entry__ as g; "
             "g.build()'`). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in {**SIGNATURES, **BATCH_SIGNATURES, **ACT_CNN_SIGNATURES}.items():
+    for name, argtypes in {**SIGNATURES, **BATCH_SIGNATURES, **ACT_CNN_SIGNATURES,
+                           **EVAL_CNN_TF32_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = (C.c_char_p if name == "estk_last_error" else

@@ -221,6 +221,15 @@ class CudaBackend:
         d = mlp_desc(dims, act)
         return bool(self.lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16_ANY, int(B)))
 
+    def eval_supports_tf32_cnn(self, dims, B, act=0) -> bool:
+        """``"tf32"`` for a convolutional policy (``dims`` its packed descriptor or ``CNNSpec``, ``act`` its code
+        with n_conv): every valid descriptor whose largest layer output is at most 2**26 floats per image."""
+        try:
+            d = cnn_desc(dims, act)
+        except ValueError:
+            return False
+        return bool(self.lib.estk_eval_cnn_tf32_supported(C.byref(d), int(B)))
+
     def shadow_f16(self, src, dst, check=True) -> int:
         """dst (float16, same numel) = src; returns how many entries were NOT exactly
         representable (0 for tables made by fill_noise_table).  ``check`` reads the
@@ -336,14 +345,25 @@ class CudaBackend:
         """Fixed-batch evaluate of a convolutional policy (estk_eval_mlp with n_conv in bits 24-31 of ``act``,
         fp32): ``dims`` the packed descriptor (``CNNSpec.dims``, or the spec itself), ``obs`` ``[B, c, h, w]``,
         ``target`` ``[B, out]``.  The arguments are ``eval_mlp``'s fp32 ones, so the engine calls either the same
-        way; ``precision`` other than "fp32" is refused by the library."""
-        code, _dt16 = self._precision(precision)
+        way.  ``precision="tf32"``: the same evaluate on TF32 tensor cores (estk_eval_cnn_tf32); any other
+        precision but "fp32" is refused by the library."""
+        code = None if precision == "tf32" else self._precision(precision)[0]
         d = cnn_desc(dims, act)
         (c, h, w), out = cnn_shapes([d.dims[i] for i in range(d.n_layers + 1)], act)
         B = int(obs.shape[0])
         if tuple(obs.shape) != (B, c, h, w) or tuple(target.shape) != (B, out):
             raise ValueError(f"obs {tuple(obs.shape)} / target {tuple(target.shape)} do not match the convolutional "
                              f"policy: expected [B, {c}, {h}, {w}] / [B, {out}]")
+        if code is None:
+            _capi.check(self.lib.estk_eval_cnn_tf32(
+                self._ctx, C.byref(d), self._ptr(theta, torch.float32, "theta"), self._ptr(table, torch.float32, "table"),
+                self._ptr(offsets, torch.int64, "offsets"), self._ptr(order, torch.int32, "order"), int(pairs),
+                float(sigma), self._ptr(obs, torch.float32, "obs"), self._ptr(target, torch.float32, "target"), B,
+                self._ptr(ret_plus, torch.float32, "ret_plus"), self._ptr(ret_minus, torch.float32, "ret_minus"),
+                self._ptr(bc_plus, torch.float32, "bc_plus"), self._ptr(bc_minus, torch.float32, "bc_minus"),
+                int(bc_obs), int(bc_dim), self._stream()), "estk_eval_cnn_tf32")
+            self.launches += 1
+            return
         self._eval_mlp(f"estk_eval_mlp[convolutional, {precision}]", d, code, B, theta, table, offsets, order, pairs,
                        sigma, obs, target, ret_plus, ret_minus, bc_plus, bc_minus, bc_obs, bc_dim)
 

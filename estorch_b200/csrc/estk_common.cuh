@@ -261,6 +261,24 @@ int eval_rnn_actions(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
 int eval_rnn_sequence(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
 // kRouteCnn: its own argument checks, then the convolutional evaluate over obs [B][c][h][w] (estk_eval_cnn.cu)
 int eval_cnn(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);
+// The layers of a packed convolutional descriptor (include/estk.h): layer l maps [cin][hin][win] to
+// [cout][ho][wo] with K = cin*k*k taps per output, its weight [cout][K] then bias [cout] at wbase (a Linear is
+// the 1x1 convolution of its flattened input); maxact the largest layer output per image.
+// eval_cnn_parse (estk_eval_cnn.cu) fills it by the fp32 route's rules; every malformed field is ESTK_ERR_INVALID.
+struct EstkCnnLayer {
+  int cin, hin, win, cout, k, s, pad, ho, wo, K;
+  int64_t wbase;
+};
+struct EstkCnnShape {
+  EstkCnnLayer layer[ESTK_MAX_LAYERS];
+  int n_layers, in_size, out, maxact;
+};
+int eval_cnn_parse(const estk_mlp_desc& d, int n_conv, EstkCnnShape& s, const char* who);
+// The activation-code checks of both convolutional routes (estk_eval_cnn.cu): n_conv in 1..7 and a defined code
+// (ESTK_ERR_INVALID), and a dense code with a return -- ESTK_ACTIONS and the recurrent cells are `route_rc`; then
+// B < 2^24 with the accuracy (ESTK_ERR_INVALID)
+int eval_cnn_code_check(int code, int route_rc, const char* who);
+int eval_cnn_batch_check(int code, int B, const char* who);
 // ESTK_PREC_F16_ANY on a shape the cluster kernel does not serve (estk_eval_mlp_tc_stream.cu); the
 // shapes it serves: every valid desc, B >= 1 (else 0 and the reason in *why)
 int eval_mlp_tc_stream(estk_ctx* ctx, const EvalMlpCall& c, cudaStream_t stream);

@@ -333,23 +333,45 @@ int cnn_parse(const estk_mlp_desc& d, int n_conv, CnnParams& p, const char* who)
 
 }  // namespace
 
-int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
-  const char* who = "estk_eval_mlp[convolutional]";
-  if (const int rc = eval_returns_supported(call, who)) return rc;
-  const estk_mlp_desc& d = call.desc;
-  const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
+int eval_cnn_parse(const estk_mlp_desc& d, int n_conv, EstkCnnShape& s, const char* who) {
+  CnnParams p = {};
+  if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;
+  for (int l = 0; l < p.n_layers; ++l) {
+    const CnnLayer& a = p.layer[l];
+    s.layer[l] = EstkCnnLayer{a.cin, a.hin, a.win, a.cout, a.k, a.s, a.pad, a.ho, a.wo, a.K, a.wbase};
+  }
+  s.n_layers = p.n_layers; s.in_size = p.in_size; s.out = p.out; s.maxact = p.maxact;
+  return ESTK_OK;
+}
+
+int eval_cnn_code_check(int code, int route_rc, const char* who) {
+  const int n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
   ESTK_CHECK_ARG(n_conv >= 1 && n_conv <= 7, "%s: n_conv=%d (bits 24-31 of activation 0x%x) is outside 1..7", who,
                  n_conv, code);
   if (estk_eval_route(low) != kRouteDense) {
     estk_set_error("%s: ESTK_ACTIONS and the recurrent cells are not supported with a conv stack (code 0x%x)", who,
                    code);
-    return ESTK_ERR_UNSUPPORTED;
+    return route_rc;
   }
   ESTK_CHECK_ARG(estk_act_valid(low), "%s: activation=0x%x: bits 0-23 are not a defined hidden | output | loss "
                  "combination", who, code);
+  return ESTK_OK;
+}
+
+int eval_cnn_batch_check(int code, int B, const char* who) {
+  ESTK_CHECK_ARG(!estk_loss_accuracy(code & 0xffffff) || B <= kAccuracyMaxB,
+                 "%s: B=%d: the accuracy's count is exact in fp32 for B < 2^24 only", who, B);
+  return ESTK_OK;
+}
+
+int eval_cnn(estk_ctx* ctx, const EvalMlpCall& call, cudaStream_t stream) {
+  const char* who = "estk_eval_mlp[convolutional]";
+  if (const int rc = eval_returns_supported(call, who)) return rc;
+  const estk_mlp_desc& d = call.desc;
+  const int code = d.activation, n_conv = (code >> 24) & 0xff, low = code & 0xffffff;
+  if (const int rc = eval_cnn_code_check(code, ESTK_ERR_UNSUPPORTED, who)) return rc;
   if (const int rc = eval_returns_check(ctx, call, who)) return rc;
-  ESTK_CHECK_ARG(!estk_loss_accuracy(low) || call.B <= kAccuracyMaxB,
-                 "%s: B=%d: the accuracy's count is exact in fp32 for B < 2^24 only", who, call.B);
+  if (const int rc = eval_cnn_batch_check(code, call.B, who)) return rc;
 
   CnnParams p = {};
   if (const int rc = cnn_parse(d, n_conv, p, who)) return rc;

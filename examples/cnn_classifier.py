@@ -53,12 +53,14 @@ def accuracy(policy, x, y):
         return float((policy(x.to(p.device)).argmax(1).cpu() == y.argmax(1)).float().mean())
 
 
-def main(generations=TEST_GENERATIONS, population=TEST_POPULATION, seed=0, verbose=False):
-    """Returns (first centre return, last centre return, accuracy before, accuracy after) on the batch."""
+def main(generations=TEST_GENERATIONS, population=TEST_POPULATION, seed=0, verbose=False, eval_precision="auto"):
+    """Returns (first centre return, last centre return, accuracy before, accuracy after) on the batch.
+    ``eval_precision="tf32"`` evaluates on TF32 tensor cores instead of fp32."""
     torch.manual_seed(seed)
     x, y = bars(256, seed)
     es = ES(Classifier, DeviceAgent, torch.optim.Adam, population_size=population, sigma=0.02,
-            agent_kwargs=dict(obs=x, target=y, loss="cross_entropy"), optimizer_kwargs={"lr": 0.01})
+            agent_kwargs=dict(obs=x, target=y, loss="cross_entropy"), optimizer_kwargs={"lr": 0.01},
+            eval_precision=eval_precision)
     assert es._fused, "the CNN should be evaluated by the fused kernel"
     acc0 = accuracy(es.policy, x, y)
     rewards = []
@@ -77,6 +79,7 @@ if __name__ == "__main__":
     ap.add_argument("--generations", type=int, default=TEST_GENERATIONS)
     ap.add_argument("--population", type=int, default=TEST_POPULATION)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--eval-precision", default="auto", choices=["auto", "fp32", "tf32"])
     a = ap.parse_args()
-    first, last, acc0, acc1 = main(a.generations, a.population, a.seed, verbose=True)
+    first, last, acc0, acc1 = main(a.generations, a.population, a.seed, verbose=True, eval_precision=a.eval_precision)
     print(f"centre return {first:.4f} -> {last:.4f}, accuracy {acc0:.3f} -> {acc1:.3f}")
