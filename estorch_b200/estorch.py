@@ -392,14 +392,12 @@ class ES:
             self._precision = "f16"
         if self._fused and not (self._is_conv or self._is_rnn or self._is_cnn or self._population) and \
                 eval_precision != "fp32":
-            probe = "eval_supports_f16" if eval_precision in ("auto", "f16") else "eval_supports_bf16"
+            probe = self._be.eval_supports_f16 if eval_precision in ("auto", "f16") else self._be.eval_supports_bf16
             act_kw = {"act": self._act_code()} if self._act_code() else {}     # ReLU + MSE: the backends' default
-            supported = getattr(self._be, probe, lambda d, b, **_: False)(self._spec.dims, self.agent.obs.shape[0],
-                                                                          **act_kw)
+            supported = probe(self._spec.dims, self.agent.obs.shape[0], **act_kw)
             # "f16" where the cluster kernel's shape rule fails: the same arithmetic on the streamed kernel
             any_shape = (eval_precision == "f16" and not supported and
-                         getattr(self._be, "eval_supports_f16_any", lambda d, b, **_: False)(
-                             self._spec.dims, self.agent.obs.shape[0], **act_kw))
+                         self._be.eval_supports_f16_any(self._spec.dims, self.agent.obs.shape[0], **act_kw))
             if eval_precision != "auto" and not supported and not any_shape:
                 raise ValueError(f"eval_precision={eval_precision!r} needs layer widths that are multiples of 64 "
                                  "(in) / 32 (out), at most 512 (f16: input width at most 256), and a batch that "
@@ -911,7 +909,7 @@ class ES:
 
     def _grad_table(self):
         """Table the gradient reduction reads: the exact fp16 copy when there is one."""
-        t = self._exact_table16() if hasattr(self._be, "shadow_f16") else None
+        t = self._exact_table16()
         return self._table if t is None else t
 
     def _ensure_table16(self):
@@ -1162,7 +1160,7 @@ class ES:
             return self._population_act_cnn(slot, centre)
         be, dims, dev, code = self._be, self._spec.dims, self._dev, self._spec.act
         M = 1 if centre else self.population_size
-        t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
+        t16 = None if centre else self._exact_table16()
 
         def act(obs):
             x = torch.as_tensor(obs).to(device=dev, dtype=torch.float32).contiguous()
@@ -1254,7 +1252,7 @@ class ES:
         The centre form keeps them in a one-member buffer of its slot."""
         be, dev, A = self._be, self._dev, self._spec.n_actions
         M = 1 if centre else self.population_size
-        t16 = None if centre or not hasattr(be, "shadow_f16") else self._exact_table16()
+        t16 = None if centre else self._exact_table16()
         if centre:
             if getattr(slot, "conv_stats", None) is None:
                 slot.conv_stats = torch.empty(1, ESTK_CONV_VBN_STATS_FLOATS, dtype=torch.float32, device=dev)

@@ -31,7 +31,8 @@ import numpy as np
 __all__ = [
     "compute_ranks", "center_values", "rank_transformation",
     "mix64", "noise_slots", "noise_offsets", "philox4x32_10", "philox_normal_table",
-    "mlp_param_count", "mlp_unflatten", "mlp_forward", "mlp_forward_bf16", "round_bf16", "synthetic_return", "synthetic_bc",
+    "mlp_param_count", "mlp_unflatten", "HIDDEN", "mlp_forward", "mlp_forward_bf16", "round_bf16",
+    "synthetic_return", "synthetic_bc",
     "round_f16", "mlp_forward_f16",
     "sample_population", "sample_population_bf16s", "evaluate_population",
     "blend_weights", "calculate_grad", "calculate_grad_pairs", "negate_clamp",
@@ -180,15 +181,42 @@ def mlp_unflatten(flat: np.ndarray, dims: Sequence[int]):
     return layers
 
 
-def mlp_forward(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Linear -> ReLU -> ... -> Linear, fp32 (cartpole_es.py:14-20)."""
+def _elu(h):
+    with np.errstate(over="ignore"):
+        return np.where(h > 0, h, np.expm1(h)).astype(np.float32)
+
+
+def _silu(h):
+    with np.errstate(over="ignore"):
+        return (h / (np.float32(1.0) + np.exp(-h))).astype(np.float32)
+
+
+def _leaky_relu(h):
+    return np.where(h > 0, h, h * np.float32(0.01)).astype(np.float32)
+
+
+# The hidden activations of include/estk.h (ESTK_ACT_*), as the kernels' epilogues compute them on the
+# fp32 value y = acc + bias: elu y > 0 ? y : expm1(y); silu y / (1 + exp(-y)) with one fp32 divide;
+# leaky_relu y > 0 ? y : y * 0.01.
+HIDDEN = {"relu": lambda h: np.maximum(h, np.float32(0.0)), "tanh": np.tanh, "elu": _elu, "silu": _silu,
+          "leaky_relu": _leaky_relu}
+
+
+def _output(h, output):
+    """The output activation: identity, or tanh in fp32 (ESTK_ACT_OUT_TANH) in every precision."""
+    return np.tanh(h).astype(np.float32) if output == "tanh" else h
+
+
+def mlp_forward(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray, hidden: str = "relu",
+                output: str = "identity") -> np.ndarray:
+    """Linear -> hidden -> ... -> Linear [-> Tanh], fp32 (cartpole_es.py:14-20 with the defaults)."""
     h = np.asarray(obs, dtype=np.float32)
     layers = mlp_unflatten(np.asarray(flat, dtype=np.float32), dims)
     for li, (w, b) in enumerate(layers):
         h = (h @ w.T + b).astype(np.float32)
         if li + 1 < len(layers):
-            h = np.maximum(h, np.float32(0.0))
-    return h
+            h = HIDDEN[hidden](h)
+    return _output(h, output)
 
 
 def round_bf16(x: np.ndarray) -> np.ndarray:
@@ -198,19 +226,21 @@ def round_bf16(x: np.ndarray) -> np.ndarray:
     return u.view(np.float32)
 
 
-def mlp_forward_bf16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Numerics of the wgmma evaluate path (estk_eval_mlp, ESTK_PREC_BF16): weights and
-    layer inputs rounded to bf16, products accumulated in fp32, bias / ReLU in
-    fp32.  ``flat`` is the already-perturbed fp32 row."""
+def mlp_forward_bf16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray, hidden: str = "relu",
+                     output: str = "identity") -> np.ndarray:
+    """Numerics of the wgmma evaluate path (estk_eval_mlp, ESTK_PREC_BF16 / BF16S): weights and
+    layer inputs rounded to bf16, products accumulated in fp32, bias and the hidden activation in
+    fp32, the activation rounded to bf16 once; the last layer is not rounded.  ``flat`` is the
+    already-perturbed fp32 row."""
     h = round_bf16(np.asarray(obs, dtype=np.float32))
     layers = mlp_unflatten(np.asarray(flat, dtype=np.float32), dims)
     for li, (w, b) in enumerate(layers):
         z = (h.astype(np.float64) @ round_bf16(w).astype(np.float64).T).astype(np.float32) + b
         if li + 1 < len(layers):
-            h = round_bf16(np.maximum(z, np.float32(0.0)))
+            h = round_bf16(HIDDEN[hidden](z))
         else:
             h = z.astype(np.float32)
-    return h
+    return _output(h, output)
 
 
 def round_f16(x: np.ndarray) -> np.ndarray:
@@ -219,11 +249,12 @@ def round_f16(x: np.ndarray) -> np.ndarray:
     return np.clip(np.asarray(x, dtype=np.float32), -65504.0, 65504.0).astype(np.float16).astype(np.float32)
 
 
-def mlp_forward_f16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> np.ndarray:
-    """Emulation of the roundings of estk_eval_mlp with ESTK_PREC_F16 (test infrastructure for the kernel's
-    own arithmetic; parity proper is against mlp_forward): weights and hidden activations
-    rounded to fp16, the observation split x_hi + x_lo, fp32 (here fp64) accumulation,
-    fp32 bias."""
+def mlp_forward_f16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray, hidden: str = "relu",
+                    output: str = "identity") -> np.ndarray:
+    """Emulation of the roundings of estk_eval_mlp with ESTK_PREC_F16 / F16_ANY (test infrastructure
+    for the kernel's own arithmetic; parity proper is against mlp_forward): weights rounded to fp16,
+    the observation split x_hi + x_lo, fp32 (here fp64) accumulation, fp32 bias, the fp32 hidden
+    activation rounded to fp16 once."""
     x = np.asarray(obs, dtype=np.float32)
     x_hi = round_f16(x)
     h = x_hi.astype(np.float64) + round_f16(x - x_hi).astype(np.float64)
@@ -231,8 +262,8 @@ def mlp_forward_f16(flat: np.ndarray, dims: Sequence[int], obs: np.ndarray) -> n
     for i, (w, b) in enumerate(layers):
         h = (h @ round_f16(w).astype(np.float64).T + b.astype(np.float64)).astype(np.float32)
         if i + 1 < len(layers):
-            h = round_f16(np.maximum(h, 0.0)).astype(np.float64)
-    return h.astype(np.float32)
+            h = round_f16(HIDDEN[hidden](h)).astype(np.float64)
+    return _output(h.astype(np.float32), output)
 
 
 def synthetic_return(out: np.ndarray, target: np.ndarray) -> np.float32:

@@ -11,14 +11,15 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import estorch_b200 as E  # noqa: E402
-from _batch_oracle import BatchOracleBackend, dataset  # noqa: E402
-from _xent_oracle import MLP  # noqa: E402
+from _batch_oracle import dataset  # noqa: E402
+from _mlp_oracle import MLP  # noqa: E402
+from _oracle_backend import OracleBackend  # noqa: E402
 
 
 def run():
     x, y = dataset(45, 4, 3, seed=12)
     torch.manual_seed(31)
-    be = BatchOracleBackend()
+    be = OracleBackend()
     es = E.ES(MLP, E.DeviceAgent, torch.optim.Adam, population_size=16, sigma=0.05,
               policy_kwargs={"dims": [4, 8, 3]}, agent_kwargs=dict(obs=x, target=y, batch_size=10, batch_seed=6),
               optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, noise_seed=5, _backend=be)

@@ -11,13 +11,14 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import estorch_b200 as E  # noqa: E402
-from _cnn_oracle import CnnOracleBackend, image_task, pack, policy_class  # noqa: E402
+from _cnn_oracle import image_task, pack, policy_class  # noqa: E402
+from _oracle_backend import OracleBackend  # noqa: E402
 
 
 def run():
     obs, tgt = image_task(6, (1, 12, 12), seed=2)
     torch.manual_seed(31)
-    be = CnnOracleBackend()
+    be = OracleBackend()
     es = E.ES(policy_class(2, "elu", True), E.DeviceAgent, torch.optim.Adam, population_size=16, sigma=0.05,
               policy_kwargs={"dims": pack((1, 12, 12), [(4, 3, 2, 1), (6, 3, 2, 0)], [8, 4])},
               agent_kwargs=dict(obs=obs, target=tgt - 0.5), optimizer_kwargs={"lr": 0.02},

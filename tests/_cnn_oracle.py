@@ -1,6 +1,5 @@
 """TEST-ONLY: the convolutional evaluate (estk_eval_mlp with n_conv in bits 24-31, include/estk.h) in numpy -- an
-fp32 forward and a float64 forward of a member's weights --, ``policy_class`` builders for the test shapes, and an
-oracle stand-in backend with ``eval_cnn`` / ``eval_cnn_center`` so the host logic runs without a GPU.
+fp32 forward and a float64 forward of a member's weights --, and ``policy_class`` builders for the test shapes.
 
 A policy is described by its packed ``dims`` (``CNNSpec.dims``: ESTK_CNN_INPUT, one ESTK_CNN_CONV per conv, the
 Linear widths) and its code (hidden | output | n_conv << 24), exactly what the library is handed."""
@@ -8,8 +7,6 @@ import numpy as np
 import torch
 from torch import nn
 
-from oracle import es_oracle as orc
-from _oracle_backend import OracleBackend, _np
 
 LOSS_XENT = 1 << 16
 HIDDEN = {0: "relu", 1: "tanh", 3: "elu", 4: "silu", 5: "leaky_relu"}
@@ -155,42 +152,6 @@ def policy_class(n_conv, hidden="relu", out_tanh=False, form="sequential"):
                     h = fn(h)
             return torch.tanh(h) if out_tanh else h
     return CNNPolicy
-
-
-class CnnOracleBackend(OracleBackend):
-    """OracleBackend plus ``eval_cnn`` / ``eval_cnn_center`` (CudaBackend's signatures), computed by ``forward``
-    (fp32) and ``returns_of``; counts its calls in ``cnn_calls``."""
-
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
-        self.cnn_calls = 0
-
-    def eval_cnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
-                 bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
-        assert precision == "fp32" and (act >> 24) & 0xff
-        self.cnn_calls += 1
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        y = np.stack([forward(r, dims, act, _np(obs)) for r in rows])
-        rets = returns_of(y, _np(target), bool(act & LOSS_XENT))
-        bcs = y[:, :bc_obs].reshape(len(rows), -1)[:, :bc_dim]
-        if offsets is None:
-            ret_plus[0] = float(rets[0])
-            if bc_plus is not None:
-                bc_plus.copy_(torch.from_numpy(bcs[0].copy()))
-            return
-        ret_plus.copy_(torch.from_numpy(rets[:pairs]))
-        ret_minus.copy_(torch.from_numpy(rets[pairs:]))
-        if bc_plus is not None:
-            bc_plus.copy_(torch.from_numpy(bcs[:pairs].copy()))
-            bc_minus.copy_(torch.from_numpy(bcs[pairs:].copy()))
-
-    def eval_cnn_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
-                        precision="fp32", act=0):
-        self.eval_cnn(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
-                      bc_dim, precision=precision, act=act)
 
 
 def image_task(B, shape=(1, 12, 12), n_classes=4, seed=0):

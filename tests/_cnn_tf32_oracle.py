@@ -1,13 +1,9 @@
 """TEST-ONLY: the TF32 convolutional evaluate (include/estk_eval_cnn_tf32.h) restated in numpy -- ``rna_tf32``
 (round to nearest, ties away from zero, to an 11-bit significand), the forward of a member's formed fp32 weights
-with every weight and every layer input rounded that way and float64 sums -- and a stand-in backend that serves
-``precision="tf32"`` with it, so the engine's mode selection runs without a GPU."""
+with every weight and every layer input rounded that way and float64 sums."""
 import numpy as np
-import torch
 
-from oracle import es_oracle as orc
-from _cnn_oracle import HIDDEN, LOSS_XENT, CnnOracleBackend, _act, layer_shapes, unpack
-from _oracle_backend import _np
+from _cnn_oracle import HIDDEN, LOSS_XENT, _act, layer_shapes, unpack
 
 LOSS_ACCURACY = 6 << 16
 
@@ -143,42 +139,3 @@ def returns64(y, target, code):
         lse = m[..., 0] + np.log(np.exp(y - m).sum(-1))
         return -(lse * tg.sum(-1)[None] - (tg[None] * y).sum(-1)).mean(1)
     return -((y - tg[None]) ** 2).mean((1, 2))
-
-
-class Tf32CnnOracleBackend(CnnOracleBackend):
-    """CnnOracleBackend plus ``precision="tf32"`` (forward_tf32, the returns rounded to fp32) and
-    ``eval_supports_tf32_cnn``; records the precision of every convolutional evaluate in ``cnn_precisions``."""
-
-    def __init__(self, *a, tf32_supported=True, **k):
-        super().__init__(*a, **k)
-        self.cnn_precisions = []
-        self.tf32_supported = tf32_supported
-
-    def eval_supports_tf32_cnn(self, dims, B, act=0):
-        return self.tf32_supported
-
-    def eval_cnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
-                 bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
-        self.cnn_precisions.append(precision)
-        if precision != "tf32":
-            return super().eval_cnn(dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus,
-                                    ret_minus, bc_plus, bc_minus, bc_obs, bc_dim, precision=precision, act=act)
-        assert (act >> 24) & 0xff
-        self.cnn_calls += 1
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        y = np.stack([forward_tf32(r, dims, act, _np(obs)) for r in rows])
-        rets = returns64(y, _np(target), act).astype(np.float32)
-        bcs = y[:, :bc_obs].reshape(len(rows), -1)[:, :bc_dim].astype(np.float32)
-        if offsets is None:
-            ret_plus[0] = float(rets[0])
-            if bc_plus is not None:
-                bc_plus.copy_(torch.from_numpy(bcs[0].copy()))
-            return
-        ret_plus.copy_(torch.from_numpy(rets[:pairs]))
-        ret_minus.copy_(torch.from_numpy(rets[pairs:]))
-        if bc_plus is not None:
-            bc_plus.copy_(torch.from_numpy(bcs[:pairs].copy()))
-            bc_minus.copy_(torch.from_numpy(bcs[pairs:].copy()))

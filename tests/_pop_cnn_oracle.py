@@ -1,16 +1,8 @@
-"""TEST-ONLY: population mode of a generic convolutional policy (estk_act_cnn, include/estk_act_cnn.h) without a
-GPU -- an oracle stand-in backend whose ``act_cnn`` runs ``_cnn_oracle.forward`` (fp32) on each member's own
-images --, the small pixel agent of the CPU tests and the goldens, and the goldens' policy shapes.
-
-The oracle's convolutions are fp32 matrix products, so it agrees with the kernel to fp32 accumulation order,
-not bit for bit."""
-import numpy as np
+"""TEST-ONLY: population mode of a generic convolutional policy (estk_act_cnn, include/estk_act_cnn.h): the small
+pixel agent of the CPU tests and the goldens, and the goldens' policy shapes."""
 import torch
 
-from oracle import es_oracle as orc
-from _cnn_oracle import pack, param_count, forward, policy_class
-from _oracle_backend import _np
-from _pop_oracle import PopOracleBackend
+from _cnn_oracle import pack, param_count, policy_class
 from estorch_b200 import PopulationAgent
 
 ACTIONS = 3 << 16        # include/estk.h ESTK_ACTIONS
@@ -25,26 +17,6 @@ NSR_POLICY = dict(n_conv=2, hidden="elu", out_tanh=False)     # nsr_pop_cnn_p8.n
 def cnn_policy(n_conv, hidden, out_tanh):
     """The policy class (``__init__(dims)``, an ``nn.Sequential`` with ``nn.Flatten``) of a golden."""
     return policy_class(n_conv, hidden, out_tanh)
-
-
-class PopCnnOracleBackend(PopOracleBackend):
-    """PopOracleBackend plus ``act_cnn`` (CudaBackend's signature); counts its calls in ``cnn_act_calls``."""
-
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
-        self.cnn_act_calls = 0
-
-    def act_cnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act):
-        self.cnn_act_calls += 1
-        assert (int(act) >> 24) & 0xff and not int(act) & (0xff << 16)
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        x = _np(obs)
-        assert x.ndim == 5 and x.shape[0] == rows.shape[0] and tuple(out.shape) == (rows.shape[0], x.shape[1],
-                                                                                    int(dims[-1]))
-        out.copy_(torch.from_numpy(np.stack([forward(r, dims, act, xm) for r, xm in zip(rows, x)])))
 
 
 class PixelPoint(PopulationAgent):

@@ -1,5 +1,5 @@
-"""TEST-ONLY: the action mode of estk_eval_conv_vbn (ESTK_ACTIONS) in numpy, an oracle stand-in backend that
-serves it, the Atari-example policy, and the deterministic pixel agent of the conv population tests and goldens.
+"""TEST-ONLY: the action mode of estk_eval_conv_vbn (ESTK_ACTIONS) in numpy, the Atari-example policy, and the
+deterministic pixel agent of the conv population tests and goldens.
 
 The oracle keeps the VirtualBatchNorm statistics as the kernels do (a = gamma / sqrt(var + 1e-5) and the
 mean per (C, H, W) position, normalising as (y - mean) * a + beta; mean and unbiased var over the reference
@@ -10,8 +10,6 @@ import torch
 from numpy.lib.stride_tricks import sliding_window_view
 
 from oracle import es_oracle as orc
-from _oracle_backend import _np
-from _pop_oracle import PopOracleBackend
 from estorch_b200 import PopulationAgent, VirtualBatchNorm
 
 STATS_FLOATS = 17984        # include/estk.h ESTK_CONV_VBN_STATS_FLOATS
@@ -100,34 +98,6 @@ def conv_act(rows, n_actions, stats, obs):
     h = h.reshape(M, h.shape[1], 2592)
     h = np.maximum(np.matmul(h, p["fc1.w"].transpose(0, 2, 1)) + p["fc1.b"][:, None], 0).astype(f32)
     return (np.matmul(h, p["fc2.w"].transpose(0, 2, 1)) + p["fc2.b"][:, None]).astype(f32)
-
-
-class PopConvOracleBackend(PopOracleBackend):
-    """PopOracleBackend plus ``act_conv_vbn`` (CudaBackend's signature); counts its stats and act launches."""
-
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
-        self.stats_calls = 0
-        self.conv_act_calls = 0
-
-    def act_conv_vbn(self, n_actions, theta, table, offsets, order, pairs, sigma, xref, obs, out, stats,
-                     table16=None):
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            if table16 is not None:
-                assert table16.dtype == torch.float16
-                table = table16.float()
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        assert tuple(stats.shape) == (rows.shape[0], STATS_FLOATS)
-        if xref is not None:
-            self.stats_calls += 1
-            stats.copy_(torch.from_numpy(conv_stats(rows, int(n_actions), _np(xref))))
-        if obs is not None:
-            self.conv_act_calls += 1
-            assert tuple(obs.shape) == (rows.shape[0], obs.shape[1], 4, 84, 84)
-            assert tuple(out.shape) == (rows.shape[0], obs.shape[1], int(n_actions))
-            out.copy_(torch.from_numpy(conv_act(rows, int(n_actions), _np(stats), _np(obs))))
 
 
 class PixelWalker(PopulationAgent):

@@ -1,7 +1,6 @@
 """TEST-ONLY: one step of estk_eval_mlp with a recurrent cell code (ESTK_CELL_GRU / ESTK_CELL_LSTM and
-ESTK_ACTIONS) in numpy -- an fp32 restatement and a float64 forward --, the recurrent policy module, an oracle
-stand-in backend that serves the step, and a deterministic recall task for the population-mode tests and
-goldens.
+ESTK_ACTIONS) in numpy -- an fp32 restatement and a float64 forward --, the recurrent policy module, and a
+deterministic recall task for the population-mode tests and goldens.
 
 Rounding model of the kernel (estorch_b200/csrc/estk_act_rnn.cu, stated in include/estk.h):
 W = theta +- (sigma*t) with two fp32 roundings; per gate row two fma chains from 0 in ascending k (x against
@@ -13,9 +12,6 @@ ulp per operation rather than bit for bit."""
 import numpy as np
 import torch
 
-from oracle import es_oracle as orc
-from _oracle_backend import _np
-from _pop_oracle import PopOracleBackend
 from estorch_b200 import PopulationAgent
 
 ACTIONS = 3 << 16            # include/estk.h ESTK_ACTIONS
@@ -160,27 +156,6 @@ def forward64(rows, cell, dims, xs, out_tanh):
 
 def cell_of(code):
     return {CELL_GRU: "gru", CELL_LSTM: "lstm"}[code & 0xff]
-
-
-class RnnOracleBackend(PopOracleBackend):
-    """PopOracleBackend plus ``act_rnn`` (CudaBackend's signature), computed by ``step32``; counts its calls in
-    ``act_calls``."""
-
-    def act_rnn(self, dims, theta, table, offsets, order, pairs, sigma, obs, out, act, table16=None):
-        self.act_calls += 1
-        dims = [int(d) for d in dims]
-        cell = cell_of(act)
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            if table16 is not None:
-                assert table16.dtype == torch.float16
-                table = table16.float()
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        S = state_width(cell, dims[1])
-        assert tuple(obs.shape) == (rows.shape[0], obs.shape[1], dims[0] + S)
-        assert tuple(out.shape) == (rows.shape[0], obs.shape[1], dims[2] + S)
-        out.copy_(torch.from_numpy(step32(rows, cell, dims, _np(obs), bool(act & OUT_TANH))))
 
 
 class RecallAgent(PopulationAgent):

@@ -12,14 +12,14 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import estorch_b200 as E  # noqa: E402
 from _rnn_oracle import policy_class  # noqa: E402
-from _seq_oracle import SeqOracleBackend  # noqa: E402
+from _oracle_backend import OracleBackend  # noqa: E402
 
 
 def run():
     g = torch.Generator().manual_seed(9)
     obs, tgt = torch.randn(5, 4, 3, generator=g), torch.rand(5, 4, 2, generator=g) - 0.5
     torch.manual_seed(31)
-    be = SeqOracleBackend()
+    be = OracleBackend()
     es = E.ES(policy_class("gru", True), E.SequenceAgent, torch.optim.Adam, population_size=16, sigma=0.05,
               policy_kwargs={"dims": (3, 8, 2)}, agent_kwargs=dict(obs=obs, target=tgt),
               optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, noise_seed=5, _backend=be)

@@ -1,13 +1,10 @@
 """TEST-ONLY: the recurrent sequence evaluate (estk_eval_mlp with ESTK_CELL_GRU / ESTK_CELL_LSTM and a return,
 include/estk.h) in numpy -- T chained ``_rnn_oracle.step32`` steps, the fp32 restatement of the documented loss
-reduction and a float64 forward --, an oracle stand-in backend that serves it, and the supervised delayed-recall
-dataset of the sequence tests and goldens."""
+reduction and a float64 forward --, and the supervised delayed-recall dataset of the sequence tests and goldens."""
 import numpy as np
 import torch
 
-from oracle import es_oracle as orc
-from _oracle_backend import _np
-from _rnn_oracle import RnnOracleBackend, cell_of, forward64, state_width, step32
+from _rnn_oracle import forward64, state_width, step32
 
 LOSS_XENT = 1 << 16          # include/estk.h ESTK_LOSS_XENT
 
@@ -87,45 +84,6 @@ def seq_returns64(y, target, xent):
         lsm = y - m - np.log(np.exp(y - m).sum(-1, keepdims=True))
         return (tg[None] * lsm).sum(-1).mean((1, 2))
     return -((y - tg[None]) ** 2).mean((1, 2, 3))
-
-
-class SeqOracleBackend(RnnOracleBackend):
-    """RnnOracleBackend plus ``eval_rnn_seq`` / ``eval_rnn_seq_center`` (CudaBackend's signatures), computed by
-    ``seq_outputs32`` and ``seq_returns32``; counts its calls in ``seq_calls``."""
-
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
-        self.seq_calls = 0
-
-    def eval_rnn_seq(self, dims, theta, table, offsets, order, pairs, sigma, obs, target, ret_plus, ret_minus,
-                     bc_plus=None, bc_minus=None, bc_obs=0, bc_dim=0, precision="fp32", act=0):
-        assert precision == "fp32"
-        self.seq_calls += 1
-        dims = [int(d) for d in dims]
-        if offsets is None:
-            rows = _np(theta)[None, :]
-        else:
-            rows, _ = orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)
-        B, T = obs.shape[:2]
-        assert tuple(obs.shape) == (B, T, dims[0]) and tuple(target.shape) == (B, T, dims[2])
-        y = seq_outputs32(rows, cell_of(act), dims, _np(obs), bool(act & 0x100))
-        rets = seq_returns32(y, _np(target), bool(act & LOSS_XENT))
-        bcs = y[:, :bc_obs].reshape(len(rows), -1)[:, :bc_dim]
-        if offsets is None:
-            ret_plus[0] = float(rets[0])
-            if bc_plus is not None:
-                bc_plus.copy_(torch.from_numpy(bcs[0].copy()))
-            return
-        ret_plus.copy_(torch.from_numpy(rets[:pairs]))
-        ret_minus.copy_(torch.from_numpy(rets[pairs:]))
-        if bc_plus is not None:
-            bc_plus.copy_(torch.from_numpy(bcs[:pairs].copy()))
-            bc_minus.copy_(torch.from_numpy(bcs[pairs:].copy()))
-
-    def eval_rnn_seq_center(self, dims, theta, obs, target, ret_out, bc_out=None, bc_obs=0, bc_dim=0,
-                            precision="fp32", act=0):
-        self.eval_rnn_seq(dims, theta, None, None, None, 1, 0.0, obs, target, ret_out, None, bc_out, None, bc_obs,
-                          bc_dim, precision=precision, act=act)
 
 
 def recall_dataset(n_cues=3, delay=4, copies=1):

@@ -1,7 +1,7 @@
 """Classification accuracy as the return, without a GPU: ``DeviceAgent(loss="accuracy")``, the ESTK_LOSS_ACCURACY
 code of ``estk_mlp_desc.activation`` in the header, the binding and the library's shape query, the fused / hooks
 decision and the precision it picks, the tie and NaN rule of the restated return against ``torch.argmax``, and ES /
-NSR-ES through the oracle stand-in (tests/_accuracy_oracle.py) against the reference-generated goldens."""
+NSR-ES through the oracle stand-in (tests/_oracle_backend.py) against the reference-generated goldens."""
 import ctypes as C
 import os
 import re
@@ -12,11 +12,10 @@ import torch
 import torch.nn.functional as F
 
 from conftest import load_golden
-import _accuracy_oracle as ao
-from _accuracy_oracle import AccuracyOracleBackend
-from _act_ext_oracle import MLP
-from _batch_oracle import with_batches
-from _cnn_oracle import CnnOracleBackend, image_task, pack, policy_class as cnn_policy_class
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
+from _oracle_backend import OracleBackend
+from _cnn_oracle import image_task, pack, policy_class as cnn_policy_class
 import estorch_b200 as E
 from estorch_b200 import _capi
 from estorch_b200.batches import batch_indices
@@ -47,16 +46,16 @@ def test_ties_and_nans_follow_torch_argmax():
                       [-1.0, -1.0, -2.0, -1.0]])
     t = F.one_hot(torch.tensor([1, 1, 0, 0, 0, 2, 0]), 4).float()
     assert np.array_equal(np.argmax(y.numpy(), 1), y.argmax(1).numpy())
-    assert np.array_equal(ao.correct_rows(y.numpy(), t.numpy()), (y.argmax(1) == t.argmax(1)).numpy())
-    assert ao.correct_rows(y.numpy(), t.numpy()).tolist() == [True, True, True, True, True, True, True]
+    assert np.array_equal(mlp.correct_rows(y.numpy(), t.numpy()), (y.argmax(1) == t.argmax(1)).numpy())
+    assert mlp.correct_rows(y.numpy(), t.numpy()).tolist() == [True, True, True, True, True, True, True]
     soft = torch.tensor([[0.25, 0.25, 0.5, 0.0]] * 7)  # a soft target's label is its first largest weight
-    assert ao.accuracy_return(y.numpy(), soft.numpy()) == np.float32(np.float32(1) / np.float32(7))   # row 5 only
+    assert mlp.accuracy_return(y.numpy(), soft.numpy()) == np.float32(np.float32(1) / np.float32(7))   # row 5 only
     pol = torch.nn.Identity()
     pol.register_parameter("p", torch.nn.Parameter(torch.zeros(1)))
     for tgt in (t, soft):
         r = E.DeviceAgent(torch.zeros(7, 4), tgt, loss="accuracy")
         r.obs = y                                     # the logits themselves through an identity policy
-        assert r.rollout(pol) == float(ao.accuracy_return(y.numpy(), tgt.numpy()))
+        assert r.rollout(pol) == float(mlp.accuracy_return(y.numpy(), tgt.numpy()))
 
 
 def test_rollout_is_the_fraction_of_correct_rows_and_bc_the_logits():
@@ -100,7 +99,7 @@ def test_sequence_agent_refuses_the_accuracy():
 def test_header_and_binding_agree():
     header = open(os.path.join(ROOT, "include", "estk.h")).read()
     m = re.search(r"#define\s+ESTK_LOSS_ACCURACY\s+\((\d+) << 16\)", header)
-    assert m and int(m.group(1)) << 16 == _capi.ESTK_LOSS_ACCURACY == ao.LOSS_ACCURACY == 0x60000
+    assert m and int(m.group(1)) << 16 == _capi.ESTK_LOSS_ACCURACY == mlp.LOSS_ACCURACY == 0x60000
     assert _capi.ESTK_LOSS_ACCURACY & _capi.ESTK_LOSS_XENT == 0     # bit 16 clear: never read as the cross-entropy
     assert re.search(r"#define\s+ESTK_VERSION\s+200\b", header)
 
@@ -141,7 +140,7 @@ def _es(hidden="relu", output="identity", tensor_core=False, dims=None, B=None, 
     rng = np.random.RandomState(3)
     obs = torch.from_numpy(rng.standard_normal((B, dims[0])).astype(np.float32))
     tgt = torch.from_numpy(rng.dirichlet(np.ones(dims[-1]), B).astype(np.float32))
-    be = backend or AccuracyOracleBackend(tensor_core=tensor_core)
+    be = backend or OracleBackend(tensor_core=tensor_core)
     es = E.ES(MLP, E.DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               policy_kwargs={"dims": dims, "hidden": hidden, "output": output},
               agent_kwargs=dict(obs=obs, target=tgt, loss="accuracy", **agent_kw), optimizer_kwargs={"lr": 0.01},
@@ -153,7 +152,7 @@ def _es(hidden="relu", output="identity", tensor_core=False, dims=None, B=None, 
 @pytest.mark.parametrize("hidden", ["relu", "tanh", "elu", "silu", "leaky_relu"])
 def test_identity_output_is_fused_and_tanh_output_is_hooks(hidden):
     es = _es(hidden)[0]
-    assert es._fused and es._act_code() == ao.LOSS_ACCURACY | \
+    assert es._fused and es._act_code() == mlp.LOSS_ACCURACY | \
         {"relu": 0, "tanh": 1, "elu": 3, "silu": 4, "leaky_relu": 5}[hidden]
     assert not _es(hidden, "tanh")[0]._fused
 
@@ -166,7 +165,7 @@ def test_the_conv_vbn_policy_runs_in_hooks_mode():
               policy_kwargs=dict(n_actions=4, xref=xref), optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 20,
               agent_kwargs=dict(obs=torch.rand(2, 4, 84, 84, generator=g),
                                 target=F.one_hot(torch.tensor([0, 3]), 4).float(), loss="accuracy"),
-              _backend=AccuracyOracleBackend())
+              _backend=OracleBackend())
     assert es._is_conv and not es._fused
 
 
@@ -183,7 +182,7 @@ def test_precision_follows_the_cross_entropy_and_the_code_reaches_the_backend(te
     es, be, obs, tgt = _es("silu", tensor_core=tensor_core, dims=dims, B=B, precision=precision)
     assert es._precision == want
     es.train(n_steps=2)
-    assert be.acts == {ao.LOSS_ACCURACY | 4}
+    assert be.acts == {mlp.LOSS_ACCURACY | 4}
     with torch.no_grad():
         exact = float((es.policy(obs).argmax(1) == tgt.argmax(1)).float().mean())
     # the post-update rollout in the selected precision: within one or two rows of the fp32 torch forward
@@ -193,13 +192,13 @@ def test_precision_follows_the_cross_entropy_and_the_code_reaches_the_backend(te
 def test_a_cnn_classifier_is_fused_with_the_accuracy_code():
     x, y = image_task(24, (1, 12, 12), seed=2)
     dims = pack((1, 12, 12), [(4, 3, 2, 1), (6, 3, 2, 0)], [8, 4])
-    be = CnnOracleBackend()
+    be = OracleBackend()
     seen = []
     orig = be.eval_cnn
 
     def eval_cnn(*a, act=0, **k):
         seen.append(act)
-        if (act & 0xff0000) == ao.LOSS_ACCURACY:       # the stand-in's forward with the accuracy return
+        if (act & 0xff0000) == mlp.LOSS_ACCURACY:       # the stand-in's forward with the accuracy return
             return _cnn_accuracy(orig, *a, act=act, **k)
         return orig(*a, act=act, **k)
     be.eval_cnn = eval_cnn
@@ -207,9 +206,9 @@ def test_a_cnn_classifier_is_fused_with_the_accuracy_code():
               policy_kwargs={"dims": dims}, agent_kwargs=dict(obs=x, target=y, loss="accuracy"),
               optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 14, _backend=be)
     es.log = lambda: None
-    assert es._fused and es._is_cnn and es._act_code() == 2 << 24 | ao.LOSS_ACCURACY
+    assert es._fused and es._is_cnn and es._act_code() == 2 << 24 | mlp.LOSS_ACCURACY
     es.train(n_steps=2)
-    assert set(seen) == {2 << 24 | ao.LOSS_ACCURACY}
+    assert set(seen) == {2 << 24 | mlp.LOSS_ACCURACY}
     with torch.no_grad():
         assert es.episode_reward == float((es.policy(x).argmax(1) == y.argmax(1)).float().mean())
 
@@ -221,7 +220,7 @@ def _cnn_accuracy(orig, dims, theta, table, offsets, order, pairs, sigma, obs, t
     from _oracle_backend import _np
     rows = _np(theta)[None, :] if offsets is None else \
         orc.sample_population(_np(theta), _np(table), _np(offsets), sigma)[0]
-    rets = np.array([ao.accuracy_return(forward(r, dims, act & ~0xff0000, _np(obs)), _np(target)) for r in rows])
+    rets = np.array([mlp.accuracy_return(forward(r, dims, act & ~0xff0000, _np(obs)), _np(target)) for r in rows])
     if offsets is None:
         ret_plus[0] = float(rets[0])
         return
@@ -249,7 +248,8 @@ def test_the_stand_in_reproduces_every_golden_return(name):
     bc_obs, bc_dim = int(g["bc_obs"]), int(g["bc_dim"])
     for gen in range(len(g["returns"])):
         pop, _ = orc.sample_population(g["theta_before"][gen], g["table"], g["offsets"][gen], np.float32(g["sigma"]))
-        rets, bcs = ao.evaluate_population(pop, dims, g["obs"], g["target"], bc_obs, bc_dim)
+        rets, bcs = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.LOSS_ACCURACY, bc_obs=bc_obs,
+                                            bc_dim=bc_dim)
         np.testing.assert_array_equal(rets, g["returns"][gen][:, 0])
         if bc_dim:
             np.testing.assert_allclose(bcs, _bcs_of(g, gen, pop, dims), rtol=1e-5, atol=1e-6)
@@ -280,7 +280,7 @@ def test_es_accuracy_first_generation_matches_the_reference_golden(mode):
     es = E.ES(MLP, agent, torch.optim.Adam, population_size=64, sigma=0.1,
               policy_kwargs={"dims": dims, "hidden": "relu"},
               agent_kwargs=akw, optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]),
-              noise_seed=int(g["noise_seed"]), _backend=AccuracyOracleBackend())
+              noise_seed=int(g["noise_seed"]), _backend=OracleBackend())
     rec = []
     es.log = lambda: rec.append(es.population_returns.copy())
     assert es._fused == (mode == "fused")
@@ -305,7 +305,7 @@ def _train(agent_cls, obs, tgt, n, seed=1, backend=None, **akw):
     es = E.ES(MLP, agent_cls, torch.optim.Adam, population_size=16, sigma=0.1,
               policy_kwargs={"dims": [obs.shape[1], 12, tgt.shape[1]], "hidden": "relu"},
               agent_kwargs=dict(obs=obs, target=tgt, **akw), optimizer_kwargs={"lr": 0.05},
-              noise_table_size=1 << 14, noise_seed=7, _backend=backend or AccuracyOracleBackend())
+              noise_table_size=1 << 14, noise_seed=7, _backend=backend or OracleBackend())
     rec = []
     es.log = lambda: rec.append((es.population_returns.copy(), float(es.episode_reward)))
     es.train(n_steps=n)
@@ -335,7 +335,7 @@ def test_checkpoint_resume_is_bit_identical():
     c = E.ES(MLP, E.DeviceAgent, torch.optim.Adam, population_size=16, sigma=0.1,
              policy_kwargs={"dims": [5, 12, 4], "hidden": "relu"},
              agent_kwargs=dict(obs=obs, target=tgt, loss="accuracy"), optimizer_kwargs={"lr": 0.05},
-             noise_table_size=1 << 14, noise_seed=7, _backend=AccuracyOracleBackend())
+             noise_table_size=1 << 14, noise_seed=7, _backend=OracleBackend())
     c.load_state_dict(sd)
     c_rec = []
     c.log = lambda: c_rec.append((c.population_returns.copy(), float(c.episode_reward)))
@@ -352,16 +352,16 @@ def test_minibatches_with_the_accuracy():
     """batch_size with loss="accuracy": fused, the accuracy code reaches the sampled evaluate, and generation g's
     returns score batch g (the same as hooks mode, which rolls out batch g on the host)."""
     obs, tgt = _pair(B=45, seed=8)
-    be = with_batches(AccuracyOracleBackend)()
+    be = OracleBackend()
     fused, a = _train(E.DeviceAgent, obs, tgt, 3, backend=be, loss="accuracy", batch_size=10, batch_seed=3)
-    assert fused._fused and fused._sampling and be.acts == {ao.LOSS_ACCURACY}
+    assert fused._fused and fused._sampling and be.acts == {mlp.LOSS_ACCURACY}
 
     torch.manual_seed(1)
     hooks = E.ES(MLP, E.DeviceAgent, torch.optim.SGD, population_size=16, sigma=0.1,     # SGD: hooks mode
                  policy_kwargs={"dims": [5, 12, 4], "hidden": "relu"},
                  agent_kwargs=dict(obs=obs, target=tgt, loss="accuracy", batch_size=10, batch_seed=3),
                  optimizer_kwargs={"lr": 0.05}, noise_table_size=1 << 14, noise_seed=7,
-                 _backend=AccuracyOracleBackend())
+                 _backend=OracleBackend())
     assert not hooks._fused
     # generation 0's returns: the same initial theta and noise, the same batch 0
     rec = []

@@ -12,12 +12,12 @@ import torch
 
 from conftest import load_golden
 from oracle import es_oracle as orc
-import _accuracy_oracle as ao
+import _mlp_oracle as mlp
 from _cnn_oracle import pack, param_count as cnn_param_count
 from test_eval_mlp_act_gpu import _eval, _tc_problem, dev
 
 pytestmark = pytest.mark.gpu
-ACC = ao.LOSS_ACCURACY
+ACC = mlp.LOSS_ACCURACY
 HIDDEN = (0, 1, 3, 4, 5)                       # ReLU, Tanh, ELU, SiLU, LeakyReLU
 
 
@@ -214,7 +214,8 @@ def test_goldens_on_the_device(be):
                             g["obs"], g["target"], ACC, int(g["bc_obs"]), int(g["bc_dim"]))
         np.testing.assert_array_equal(ret, g["returns"][gen][:, 0])
         pop, _ = orc.sample_population(g["theta_before"][gen], g["table"], g["offsets"][gen], np.float32(g["sigma"]))
-        _, want_bc = ao.evaluate_population(pop, dims, g["obs"], g["target"], int(g["bc_obs"]), int(g["bc_dim"]))
+        _, want_bc = mlp.evaluate_population(pop, dims, g["obs"], g["target"], ACC, bc_obs=int(g["bc_obs"]),
+                                             bc_dim=int(g["bc_dim"]))
         np.testing.assert_allclose(bcs, want_bc, rtol=1e-5, atol=1e-6)
 
 

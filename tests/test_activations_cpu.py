@@ -1,6 +1,6 @@
 """Tanh MLP policies on the CPU: recognition (estorch_b200.policy_spec), the activation-aware
 oracle forward against the reference-generated Tanh goldens, and the fused generation of the
-ES / NSR-ES classes through the oracle stand-in (tests/_act_oracle.py) against the same goldens."""
+ES / NSR-ES classes through the oracle stand-in (tests/_oracle_backend.py) against the same goldens."""
 import numpy as np
 import pytest
 import torch
@@ -8,8 +8,8 @@ from torch import nn
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _act_oracle as act
-from _act_oracle import ActOracleBackend
+import _mlp_oracle as mlp
+from _oracle_backend import OracleBackend
 import estorch_b200 as E
 from estorch_b200.policy_spec import MLPSpec, mlp_spec_from_module
 
@@ -39,7 +39,7 @@ class ActMLP(nn.Module):
 def test_recognition_of_registered_activations(hidden, output):
     spec = mlp_spec_from_module(ActMLP([4, 64, 64, 2], hidden, output))
     assert spec == MLPSpec((4, 64, 64, 2), hidden, output)
-    assert spec.act == act.code(hidden, output)
+    assert spec.act == mlp.code(hidden, output)
     assert spec.n_parameters == 4610
 
 
@@ -102,12 +102,12 @@ def test_oracle_tanh_forward_matches_reference_golden_es():
     dims, sigma = [int(d) for d in g["dims"]], float(g["sigma"])
     for gen in range(len(g["grad"])):
         pop, _ = orc.sample_population(g["theta_before"][gen], g["table"], g["offsets"][gen], sigma)
-        rets, _ = act.evaluate_population(pop, dims, g["obs"], g["target"], hidden="tanh")
+        rets, _ = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.ACT_TANH)
         assert rel_err(rets, g["returns"][gen][:, 0]) < 2e-6
-        ep = orc.synthetic_return(act.mlp_forward(g["theta_after"][gen], dims, g["obs"], "tanh"), g["target"])
+        ep = orc.synthetic_return(orc.mlp_forward(g["theta_after"][gen], dims, g["obs"], "tanh"), g["target"])
         assert abs(float(ep) - float(g["episode_reward"][gen])) < 1e-5
     # the default keywords are the ReLU oracle
-    rr, _ = act.evaluate_population(pop[:4], dims, g["obs"], g["target"])
+    rr, _ = mlp.evaluate_population(pop[:4], dims, g["obs"], g["target"])
     np.testing.assert_array_equal(rr, orc.evaluate_population(pop[:4], dims, g["obs"], g["target"])[0])
 
 
@@ -115,13 +115,14 @@ def test_oracle_tanh_forward_matches_reference_golden_nsr_bc():
     g = load_golden("nsr_tanh_bipedal_p32.npz")
     dims, sigma, k = [int(d) for d in g["dims"]], float(g["sigma"]), int(g["k"])
     bc_obs, bc_dim = int(g["bc_obs"]), int(g["bc_dim"])
-    fwd = lambda th: act.mlp_forward(th, dims, g["obs"], "tanh", "tanh")  # noqa: E731
+    fwd = lambda th: orc.mlp_forward(th, dims, g["obs"], "tanh", "tanh")  # noqa: E731
     arch0 = np.stack([orc.synthetic_bc(fwd(th), bc_obs, bc_dim) for th in g["meta_theta0"]])
     np.testing.assert_allclose(arch0, g["archive0"], rtol=1e-5, atol=1e-6)
     archive = list(arch0)
     for gen in range(len(g["grad"])):
         pop, _ = orc.sample_population(g["theta_before"][gen], g["table"], g["offsets"][gen], sigma)
-        rets, bcs = act.evaluate_population(pop, dims, g["obs"], g["target"], bc_obs, bc_dim, "tanh", "tanh")
+        rets, bcs = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.code("tanh", "tanh"), bc_obs=bc_obs,
+                                            bc_dim=bc_dim)
         nov = np.array([orc.novelty(b, np.stack(archive), k) for b in bcs], dtype=np.float32)
         assert rel_err(rets, g["returns"][gen][:, 0]) < 2e-6
         assert rel_err(nov, g["returns"][gen][:, 1]) < 2e-5
@@ -154,7 +155,7 @@ def test_es_fused_tanh_matches_reference_golden():
            policy_kwargs={"dims": dims, "hidden": "tanh"},
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"])),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]),
-           _backend=ActOracleBackend())
+           _backend=OracleBackend())
     es.rec = []
     assert es._fused and es._spec == MLPSpec(tuple(dims), "tanh", "identity")
     es._table.copy_(torch.from_numpy(g["table"]))
@@ -186,9 +187,9 @@ def test_nsr_fused_tanh_matches_reference_golden():
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]), bc_obs=64,
                              bc_dim=256),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]),
-           _backend=ActOracleBackend())
+           _backend=OracleBackend())
     es.rec = []
-    assert es._fused and es._spec.act == act.ACT_TANH | act.ACT_OUT_TANH
+    assert es._fused and es._spec.act == mlp.ACT_TANH | mlp.ACT_OUT_TANH
     es._table.copy_(torch.from_numpy(g["table"]))
     for i, (p, _) in enumerate(es.meta_population):
         _load_theta(p, g["meta_theta0"][i])
@@ -211,7 +212,7 @@ def test_nsr_fused_tanh_matches_reference_golden():
 
 
 # ------------------------------------------------------------------ fused mode for every combination
-class _Spy(ActOracleBackend):
+class _Spy(OracleBackend):
     def __init__(self, **kw):
         super().__init__(**kw)
         self.acts = set()
@@ -239,14 +240,14 @@ def test_fused_for_every_combination_and_the_code_reaches_the_kernels(hidden, ou
               agent_kwargs=dict(obs=obs, target=tgt), optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 16,
               _backend=be)
     es.log = lambda: None
-    assert es._fused and es._spec.act == act.code(hidden, output)
+    assert es._fused and es._spec.act == mlp.code(hidden, output)
     assert es._precision == ("f16" if tensor_core else "fp32")       # "auto" picks f16 where the shape allows
     es.train(n_steps=3)
-    assert be.acts == {act.code(hidden, output)}
+    assert be.acts == {mlp.code(hidden, output)}
     # the trained policy's own forward agrees with the fused episode reward
     with torch.no_grad():
         want = float(-((es.policy(obs) - tgt) ** 2).mean())
-    fwd = act.FORWARD[es._precision]
+    fwd = mlp.FORWARD[es._precision]
     emu = float(orc.synthetic_return(fwd(es._slots[0].theta.numpy(), dims, obs.numpy(), hidden, output), tgt.numpy()))
     assert abs(es.episode_reward - emu) < 1e-6 * abs(emu) + 1e-7
     assert abs(es.episode_reward - want) < (1e-5 if not tensor_core else 1e-4) * abs(want)
@@ -256,5 +257,5 @@ def test_gelu_policy_stays_in_hooks_mode():
     es = E.ES(ActMLP, E.DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               policy_kwargs={"dims": [4, 16, 2], "hidden": "gelu"},
               agent_kwargs=dict(obs=torch.randn(8, 4), target=torch.randn(8, 2)), noise_table_size=1 << 12,
-              _backend=ActOracleBackend())
+              _backend=OracleBackend())
     assert es._spec is None and not es._fused

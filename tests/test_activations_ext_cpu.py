@@ -1,7 +1,7 @@
 """ELU, SiLU and LeakyReLU MLP policies on the CPU: recognition (estorch_b200.policy_spec), the
 activation codes of the C ABI and its support probe, the oracle forwards against the reference-
 generated goldens, and the fused generation of ES / NSR-ES through the oracle stand-in
-(tests/_act_ext_oracle.py) against the same goldens."""
+(tests/_oracle_backend.py) against the same goldens."""
 import ctypes as C
 import os
 import re
@@ -14,14 +14,15 @@ import torch.nn.functional as F
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _act_ext_oracle as ext
-from _act_ext_oracle import MLP, ActExtOracleBackend
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
+from _oracle_backend import OracleBackend
 import estorch_b200 as E
 from estorch_b200 import _capi
 from estorch_b200.policy_spec import MLPSpec, mlp_spec_from_module
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KINDS = ext.NEW_KINDS
+KINDS = mlp.NEW_KINDS
 
 
 # ------------------------------------------------------------------ recognition
@@ -30,7 +31,7 @@ KINDS = ext.NEW_KINDS
 def test_recognition_of_registered_activations(hidden, output):
     spec = mlp_spec_from_module(MLP([4, 64, 64, 2], hidden, output))
     assert spec == MLPSpec((4, 64, 64, 2), hidden, output)
-    assert spec.act == ext.code(hidden, output) == ext.HIDDEN_CODES[hidden] | (256 if output == "tanh" else 0)
+    assert spec.act == mlp.code(hidden, output) == mlp.HIDDEN_CODES[hidden] | (256 if output == "tanh" else 0)
 
 
 @pytest.mark.parametrize("output", ["identity", "tanh"])
@@ -108,11 +109,11 @@ def test_header_and_binding_agree_on_the_codes():
     header = open(os.path.join(ROOT, "include", "estk.h")).read()
     for name, want in (("ESTK_ACT_ELU", 3), ("ESTK_ACT_SILU", 4), ("ESTK_ACT_LEAKY_RELU", 5)):
         m = re.search(r"#define\s+%s\s+(\d+)" % name, header)
-        assert m and int(m.group(1)) == getattr(_capi, name) == want == ext.HIDDEN_CODES[name[9:].lower()]
+        assert m and int(m.group(1)) == getattr(_capi, name) == want == mlp.HIDDEN_CODES[name[9:].lower()]
     assert not re.search(r"#define\s+ESTK_ACT_\w+\s+2\b", header)              # 2 stays undefined
     assert re.search(r"#define\s+ESTK_VERSION\s+200\b", header)
     from estorch_b200.policy_spec import _HIDDEN_CODES
-    assert _HIDDEN_CODES == ext.HIDDEN_CODES
+    assert _HIDDEN_CODES == mlp.HIDDEN_CODES
 
 
 def _lib():
@@ -134,7 +135,7 @@ REFUSED = [2, 0xff, 0x200, -1, 1 << 24, 0x20000, 0x10200, 6, 0x0102, 0x10002] + 
 def test_support_probe_takes_the_new_codes_and_refuses_the_rest():
     lib = _lib()
     TC = (_capi.ESTK_PREC_F16, _capi.ESTK_PREC_BF16, _capi.ESTK_PREC_BF16S)
-    for code in ext.NEW_ACTS:
+    for code in mlp.NEW_ACTS:
         for prec in TC:
             assert _supported(lib, [64, 64, 32], code, prec, 256) == 1, (hex(code), prec)
             assert _supported(lib, [64, 64, 32], code, prec, 100) == 0, (hex(code), prec)    # the shape rule
@@ -151,10 +152,10 @@ def test_support_probe_takes_the_new_codes_and_refuses_the_rest():
 def test_oracle_activations_match_torch():
     y = torch.tensor([-100.0, -30.0, -1.0, -1e-30, -0.0, 0.0, 1e-30, 0.5, 3.0, 100.0])
     yn = y.numpy()
-    np.testing.assert_array_equal(ext._leaky_relu(yn), F.leaky_relu(y).numpy())
-    np.testing.assert_allclose(ext._elu(yn), F.elu(y).numpy(), rtol=2e-7, atol=0)
-    np.testing.assert_allclose(ext._silu(yn), (y / (1 + torch.exp(-y))).numpy(), rtol=2e-7, atol=0)
-    assert ext._silu(np.float32([-100.0]))[0] == 0 and ext._elu(np.float32([-100.0]))[0] == -1
+    np.testing.assert_array_equal(orc.HIDDEN["leaky_relu"](yn), F.leaky_relu(y).numpy())
+    np.testing.assert_allclose(orc.HIDDEN["elu"](yn), F.elu(y).numpy(), rtol=2e-7, atol=0)
+    np.testing.assert_allclose(orc.HIDDEN["silu"](yn), (y / (1 + torch.exp(-y))).numpy(), rtol=2e-7, atol=0)
+    assert orc.HIDDEN["silu"](np.float32([-100.0]))[0] == 0 and orc.HIDDEN["elu"](np.float32([-100.0]))[0] == -1
 
 
 def _check_population_golden(g, hidden, output, loss, bc=False):
@@ -163,10 +164,10 @@ def _check_population_golden(g, hidden, output, loss, bc=False):
     out = []
     for gen in range(len(g["grad"])):
         pop, _ = orc.sample_population(g["theta_before"][gen], g["table"], g["offsets"][gen], sigma)
-        rets, bcs = ext.evaluate_population(pop, dims, g["obs"], g["target"], bc_obs, bc_dim, hidden, output,
-                                            loss=loss)
+        rets, bcs = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.code(hidden, output, loss),
+                                            bc_obs=bc_obs, bc_dim=bc_dim)
         assert rel_err(rets, g["returns"][gen][:, 0]) < 2e-6
-        ep = ext.member_return(ext.mlp_forward(g["theta_after"][gen], dims, g["obs"], hidden, output), g["target"],
+        ep = mlp.member_return(orc.mlp_forward(g["theta_after"][gen], dims, g["obs"], hidden, output), g["target"],
                                loss)
         assert abs(float(ep) - float(g["episode_reward"][gen])) < 1e-5
         out.append(bcs)
@@ -185,7 +186,7 @@ def test_oracle_silu_forward_matches_reference_golden_nsr_bc():
     g = load_golden("nsr_silu_bipedal_p32.npz")
     dims, k = [int(d) for d in g["dims"]], int(g["k"])
     bc_obs, bc_dim = int(g["bc_obs"]), int(g["bc_dim"])
-    fwd = lambda th: ext.mlp_forward(th, dims, g["obs"], "silu", "tanh")  # noqa: E731
+    fwd = lambda th: orc.mlp_forward(th, dims, g["obs"], "silu", "tanh")  # noqa: E731
     archive = [orc.synthetic_bc(fwd(th), bc_obs, bc_dim) for th in g["meta_theta0"]]
     np.testing.assert_allclose(np.stack(archive), g["archive0"], rtol=1e-5, atol=1e-6)
     bcs_all = _check_population_golden(g, "silu", "tanh", "mse", bc=True)
@@ -219,7 +220,7 @@ def test_es_fused_matches_reference_golden(fixture, hidden, loss):
     akw = dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]))
     if loss == "xent":
         akw["loss"] = "cross_entropy"
-    be = ActExtOracleBackend()
+    be = OracleBackend()
     es = R(MLP, E.DeviceAgent, torch.optim.Adam, population_size=64, sigma=0.1,
            policy_kwargs={"dims": dims, "hidden": hidden}, agent_kwargs=akw, optimizer_kwargs={"lr": 0.01},
            noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]), _backend=be)
@@ -229,7 +230,7 @@ def test_es_fused_matches_reference_golden(fixture, hidden, loss):
     _load_theta(es.policy, g["theta0"])
     es._slots[0].ensure_flat()
     es.train(n_steps=3)
-    assert be.acts == {ext.code(hidden, "identity", loss)}
+    assert be.acts == {mlp.code(hidden, "identity", loss)}
     for gen in range(3):
         assert rel_err(es.rec[gen]["returns"][:, 0], g["returns"][gen][:, 0]) < 1e-5
         assert abs(es.rec[gen]["episode"] - float(g["episode_reward"][gen])) < 2e-5
@@ -252,7 +253,7 @@ def test_nsr_fused_silu_matches_reference_golden():
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]), bc_obs=64,
                              bc_dim=256),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]),
-           _backend=ActExtOracleBackend())
+           _backend=OracleBackend())
     es.rec = []
     assert es._fused and es._spec.act == _capi.ESTK_ACT_SILU | _capi.ESTK_ACT_OUT_TANH
     es._table.copy_(torch.from_numpy(g["table"]))
@@ -285,7 +286,7 @@ def test_fused_and_the_code_reaches_every_evaluate(hidden, tensor_core, loss):
         tgt = torch.nn.functional.one_hot(torch.from_numpy(rng.randint(0, dims[-1], B)), dims[-1]).float()
     else:
         tgt = torch.from_numpy(rng.uniform(-0.9, 0.9, (B, dims[-1])).astype(np.float32))
-    be = ActExtOracleBackend(tensor_core=tensor_core)
+    be = OracleBackend(tensor_core=tensor_core)
     akw = dict(obs=obs, target=tgt)
     if loss == "xent":
         akw["loss"] = "cross_entropy"
@@ -293,7 +294,7 @@ def test_fused_and_the_code_reaches_every_evaluate(hidden, tensor_core, loss):
               policy_kwargs={"dims": dims, "hidden": hidden}, agent_kwargs=akw, optimizer_kwargs={"lr": 0.01},
               noise_table_size=1 << 16, _backend=be)
     es.log = lambda: None
-    code = ext.code(hidden, "identity", loss)
+    code = mlp.code(hidden, "identity", loss)
     assert es._fused and es._act_code() == code
     assert es._precision == ("f16" if tensor_core else "fp32")       # "auto" picks f16 where the shape allows
     es.train(n_steps=2)
@@ -304,7 +305,7 @@ def test_default_elu_is_fused_and_a_nondefault_alpha_stays_in_hooks_mode():
     es = E.ES(MLP, E.DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               policy_kwargs={"dims": [4, 16, 2], "hidden": "elu"},
               agent_kwargs=dict(obs=torch.randn(8, 4), target=torch.randn(8, 2)), noise_table_size=1 << 12,
-              _backend=ActExtOracleBackend())
+              _backend=OracleBackend())
     assert es._fused
 
     class Elu05(nn.Module):
@@ -316,5 +317,5 @@ def test_default_elu_is_fused_and_a_nondefault_alpha_stays_in_hooks_mode():
             return self.net(x)
     es = E.ES(Elu05, E.DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               agent_kwargs=dict(obs=torch.randn(8, 4), target=torch.randn(8, 2)), noise_table_size=1 << 12,
-              _backend=ActExtOracleBackend())
+              _backend=OracleBackend())
     assert es._spec is None and not es._fused

@@ -1,6 +1,6 @@
 """ELU, SiLU and LeakyReLU MLP policies on the H100: the nine new activation codes of include/estk.h
 in every MLP evaluate kernel (fp32 shared-memory, fp32 streamed, f16 / bf16 / bf16s cluster, f16_any
-streamed) against the oracle emulations of tests/_act_ext_oracle.py and the exact fp32 forward;
+streamed) against the oracle emulations of tests/_mlp_oracle.py and the exact fp32 forward;
 determinism; large pre-activations; the north-star shape per kind; and ES / NSR-ES runs against the
 reference-generated goldens."""
 import json
@@ -12,8 +12,9 @@ import torch.nn.functional as F
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _act_ext_oracle as ext
-from _act_ext_oracle import MLP, NEW_ACTS, ActExtOracleBackend, decode
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP, NEW_ACTS, decode
+from _oracle_backend import OracleBackend
 import estorch_b200 as E
 
 pytestmark = pytest.mark.gpu
@@ -76,13 +77,12 @@ def _eval(be, dims, th, tb, offs, sigma, obs, tgt, code, mode, kw, bc_obs=0, bc_
 
 
 def _want(dims, theta, table, offs, obs, tgt, code, mode, bc_obs=0, bc_dim=0):
-    hidden, output, loss = decode(code)
     if mode == "fp32":
         rows, _ = orc.sample_population(theta, table, offs, 0.02)
     else:
-        rows = ActExtOracleBackend(tensor_core=True)._rows(torch.from_numpy(theta), torch.from_numpy(table),
-                                                           torch.from_numpy(offs), 0.02, dims, mode)
-    return ext.evaluate_population(rows, dims, obs, tgt, bc_obs, bc_dim, hidden, output, mode, loss)
+        rows = OracleBackend(tensor_core=True)._rows(torch.from_numpy(theta), torch.from_numpy(table),
+                                                     torch.from_numpy(offs), 0.02, dims, mode)
+    return mlp.evaluate_population(rows, dims, obs, tgt, code, mode, bc_obs, bc_dim)
 
 
 # ------------------------------------------------------------------ fp32 CUDA-core kernels
@@ -102,7 +102,7 @@ def test_fp32_kernels_vs_oracle(be, dims, B, pairs, code):
     assert rel_err(bcs, want_bc) < 5e-6
     one = be.zeros(1)
     be.eval_mlp_center(dims, th, dev(be, obs), dev(be, tgt), one, act=code)
-    w = float(ext.member_return(ext.mlp_forward(theta, dims, obs, hidden, output), tgt, loss))
+    w = float(mlp.member_return(orc.mlp_forward(theta, dims, obs, hidden, output), tgt, loss))
     assert abs(float(one) - w) < 5e-6 * abs(w) + 1e-7
 
 
@@ -148,7 +148,7 @@ def test_tensor_core_modes_vs_emulation_and_fp32(be, mode, dims, B, pairs, code)
     be.eval_mlp_center(dims, th, dev(be, obs), dev(be, tgt), one, precision=mode, act=code,
                        **({"theta16": kw["theta16"]} if mode == "bf16s" else {}))
     ct = torch.zeros(1)
-    ActExtOracleBackend(tensor_core=True).eval_mlp_center(dims, torch.from_numpy(theta), torch.from_numpy(obs),
+    OracleBackend(tensor_core=True).eval_mlp_center(dims, torch.from_numpy(theta), torch.from_numpy(obs),
                                                           torch.from_numpy(tgt), ct, precision=mode, act=code)
     assert abs(float(one) - float(ct)) < t_emu * abs(float(ct))
     if centre:
@@ -173,14 +173,14 @@ XS = np.float32([-1e4, -100.0, -90.0, -89.0, -88.5, -50.0, -17.0, -1.0, -0.125, 
 
 
 @pytest.mark.parametrize("mode", ["fp32", "f16", "bf16"])
-@pytest.mark.parametrize("hidden", ext.NEW_KINDS)
+@pytest.mark.parametrize("hidden", mlp.NEW_KINDS)
 def test_large_preactivations_are_finite_and_exact(be, hidden, mode):
     dims, B = [64, 64, 64], 256
     eye = np.eye(64, dtype=np.float32)
     theta = np.concatenate([eye.ravel(), np.zeros(64, np.float32), eye.ravel(), np.zeros(64, np.float32)])
     obs = np.resize(XS, (B, 64)).astype(np.float32)
     tgt = np.zeros((B, 64), np.float32)
-    code = ext.code(hidden)
+    code = mlp.code(hidden)
     one, bc = be.zeros(1), be.zeros(B * 64)
     be.eval_mlp_center(dims, dev(be, theta), dev(be, obs), dev(be, tgt), one, bc, B, B * 64, precision=mode, act=code)
     got = bc.cpu().numpy().reshape(B, 64)
@@ -192,19 +192,19 @@ def test_large_preactivations_are_finite_and_exact(be, hidden, mode):
         np.testing.assert_array_equal(got, want)                  # the device's IEEE functions, bit for bit
         assert got[0, 1] == (-1.0 if hidden == "elu" else 0.0 if hidden == "silu" else -1.0)
     else:
-        want = ext.FORWARD[mode](theta, dims, obs, hidden)
+        want = mlp.FORWARD[mode](theta, dims, obs, hidden)
         np.testing.assert_allclose(got, want, rtol=1e-6, atol=0)
         if mode == "f16" and hidden != "leaky_relu":
             assert got.min() >= -1.0 and got.max() == 65504.0     # only the positive side saturates
 
 
 # ------------------------------------------------------------------ north-star shape
-@pytest.mark.parametrize("hidden", ext.NEW_KINDS)
+@pytest.mark.parametrize("hidden", mlp.NEW_KINDS)
 def test_north_star_fp32_and_f16_vs_cpu_oracle(be, hidden):
     """P = 4096, n = 1,001,760, B = 256: 512 members (the + and - of 256 pairs) of the fp32 and f16
     device evaluate against the CPU oracle's fp32 forward (max-norm relative)."""
     dims = [128, 512, 512, 512, 512, 288]
-    code = ext.code(hidden)
+    code = mlp.code(hidden)
     n, P, pairs, sigma = orc.mlp_param_count(dims), 4096, 2048, 0.02
     torch.manual_seed(0)
     mods = []
@@ -233,7 +233,7 @@ def test_north_star_fp32_and_f16_vs_cpu_oracle(be, hidden):
     want_p, want_m = [], []
     for c in range(0, sel.size, 32):
         pop, _ = orc.sample_population(th_h, tab_h, offs_h[sel[c: c + 32]], sigma)
-        w, _ = ext.evaluate_population(pop, dims, obs.numpy(), tgt.numpy(), hidden=hidden)
+        w, _ = mlp.evaluate_population(pop, dims, obs.numpy(), tgt.numpy(), mlp.code(hidden))
         want_p.append(w[:len(w) // 2])
         want_m.append(w[len(w) // 2:])
     want = np.concatenate(want_p + want_m)
@@ -268,7 +268,7 @@ def test_es_fused_vs_reference_golden(fixture, hidden, loss):
     es = R(MLP, E.DeviceAgent, torch.optim.Adam, population_size=64, sigma=0.1,
            policy_kwargs={"dims": dims, "hidden": hidden}, agent_kwargs=akw, optimizer_kwargs={"lr": 0.01},
            noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]))
-    assert es._fused and es._be.name == "cuda" and es._act_code() == ext.code(hidden, "identity", loss)
+    assert es._fused and es._be.name == "cuda" and es._act_code() == mlp.code(hidden, "identity", loss)
     es._table.copy_(torch.from_numpy(g["table"]))
     _set_theta(es.policy, g["theta0"])
     es.train(n_steps=3)
@@ -294,7 +294,7 @@ def test_nsr_fused_silu_vs_reference_golden():
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]),
                              bc_obs=64, bc_dim=256),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]))
-    assert es._fused and es._spec.act == ext.code("silu", "tanh")
+    assert es._fused and es._spec.act == mlp.code("silu", "tanh")
     es._table.copy_(torch.from_numpy(g["table"]))
     for i, (p, _) in enumerate(es.meta_population):
         _set_theta(p, g["meta_theta0"][i])
@@ -309,7 +309,7 @@ def test_nsr_fused_silu_vs_reference_golden():
     np.testing.assert_allclose(np.stack(es._archive), g["archive_final"], rtol=1e-3, atol=1e-4)
 
 
-@pytest.mark.parametrize("hidden", ext.NEW_KINDS)
+@pytest.mark.parametrize("hidden", mlp.NEW_KINDS)
 def test_auto_picks_f16_and_trains_fused(hidden):
     dims = [128, 256, 64]
     g = torch.Generator().manual_seed(8)

@@ -291,7 +291,7 @@ def test_engine_conv_vbn_fused_every_step():
 
 def test_engine_mlp_population_mode_every_step():
     import estorch_b200 as E
-    from _act_ext_oracle import MLP
+    from _mlp_oracle import MLP
     from _pop_oracle import LinearWalker
     from test_population_cpu import DIMS
     torch.manual_seed(2)

@@ -17,7 +17,8 @@ import estorch_b200.estorch as E
 from estorch_b200 import DeviceAgent, PopulationAgent, SequenceAgent, _capi
 from estorch_b200.policy_spec import CNNSpec, cnn_spec_from_module
 from conftest import ROOT, load_golden, rel_err
-from _cnn_oracle import CnnOracleBackend, forward, image_task, pack, param_count, policy_class, returns_of
+from _cnn_oracle import forward, image_task, pack, param_count, policy_class, returns_of
+from _oracle_backend import OracleBackend
 from test_population_rnn_cpu import _load_theta, _Rec, check_es_golden, check_nsr_golden
 
 SHAPE = (1, 12, 12)
@@ -31,7 +32,7 @@ def _es(cls=E.ES, hidden="relu", out_tanh=False, optimizer=torch.optim.Adam, age
         tgt = tgt - 0.5
     es = cls(policy_class(2, hidden, out_tanh), agent, optimizer, population_size=P, sigma=0.05,
              policy_kwargs={"dims": dims}, agent_kwargs=agent_kwargs or dict(obs=obs, target=tgt, loss=loss),
-             optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, _backend=CnnOracleBackend(), **kw)
+             optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, _backend=OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -129,24 +130,23 @@ def test_the_global_rng_is_untouched_and_existing_specs_unchanged():
     from test_api_cpu import MLP
     obs, tgt = torch.randn(6, 3), torch.randn(6, 2)
     es = E.ES(MLP, DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05, policy_kwargs={"dims": [3, 8, 2]},
-              agent_kwargs=dict(obs=obs, target=tgt), noise_table_size=1 << 13, _backend=CnnOracleBackend())
+              agent_kwargs=dict(obs=obs, target=tgt), noise_table_size=1 << 13, _backend=OracleBackend())
     assert type(es._spec).__name__ == "MLPSpec" and not es._is_cnn
     # the conv + VirtualBatchNorm policy of the Atari example and a recurrent policy keep their specs
     from _pop_conv_oracle import AtariPolicy
     from _rnn_oracle import policy_class as rnn_policy_class
     from estorch_b200.policy_spec import ConvVBNSpec, RNNSpec
-    from _pop_conv_oracle import PopConvOracleBackend
     # (SGD: hooks mode, so the stand-in needs no conv scratch; the spec is recognised the same way)
     es = E.ES(AtariPolicy, DeviceAgent, torch.optim.SGD, population_size=8, sigma=0.05,
               policy_kwargs={"n_actions": 4, "xref": torch.rand(3, 4, 84, 84)}, optimizer_kwargs={"lr": 0.01},
               agent_kwargs=dict(obs=torch.rand(2, 4, 84, 84), target=torch.rand(2, 4)), noise_table_size=1 << 20,
-              _backend=PopConvOracleBackend())
+              _backend=OracleBackend())
     assert isinstance(es._spec, ConvVBNSpec) and es._spec.n_actions == 4 and not es._is_cnn
     g = torch.Generator().manual_seed(9)
     es = E.ES(rnn_policy_class("lstm", True), SequenceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               policy_kwargs={"dims": (3, 8, 2)},
               agent_kwargs=dict(obs=torch.randn(5, 4, 3, generator=g), target=torch.rand(5, 4, 2, generator=g)),
-              noise_table_size=1 << 13, _backend=CnnOracleBackend())
+              noise_table_size=1 << 13, _backend=OracleBackend())
     assert es._spec == RNNSpec("lstm", (3, 8, 2), "tanh") and not es._is_cnn
 
 
@@ -247,11 +247,11 @@ def run_nsr_cnn_golden(backend):
 
 
 def test_es_cnn_matches_reference_golden():
-    check_es_golden(*run_es_cnn_golden(CnnOracleBackend()))
+    check_es_golden(*run_es_cnn_golden(OracleBackend()))
 
 
 def test_nsr_cnn_cross_entropy_matches_reference_golden():
-    check_nsr_golden(*run_nsr_cnn_golden(CnnOracleBackend()))
+    check_nsr_golden(*run_nsr_cnn_golden(OracleBackend()))
 
 
 # ------------------------------------------------------------------ two processes over gloo

@@ -1,6 +1,6 @@
 """The TF32 convolutional evaluate without a GPU: the companion header and its binding, refusals through the ABI
 before any launch (fake device pointers: nothing is dereferenced), the engine's eval_precision="tf32" mode
-selection on the TF32 stand-in backend (tests/_cnn_tf32_oracle.py), and the numpy restatement of rna_tf32."""
+selection on the stand-in backend (tests/_oracle_backend.py), and the numpy restatement of rna_tf32."""
 import ctypes as C
 import os
 import re
@@ -14,8 +14,8 @@ from estorch_b200 import DeviceAgent, PopulationAgent, _capi
 from estorch_b200.backend import cnn_desc
 from conftest import ROOT
 from _cnn_oracle import image_task, pack, policy_class
-from _batch_oracle import BatchMixin
-from _cnn_tf32_oracle import LOSS_ACCURACY, Tf32CnnOracleBackend, rna_tf32
+from _cnn_tf32_oracle import LOSS_ACCURACY, rna_tf32
+from _oracle_backend import OracleBackend
 
 SHAPE = (1, 12, 12)
 DIMS = pack(SHAPE, [(4, 3, 2, 1), (6, 3, 2, 0)], [8, 4])
@@ -31,7 +31,7 @@ def _es(cls=E.ES, loss="mse", backend=None, agent_kwargs=None, P=8, **kw):
     es = cls(policy_class(2), DeviceAgent, torch.optim.Adam, population_size=P, sigma=0.05,
              policy_kwargs={"dims": DIMS}, agent_kwargs=agent_kwargs or dict(obs=obs, target=tgt, loss=loss),
              optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13,
-             _backend=backend or Tf32CnnOracleBackend(), **kw)
+             _backend=backend or OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -157,10 +157,8 @@ def test_auto_stays_fp32():
 
 def test_tf32_with_batch_size_and_nsr_with_bc():
     obs, tgt = image_task(40, SHAPE, seed=2)
-    class Sampling(BatchMixin, Tf32CnnOracleBackend):
-        pass
     es = _es(agent_kwargs=dict(obs=obs, target=tgt, loss="cross_entropy", batch_size=8), eval_precision="tf32",
-             backend=Sampling())
+             backend=OracleBackend())
     assert es._fused and es._precision == "tf32"
     es.train(n_steps=2)
     assert set(es._be.cnn_precisions) == {"tf32"}
@@ -176,11 +174,10 @@ def test_refusals_in_the_engine():
         with pytest.raises(ValueError, match="fp32 only"):
             _es(eval_precision=prec)
     with pytest.raises(ValueError, match="2\\*\\*26 floats"):
-        _es(eval_precision="tf32", backend=Tf32CnnOracleBackend(tf32_supported=False))
+        _es(eval_precision="tf32", backend=OracleBackend(tf32=False))
     with pytest.raises(ValueError, match="'tf32'"):
         _es(eval_precision="tf33")
     # an MLP on a device agent
-    from _oracle_backend import OracleBackend
     from estorch_b200.policy_spec import MLPSpec  # noqa: F401
 
     class MLP(torch.nn.Module):
@@ -199,12 +196,11 @@ def test_refusals_in_the_engine():
 
 def test_a_fused_recurrent_policy_refuses_tf32():
     from estorch_b200 import SequenceAgent
-    from _cnn_oracle import CnnOracleBackend
     from _rnn_oracle import policy_class as rnn_policy_class
     g = torch.Generator().manual_seed(9)
     kw = dict(policy_kwargs={"dims": (3, 8, 2)},
               agent_kwargs=dict(obs=torch.randn(5, 4, 3, generator=g), target=torch.rand(5, 4, 2, generator=g)),
-              noise_table_size=1 << 13, _backend=CnnOracleBackend())
+              noise_table_size=1 << 13, _backend=OracleBackend())
     es = E.ES(rnn_policy_class("lstm", True), SequenceAgent, torch.optim.Adam, population_size=8, sigma=0.05, **kw)
     assert es._fused and es._is_rnn
     with pytest.raises(ValueError, match="'tf32' is for convolutional policies"):
@@ -220,7 +216,7 @@ def test_population_mode_refuses_tf32():
             raise AssertionError
     with pytest.raises(ValueError, match="fp32 only"):
         E.ES(policy_class(2), Pop, torch.optim.Adam, population_size=8, sigma=0.05, policy_kwargs={"dims": DIMS},
-             noise_table_size=1 << 13, eval_precision="tf32", _backend=Tf32CnnOracleBackend())
+             noise_table_size=1 << 13, eval_precision="tf32", _backend=OracleBackend())
 
 
 def test_hooks_mode_ignores_tf32():

@@ -1,6 +1,6 @@
 """Tanh MLP policies on the H100: every MLP evaluate precision with the four activation codes of
 include/estk.h (hidden ReLU / Tanh x output identity / Tanh), against the reference-generated Tanh
-goldens and the activation-aware oracle (tests/_act_oracle.py); the north-star shape in fp32 and
+goldens and the activation-aware oracle (tests/_mlp_oracle.py); the north-star shape in fp32 and
 f16; and the public API (ES / NSR-ES fused runs, CUDA-graph replay, an f16 fused generation)."""
 import ctypes as C
 import json
@@ -11,10 +11,12 @@ import torch
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _act_oracle as act
-from _act_oracle import ALL_ACTS, ActOracleBackend, kinds
+import _mlp_oracle as mlp
+from _oracle_backend import OracleBackend
 from test_activations_cpu import ActMLP
 import estorch_b200 as E
+
+ACTS = (0, mlp.ACT_TANH, mlp.ACT_OUT_TANH, mlp.ACT_TANH | mlp.ACT_OUT_TANH)     # ReLU / Tanh hidden x output
 
 pytestmark = pytest.mark.gpu
 
@@ -62,16 +64,16 @@ def test_fp32_tanh_matches_reference_goldens(be):
     dims = [int(d) for d in g["dims"]]
     for gen in range(len(g["grad"])):
         ret, _, _ = _eval(be, dims, g["theta_before"][gen], g["table"], g["offsets"][gen], float(g["sigma"]),
-                          g["obs"], g["target"], act.ACT_TANH)
+                          g["obs"], g["target"], mlp.ACT_TANH)
         assert rel_err(ret, g["returns"][gen][:, 0]) < 2e-6
     g = load_golden("nsr_tanh_bipedal_p32.npz")
-    dims, code = [int(d) for d in g["dims"]], act.ACT_TANH | act.ACT_OUT_TANH
+    dims, code = [int(d) for d in g["dims"]], mlp.ACT_TANH | mlp.ACT_OUT_TANH
     theta, offs = g["theta_before"][0], g["offsets"][0]
     ret, bcs, _ = _eval(be, dims, theta, g["table"], offs, float(g["sigma"]), g["obs"], g["target"], code,
                         bc_obs=64, bc_dim=256)
     assert rel_err(ret, g["returns"][0][:, 0]) < 2e-6
     pop, _ = orc.sample_population(theta, g["table"], offs, float(g["sigma"]))
-    _, want_bc = act.evaluate_population(pop, dims, g["obs"], g["target"], 64, 256, "tanh", "tanh")
+    _, want_bc = mlp.evaluate_population(pop, dims, g["obs"], g["target"], code, bc_obs=64, bc_dim=256)
     assert rel_err(bcs, want_bc) < 2e-6
     # centre evaluation: the archive's first entry is the BC of meta_theta0[0]
     one, bc1 = be.zeros(1), be.zeros(256)
@@ -80,11 +82,11 @@ def test_fp32_tanh_matches_reference_goldens(be):
     assert rel_err(bc1.cpu().numpy(), g["archive0"][0]) < 2e-6
 
 
-@pytest.mark.parametrize("act_code", ALL_ACTS)
+@pytest.mark.parametrize("act_code", ACTS)
 @pytest.mark.parametrize("dims,B,pairs", [([128, 512, 512, 288], 48, 4), ([17, 33, 5], 100, 6), ([4, 2], 1, 3),
                                           ([9, 130, 70, 70, 3], 256, 3)])
 def test_fp32_shapes_vs_oracle(be, dims, B, pairs, act_code):
-    hidden, output = kinds(act_code)
+    hidden, output = mlp.decode(act_code)[:2]
     rng = np.random.RandomState(1)
     n = orc.mlp_param_count(dims)
     table_len = max(1 << 14, (n + 31) // 32 * 32 + 4096)
@@ -95,11 +97,11 @@ def test_fp32_shapes_vs_oracle(be, dims, B, pairs, act_code):
     offs = orc.noise_offsets(5, 0, 0, pairs, table_len, n)
     ret, _, _ = _eval(be, dims, theta, table, offs, 0.02, obs, tgt, act_code)
     pop, _ = orc.sample_population(theta, table, offs, 0.02)
-    want, _ = act.evaluate_population(pop, dims, obs, tgt, hidden=hidden, output=output)
+    want, _ = mlp.evaluate_population(pop, dims, obs, tgt, act_code)
     assert rel_err(ret, want) < 5e-6
     one = be.zeros(1)
     be.eval_mlp_center(dims, dev(be, theta), dev(be, obs), dev(be, tgt), one, act=act_code)
-    w = float(orc.synthetic_return(act.mlp_forward(theta, dims, obs, hidden, output), tgt))
+    w = float(orc.synthetic_return(orc.mlp_forward(theta, dims, obs, hidden, output), tgt))
     assert abs(float(one) - w) < 5e-6 * abs(w) + 1e-7
 
 
@@ -122,11 +124,10 @@ def _tc_problem(dims, B, pairs, seed=23):
 TC_TOL = {"f16": (1e-5, 3e-5, 2e-3), "bf16": (5e-4, 2e-2, 5e-3), "bf16s": (5e-4, 3e-2, 5e-3)}
 
 
-@pytest.mark.parametrize("act_code", ALL_ACTS)
+@pytest.mark.parametrize("act_code", ACTS)
 @pytest.mark.parametrize("mode", ["f16", "bf16", "bf16s"])
 @pytest.mark.parametrize("dims,B,pairs,bc", [([64, 256, 64], 512, 4, 256), ([128, 512, 512, 288], 256, 3, 0)])
 def test_tensor_core_modes_vs_emulation_and_fp32(be, dims, B, pairs, bc, mode, act_code):
-    hidden, output = kinds(act_code)
     n, table, theta, obs, tgt, offs = _tc_problem(dims, B, pairs)
     assert be.eval_supports_f16(dims, B, act=act_code) and be.eval_supports_bf16(dims, B, act=act_code)
     th, tb = dev(be, theta), dev(be, table)
@@ -140,11 +141,11 @@ def test_tensor_core_modes_vs_emulation_and_fp32(be, dims, B, pairs, bc, mode, a
         be.shadow_bf16(tb, kw["table16"])
     got, got_bc, centre = _eval(be, dims, theta, table, offs, 0.02, obs, tgt, act_code, 64 if bc else 0, bc,
                                 precision=mode, centre=True, **kw)
-    emu_be = ActOracleBackend(tensor_core=True)
+    emu_be = OracleBackend(tensor_core=True)
     rows = emu_be._rows(torch.from_numpy(theta), torch.from_numpy(table), torch.from_numpy(offs), 0.02, dims, mode)
-    emu, emu_bc = act.evaluate_population(rows, dims, obs, tgt, 64 if bc else 0, bc, hidden, output, precision=mode)
+    emu, emu_bc = mlp.evaluate_population(rows, dims, obs, tgt, act_code, mode, 64 if bc else 0, bc)
     pop, _ = orc.sample_population(theta, table, offs, 0.02)
-    exact, exact_bc = act.evaluate_population(pop, dims, obs, tgt, 64 if bc else 0, bc, hidden, output)
+    exact, exact_bc = mlp.evaluate_population(pop, dims, obs, tgt, act_code, "fp32", 64 if bc else 0, bc)
     t_emu, t_exact, t_bc = TC_TOL[mode]
     print(f"{mode} act={act_code:#x} {dims}: vs emulation {rel_err(got, emu):.2e}, vs fp32 {rel_err(got, exact):.2e}")
     assert rel_err(got, emu) < t_emu
@@ -170,7 +171,7 @@ def test_invalid_activation_codes_are_refused_by_every_precision(be):
     from estorch_b200.backend import mlp_desc
     lib = _capi.load()
     dims, B = [64, 64, 32], 256
-    for code in ALL_ACTS:
+    for code in ACTS:
         d = mlp_desc(dims, code)
         assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_F16, B) == 1
         assert lib.estk_eval_mlp_supported(C.byref(d), _capi.ESTK_PREC_BF16, B) == 1
@@ -197,7 +198,7 @@ def test_north_star_tanh_fp32_and_f16_vs_cpu_oracle(be, output):
     """P = 4096, n = 1,001,760, B = 256, Tanh hidden: 512 members (the + and - of 256 pairs) of the
     fp32 and f16 device evaluate against the CPU oracle's fp32 forward (max-norm relative)."""
     dims = [128, 512, 512, 512, 512, 288]
-    code = act.code("tanh", output)
+    code = mlp.code("tanh", output)
     n, P, pairs, sigma = orc.mlp_param_count(dims), 4096, 2048, 0.02
     torch.manual_seed(0)
     mods = []
@@ -226,7 +227,7 @@ def test_north_star_tanh_fp32_and_f16_vs_cpu_oracle(be, output):
     want_p, want_m = [], []
     for c in range(0, sel.size, 32):                              # 64 rows (256 MB) at a time
         pop, _ = orc.sample_population(th_h, tab_h, offs_h[sel[c: c + 32]], sigma)
-        w, _ = act.evaluate_population(pop, dims, obs.numpy(), tgt.numpy(), hidden="tanh", output=output)
+        w, _ = mlp.evaluate_population(pop, dims, obs.numpy(), tgt.numpy(), mlp.code("tanh", output))
         want_p.append(w[:len(w) // 2])
         want_m.append(w[len(w) // 2:])
     want = np.concatenate(want_p + want_m)
@@ -253,7 +254,7 @@ def test_es_fused_tanh_vs_reference_golden():
            policy_kwargs={"dims": dims, "hidden": "tanh"},
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"])),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]))
-    assert es._fused and es._be.name == "cuda" and es._spec.act == act.ACT_TANH
+    assert es._fused and es._be.name == "cuda" and es._spec.act == mlp.ACT_TANH
     es._table.copy_(torch.from_numpy(g["table"]))
     _set_theta(es.policy, g["theta0"])
     es.train(n_steps=3)
@@ -261,12 +262,12 @@ def test_es_fused_tanh_vs_reference_golden():
     for gen in range(3):
         r = rec[gen]
         pop, eps = orc.sample_population(theta, g["table"], g["offsets"][gen], 0.1)
-        want, _ = act.evaluate_population(pop, dims, g["obs"], g["target"], hidden="tanh")
+        want, _ = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.ACT_TANH)
         assert rel_err(r["returns"][:, 0], want) < 5e-6
         assert rel_err(r["grad"], orc.calculate_grad(r["returns"][:, 0], eps, 0.1)) < 1e-5
         th, m, v = orc.adam_step(theta, m, v, orc.negate_clamp(r["grad"]), gen + 1)
         assert rel_err(r["theta"], th) < 1e-6
-        ep = orc.synthetic_return(act.mlp_forward(th, dims, g["obs"], "tanh"), g["target"])
+        ep = orc.synthetic_return(orc.mlp_forward(th, dims, g["obs"], "tanh"), g["target"])
         assert abs(r["episode"] - float(ep)) < 1e-5
         theta = r["theta"]
         assert rel_err(r["returns"][:, 0], g["returns"][gen][:, 0]) < 1e-4   # the reference's trajectory
@@ -290,7 +291,7 @@ def test_nsr_fused_tanh_vs_reference_golden():
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]),
                              bc_obs=64, bc_dim=256),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]))
-    assert es._fused and es._spec.act == act.ACT_TANH | act.ACT_OUT_TANH
+    assert es._fused and es._spec.act == mlp.ACT_TANH | mlp.ACT_OUT_TANH
     es._table.copy_(torch.from_numpy(g["table"]))
     for i, (p, _) in enumerate(es.meta_population):
         _set_theta(p, g["meta_theta0"][i])
@@ -320,7 +321,7 @@ def test_graph_replay_equals_eager_tanh(monkeypatch):
                   policy_kwargs={"dims": dims, "hidden": "tanh", "output": "tanh"},
                   agent_kwargs=dict(obs=obs, target=tgt), optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 22,
                   log_interval=4)
-        assert es._precision == "f16" and es._spec.act == act.ACT_TANH | act.ACT_OUT_TANH
+        assert es._precision == "f16" and es._spec.act == mlp.ACT_TANH | mlp.ACT_OUT_TANH
         es.log = lambda: None
         es.train(n_steps=13)
         out[mode] = (es._slots[0].theta.clone(), es._slots[0].best_theta.clone(), es.episode_reward, es.best_reward,
@@ -339,7 +340,7 @@ def test_f16_tanh_fused_generation_vs_oracle_emulation(output):
     g = torch.Generator().manual_seed(8)
     obs, tgt = torch.randn(256, 128, generator=g), torch.rand(256, 64, generator=g) * 1.8 - 0.9
     res, table = {}, None
-    for name, backend in (("cuda", None), ("oracle", ActOracleBackend(tensor_core=True))):
+    for name, backend in (("cuda", None), ("oracle", OracleBackend(tensor_core=True))):
         torch.manual_seed(6)
         rec = []
 

@@ -9,9 +9,9 @@ import numpy as np
 import pytest
 import torch
 
-import _act_oracle as act
-import _xent_oracle as xo
-from _xent_oracle import MLP, XentOracleBackend
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
+from _oracle_backend import OracleBackend
 import estorch_b200 as E
 from estorch_b200 import _capi
 
@@ -43,10 +43,10 @@ def test_header_and_binding_agree_on_the_code():
 def test_support_probe_serves_every_shape_and_leaves_f16_unchanged():
     lib = _lib()
     F16_ANY = _capi.ESTK_PREC_F16_ANY
-    assert _supported(lib, [784, 100, 10], xo.LOSS_XENT, F16_ANY, 100) == 1
-    assert _supported(lib, [3072, 512, 10], xo.LOSS_XENT, F16_ANY, 256) == 1
+    assert _supported(lib, [784, 100, 10], mlp.LOSS_XENT, F16_ANY, 100) == 1
+    assert _supported(lib, [3072, 512, 10], mlp.LOSS_XENT, F16_ANY, 256) == 1
     assert _supported(lib, [4, 64, 64, 2], 0, F16_ANY, 1) == 1
-    assert _supported(lib, [1, 1], act.ACT_TANH | act.ACT_OUT_TANH, F16_ANY, 60000) == 1
+    assert _supported(lib, [1, 1], mlp.ACT_TANH | mlp.ACT_OUT_TANH, F16_ANY, 60000) == 1
     assert _supported(lib, [128, 512, 512, 288], 0, F16_ANY, 256) == 1           # a rule shape too
     for code in (2, 0x200, 0x10101, 0x20000, 0x10200, 0x10100, 0x1000000, 0x10002):
         assert _supported(lib, [784, 100, 10], code, F16_ANY, 100) == 0, hex(code)
@@ -58,7 +58,7 @@ def test_support_probe_serves_every_shape_and_leaves_f16_unchanged():
         assert _supported(lib, [64, 64, 32], 0, prec, 100) == 0
         assert _supported(lib, [64, 64, 32], 0, prec, 256) == 1
     assert _supported(lib, [320, 64, 32], 0, _capi.ESTK_PREC_F16, 256) == 0
-    assert _supported(lib, [64, 64, 10], xo.LOSS_XENT, _capi.ESTK_PREC_F16, 256) == 0
+    assert _supported(lib, [64, 64, 10], mlp.LOSS_XENT, _capi.ESTK_PREC_F16, 256) == 0
     for prec in (_capi.ESTK_PREC_FP32, 5, -1):
         assert _supported(lib, [64, 64, 32], 0, prec, 256) == 0
 
@@ -66,7 +66,7 @@ def test_support_probe_serves_every_shape_and_leaves_f16_unchanged():
 def test_null_arguments_are_refused_before_any_cuda_call():
     from estorch_b200.backend import mlp_desc
     lib = _lib()
-    d = mlp_desc([784, 100, 10], xo.LOSS_XENT)
+    d = mlp_desc([784, 100, 10], mlp.LOSS_XENT)
     fake = C.c_void_p(16)                    # never dereferenced: the checks fail first
     args = dict(ctx=fake, desc=C.byref(d), theta=fake, theta16=None, table=fake, table16=fake, offsets=fake,
                 obs=fake, target=fake, rp=fake, rm=fake)
@@ -82,28 +82,24 @@ def test_null_arguments_are_refused_before_any_cuda_call():
 
 
 # ------------------------------------------------------------------ ES routing with a stand-in backend
-class AnyShapeBackend(XentOracleBackend):
-    """Stand-in with the "f16_any" precision: the f16 emulation on every shape, no folded centre."""
+class AnyShapeBackend(OracleBackend):
+    """Stand-in that records the evaluate precisions; ``with_f16_any=False`` answers no to every "f16_any" probe."""
 
     def __init__(self, with_f16_any=True):
         super().__init__(tensor_core=True)
         self.precisions = set()
-        if with_f16_any:
-            self.eval_supports_f16_any = lambda dims, B, act=0: act in ACT_CODES and B >= 1
+        if not with_f16_any:
+            self.eval_supports_f16_any = lambda dims, B, act=0: False
 
     def eval_mlp(self, *a, precision="fp32", centre_out=None, **kw):
         self.precisions.add(precision)
         if precision == "f16_any":
             assert centre_out is None
-            precision = "f16"
         return super().eval_mlp(*a, precision=precision, centre_out=centre_out, **kw)
 
     def eval_mlp_center(self, *a, precision="fp32", **kw):
         self.precisions.add(precision)
-        return super().eval_mlp_center(*a, precision="f16" if precision == "f16_any" else precision, **kw)
-
-
-ACT_CODES = act.ALL_ACTS + xo.XENT_ACTS
+        return super().eval_mlp_center(*a, precision=precision, **kw)
 
 
 def _es(dims, B, eval_precision, loss="cross_entropy", be=None):
@@ -147,7 +143,8 @@ def test_bf16_off_rule_still_raises(mode):
         _es(*OFF_RULE, mode)
 
 
-def test_backend_without_f16_any_behaves_as_before():
+def test_backend_refusing_f16_any_behaves_as_before():
+    """A backend whose f16_any probe answers no: off-rule "f16" is refused, on-rule "f16" keeps the cluster kernel."""
     with pytest.raises(ValueError, match="multiples of 64"):
         _es(*OFF_RULE, "f16", be=AnyShapeBackend(with_f16_any=False))
     assert _es(*ON_RULE, "f16", be=AnyShapeBackend(with_f16_any=False))[0]._precision == "f16"

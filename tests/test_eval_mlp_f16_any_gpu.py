@@ -1,8 +1,8 @@
 """ESTK_PREC_F16_ANY on the H100: the F16 arithmetic for every MLP shape.  The streamed wgmma kernel
-(estk_eval_mlp_tc_stream.cu) against the f16 emulation and the exact fp32 forward (tests/_act_oracle.py,
-tests/_xent_oracle.py), bit agreement with the cluster kernel, run-to-run bits, the ABI, workspace growth
-under CUDA graphs, kernel selection and the launch counter read from torch.profiler, and ES / NSR-ES runs
-with eval_precision="f16" through the public API."""
+(estk_eval_mlp_tc_stream.cu) against the f16 emulation and the exact fp32 forward (tests/_mlp_oracle.py), bit
+agreement with the cluster kernel, run-to-run bits, the ABI, workspace growth under CUDA graphs, kernel selection
+and the launch counter read from torch.profiler, and ES / NSR-ES runs with eval_precision="f16" through the public
+API."""
 import json
 import os
 import subprocess
@@ -14,17 +14,16 @@ import torch
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _act_oracle as act
-import _xent_oracle as xo
-from _xent_oracle import MLP
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
 from test_eval_mlp_act_gpu import _set_theta, _tc_problem, dev
 import estorch_b200 as E
 
 pytestmark = pytest.mark.gpu
 
 STREAM, CLUSTER, SPLIT = "eval_mlp_tc_stream_kernel", "eval_mlp_tc_kernel", "split_obs_f16_kernel"
-ALL_CODES = (0, act.ACT_TANH, act.ACT_OUT_TANH, act.ACT_TANH | act.ACT_OUT_TANH, xo.LOSS_XENT,
-             xo.LOSS_XENT | act.ACT_TANH)
+ALL_CODES = (0, mlp.ACT_TANH, mlp.ACT_OUT_TANH, mlp.ACT_TANH | mlp.ACT_OUT_TANH, mlp.LOSS_XENT,
+             mlp.LOSS_XENT | mlp.ACT_TANH)
 
 
 @pytest.fixture(scope="module")
@@ -35,7 +34,7 @@ def be():
 
 def _problem(dims, B, pairs, code, seed=23):
     n, table, theta, obs, tgt, offs = _tc_problem(dims, B, pairs, seed=seed)
-    if code & xo.LOSS_XENT:
+    if code & mlp.LOSS_XENT:
         tgt = np.eye(dims[-1], dtype=np.float32)[np.random.RandomState(seed).randint(0, dims[-1], B)]
     return n, table, theta, obs, tgt, offs
 
@@ -70,14 +69,10 @@ def _centre(be, dims, d, code, bc_obs=0, bc_dim=0):
 
 def _oracle(dims, theta, table, offs, sigma, obs, tgt, code, bc_obs, bc_dim, precision):
     """Returns (and BCs) of pairs `offs`, [plus..., minus...], one pair at a time."""
-    hidden, output = ("tanh" if code & act.ACT_TANH else "relu"), ("tanh" if code & act.ACT_OUT_TANH else "identity")
     rp, rm, bp, bm = [], [], [], []
     for off in offs:
         pop, _ = orc.sample_population(theta, table, np.array([off]), sigma)
-        if code & xo.LOSS_XENT:
-            r, b = xo.evaluate_population(pop, dims, obs, tgt, bc_obs, bc_dim, hidden, precision)
-        else:
-            r, b = act.evaluate_population(pop, dims, obs, tgt, bc_obs, bc_dim, hidden, output, precision)
+        r, b = mlp.evaluate_population(pop, dims, obs, tgt, code, precision, bc_obs, bc_dim)
         rp.append(r[0]); rm.append(r[1])
         if bc_dim:
             bp.append(b[0]); bm.append(b[1])
@@ -85,18 +80,18 @@ def _oracle(dims, theta, table, offs, sigma, obs, tgt, code, bc_obs, bc_dim, pre
 
 
 def _centre_oracle(dims, theta, obs, tgt, code, precision):
-    hidden, output = ("tanh" if code & act.ACT_TANH else "relu"), ("tanh" if code & act.ACT_OUT_TANH else "identity")
-    y = act.FORWARD[precision](theta, list(dims), obs, hidden, output)
-    return float(xo.xent_return(y, tgt) if code & xo.LOSS_XENT else orc.synthetic_return(y, tgt))
+    hidden, output = ("tanh" if code & mlp.ACT_TANH else "relu"), ("tanh" if code & mlp.ACT_OUT_TANH else "identity")
+    y = mlp.FORWARD[precision](theta, list(dims), obs, hidden, output)
+    return float(mlp.xent_return(y, tgt) if code & mlp.LOSS_XENT else orc.synthetic_return(y, tgt))
 
 
 # ------------------------------------------------------------------ returns against the emulation and fp32
 # (dims, B, pairs, code, bc_obs, bc_dim); every one is a shape ESTK_PREC_F16 refuses
 SHAPES = [([4, 64, 64, 2], 1, 8, 0, 0, 0),
           ([4, 64, 64, 2], 256, 8, 0, 0, 0),
-          ([784, 256, 10], 100, 4, xo.LOSS_XENT, 0, 0),
-          ([784, 256, 10], 1000, 4, xo.LOSS_XENT, 8, 64),        # ragged last chunk
-          ([3072, 512, 10], 256, 3, xo.LOSS_XENT, 0, 0),
+          ([784, 256, 10], 100, 4, mlp.LOSS_XENT, 0, 0),
+          ([784, 256, 10], 1000, 4, mlp.LOSS_XENT, 8, 64),        # ragged last chunk
+          ([3072, 512, 10], 256, 3, mlp.LOSS_XENT, 0, 0),
           ([320, 64, 32], 256, 4, 0, 0, 0),
           ([64, 1024, 1024, 32], 128, 3, 0, 0, 0),
           ([24, 64, 64, 4], 256, 6, 0, 64, 256),
@@ -146,8 +141,8 @@ def test_streamed_bcs_equal_cluster_kernel_bits(be, dims):
 
 
 # ------------------------------------------------------------------ determinism and special cases
-@pytest.mark.parametrize("dims,B,code", [([784, 256, 10], 200, xo.LOSS_XENT), ([320, 64, 32], 100, act.ACT_TANH),
-                                         ([24, 64, 64, 4], 300, act.ACT_OUT_TANH)])
+@pytest.mark.parametrize("dims,B,code", [([784, 256, 10], 200, mlp.LOSS_XENT), ([320, 64, 32], 100, mlp.ACT_TANH),
+                                         ([24, 64, 64, 4], 300, mlp.ACT_OUT_TANH)])
 def test_bits_repeat_with_and_without_order_and_sigma0_is_centre(be, dims, B, code):
     pairs = 150
     n, table, theta, obs, tgt, offs = _problem(dims, B, pairs, code, seed=8)
@@ -185,7 +180,7 @@ def test_abi_centre_fold_alignment_and_codes(be):
                     precision="f16_any", table16=d.tb16)
     with pytest.raises(RuntimeError, match=r"estk_status -1\)"):      # a population needs table16
         be.eval_mlp(dims, d.th, d.tb, dev(be, offs), None, 2, 0.02, d.ob, d.tg, ret[:2], ret[2:], precision="f16_any")
-    for bad in (2, 0x200, xo.LOSS_XENT | act.ACT_OUT_TANH, 1 << 24):
+    for bad in (2, 0x200, mlp.LOSS_XENT | mlp.ACT_OUT_TANH, 1 << 24):
         assert not be.eval_supports_f16_any(dims, B, act=bad)
         with pytest.raises(RuntimeError, match=r"estk_status -3\)"):
             be.eval_mlp(dims, d.th, d.tb, dev(be, offs), None, 2, 0.02, d.ob, d.tg, ret[:2], ret[2:],
@@ -288,7 +283,7 @@ def test_launch_counter_matches_profiled_kernels_in_fused_generations():
         os.environ["ESTORCH_B200_GRAPH"] = "0"
         import numpy as np, torch
         import estorch_b200 as E
-        from _xent_oracle import MLP
+        from _mlp_oracle import MLP
         root = sys.argv[1]
         names = set()
         for path in glob.glob(os.path.join(root, "estorch_b200", "csrc", "*.cu")):

@@ -1,6 +1,6 @@
 """The streamed fp32 evaluate (eval_mlp_wide_kernel, estk_eval_mlp.cu) on the H100: the shapes the
 shared-memory fp32 kernel cannot hold -- layers wider than 1080 and batches of more than 64 chunks --
-against the oracle's fp32 forwards (tests/_act_oracle.py, tests/_xent_oracle.py), run-to-run and
+against the oracle's fp32 forwards (tests/_mlp_oracle.py), run-to-run and
 order-independent bits, kernel selection read from torch.profiler, workspace growth and CUDA-graph
 capture, and ES / NSR-ES runs through the public API."""
 import json
@@ -14,9 +14,9 @@ import torch
 
 from conftest import rel_err
 from oracle import es_oracle as orc
-import _act_oracle as act
-import _xent_oracle as xo
-from _xent_oracle import MLP, XentOracleBackend
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
+from _oracle_backend import OracleBackend
 from test_eval_mlp_act_gpu import _tc_problem, dev
 import estorch_b200 as E
 
@@ -33,7 +33,7 @@ def be():
 
 def _problem(dims, B, pairs, code, seed=3):
     n, table, theta, obs, tgt, offs = _tc_problem(dims, B, pairs, seed=seed)
-    if code & xo.LOSS_XENT:
+    if code & mlp.LOSS_XENT:
         tgt = np.eye(dims[-1], dtype=np.float32)[np.random.RandomState(seed).randint(0, dims[-1], B)]
     return n, table, theta, obs, tgt, offs
 
@@ -51,14 +51,10 @@ def _run(be, dims, theta, table, offs, sigma, obs, tgt, code, bc_obs=0, bc_dim=0
 
 def _oracle(dims, theta, table, offs, sigma, obs, tgt, code, bc_obs=0, bc_dim=0):
     """Returns (and BCs) of pairs `offs`, [plus..., minus...], one pair at a time (wide rows are large)."""
-    hidden, output = ("tanh" if code & act.ACT_TANH else "relu"), ("tanh" if code & act.ACT_OUT_TANH else "identity")
     rp, rm, bp, bm = [], [], [], []
     for off in offs:
         pop, _ = orc.sample_population(theta, table, np.array([off]), sigma)
-        if code & xo.LOSS_XENT:
-            r, b = xo.evaluate_population(pop, dims, obs, tgt, bc_obs, bc_dim, hidden)
-        else:
-            r, b = act.evaluate_population(pop, dims, obs, tgt, bc_obs, bc_dim, hidden, output)
+        r, b = mlp.evaluate_population(pop, dims, obs, tgt, code, "fp32", bc_obs, bc_dim)
         rp.append(r[0]); rm.append(r[1])
         if bc_dim:
             bp.append(b[0]); bm.append(b[1])
@@ -82,15 +78,15 @@ def _kernels(fn):
 # (dims, B, pairs, code, bc_obs, bc_dim): pairs x chunks of 64 observations > the SMs' persistent CTAs
 SHAPES = [([1088, 64, 8], 256, 40, 0, 0, 0),
           ([16, 64, 2000], 256, 40, 0, 64, 256),
-          ([32, 2048, 2048, 4], 128, 80, act.ACT_TANH | act.ACT_OUT_TANH, 0, 0),
-          ([3072, 256, 10], 256, 40, xo.LOSS_XENT, 0, 0),
+          ([32, 2048, 2048, 4], 128, 80, mlp.ACT_TANH | mlp.ACT_OUT_TANH, 0, 0),
+          ([3072, 256, 10], 256, 40, mlp.LOSS_XENT, 0, 0),
           ([32, 4096, 4096, 4], 128, 80, 0, 0, 0),
           ([784, 128, 10], 1024, 12, 0, 0, 0),
-          ([784, 128, 10], 1000, 12, xo.LOSS_XENT, 8, 64),   # ragged last chunk
+          ([784, 128, 10], 1000, 12, mlp.LOSS_XENT, 8, 64),   # ragged last chunk
           ([784, 128, 10], 100, 4, 0, 0, 0),                  # the shared-memory kernel (13 chunks)
           ([784, 128, 10], 1, 4, 0, 0, 0),
-          ([1088, 64, 8], 100, 150, act.ACT_TANH, 0, 0),      # ragged, one chunk per pair
-          ([1088, 64, 8], 1, 150, xo.LOSS_XENT | act.ACT_TANH, 0, 0),
+          ([1088, 64, 8], 100, 150, mlp.ACT_TANH, 0, 0),      # ragged, one chunk per pair
+          ([1088, 64, 8], 1, 150, mlp.LOSS_XENT | mlp.ACT_TANH, 0, 0),
           ([784, 128, 10], 60000, 2, 0, 0, 0)]                # full-batch MNIST: 938 chunks per pair
 
 
@@ -108,15 +104,15 @@ def test_wide_returns_vs_oracle(be, dims, B, pairs, code, bc_obs, bc_dim):
         assert rel_err(got_bc[idx], want_bc) < 1e-5
     one = be.zeros(1)
     be.eval_mlp_center(dims, th, ob, tg, one, act=code)
-    hidden, output = ("tanh" if code & act.ACT_TANH else "relu"), ("tanh" if code & act.ACT_OUT_TANH else "identity")
-    y = act.mlp_forward(theta, dims, obs, hidden, output)
-    w = float(xo.xent_return(y, tgt) if code & xo.LOSS_XENT else orc.synthetic_return(y, tgt))
+    hidden, output = ("tanh" if code & mlp.ACT_TANH else "relu"), ("tanh" if code & mlp.ACT_OUT_TANH else "identity")
+    y = orc.mlp_forward(theta, dims, obs, hidden, output)
+    w = float(mlp.xent_return(y, tgt) if code & mlp.LOSS_XENT else orc.synthetic_return(y, tgt))
     assert abs(float(one) - w) < 1e-5 * abs(w)
 
 
 # ------------------------------------------------------------------ determinism
-@pytest.mark.parametrize("dims,B,code", [([1088, 64, 8], 256, 0), ([3072, 256, 10], 200, xo.LOSS_XENT),
-                                         ([784, 128, 10], 2000, act.ACT_TANH)])
+@pytest.mark.parametrize("dims,B,code", [([1088, 64, 8], 256, 0), ([3072, 256, 10], 200, mlp.LOSS_XENT),
+                                         ([784, 128, 10], 2000, mlp.ACT_TANH)])
 def test_wide_bits_repeat_with_and_without_order_and_sigma0_is_centre(be, dims, B, code):
     pairs = 150
     n, table, theta, obs, tgt, offs = _problem(dims, B, pairs, code, seed=8)
@@ -223,7 +219,7 @@ def test_es_wide_xent_fused_fp32_vs_oracle_standin_and_graph(monkeypatch):
     assert es._fused and es._be.name == "cuda" and es._precision == "fp32"
     table = es._table.cpu()
     es.train(n_steps=3)
-    ref, rref = _xent_es(XentOracleBackend(), "0", monkeypatch)
+    ref, rref = _xent_es(OracleBackend(), "0", monkeypatch)
     ref._table.copy_(table)
     ref.train(n_steps=3)
     (r_c, ep_c, _), (r_o, ep_o, _) = rec[0], rref[0]

@@ -15,12 +15,11 @@ import torch
 import estorch_b200.estorch as E
 from estorch_b200 import DeviceAgent, SequenceAgent, _capi, batch_indices
 from conftest import ROOT, rel_err
-from _batch_oracle import BatchOracleBackend, dataset, with_batches
-from _cnn_oracle import CnnOracleBackend, image_task, pack, policy_class as cnn_policy_class
+from _batch_oracle import dataset
+from _cnn_oracle import image_task, pack, policy_class as cnn_policy_class
 from _oracle_backend import OracleBackend
 from _rnn_oracle import policy_class as rnn_policy_class
-from _seq_oracle import SeqOracleBackend
-from _xent_oracle import MLP
+from _mlp_oracle import MLP
 
 
 # ------------------------------------------------------------------ the restatement
@@ -162,19 +161,19 @@ def _es(cls=E.ES, policy=MLP, dims=(3, 8, 2), n=40, b=8, backend=None, agent=Dev
     return cls(policy, agent, optimizer, population_size=kw.pop("P", 8), sigma=0.05,
                policy_kwargs=kw.pop("policy_kwargs", {"dims": list(dims)}), agent_kwargs=agent_kwargs,
                optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, noise_seed=5,
-               _backend=backend or BatchOracleBackend(), **kw)
+               _backend=backend or OracleBackend(), **kw)
 
 
 def test_es_adam_with_a_sampling_agent_is_fused_for_an_mlp_a_cnn_and_a_sequence_agent():
     es = _es()
     assert es._fused and es._sampling and es._data_obs.shape == (40, 3) and es._obs.shape == (8, 3)
     x, y = image_task(30, (1, 12, 12), seed=2)
-    cnn = _es(policy=cnn_policy_class(2, "relu"), backend=with_batches(CnnOracleBackend)(),
+    cnn = _es(policy=cnn_policy_class(2, "relu"), backend=OracleBackend(),
               policy_kwargs={"dims": pack((1, 12, 12), [(4, 3, 2, 1), (6, 3, 2, 0)], [8, 4])},
               agent_kwargs=dict(obs=x, target=y, loss="cross_entropy", batch_size=6))
     assert cnn._fused and cnn._is_cnn and cnn._sampling and cnn._obs.shape == (6, 1, 12, 12)
     g = torch.Generator().manual_seed(9)
-    seq = _es(policy=rnn_policy_class("gru", True), backend=with_batches(SeqOracleBackend)(), agent=SequenceAgent,
+    seq = _es(policy=rnn_policy_class("gru", True), backend=OracleBackend(), agent=SequenceAgent,
               policy_kwargs={"dims": (3, 8, 2)},
               agent_kwargs=dict(obs=torch.randn(25, 4, 3, generator=g), target=torch.rand(25, 4, 2, generator=g),
                                 batch_size=5))
@@ -190,7 +189,7 @@ def test_the_post_update_rollout_is_never_deferred_while_sampling():
     for b in (None, 256):
         x, y = dataset(512, 64, 32)
         kw = dict(obs=x[:256], target=y[:256]) if b is None else dict(obs=x, target=y, batch_size=b)
-        es = _es(dims=(64, 64, 32), agent_kwargs=kw, backend=BatchOracleBackend(tensor_core=True),
+        es = _es(dims=(64, 64, 32), agent_kwargs=kw, backend=OracleBackend(tensor_core=True),
                  eval_precision="bf16", log_interval=4)
         es.n_steps, es.step = 8, 0
         runs[b] = es._defers_centre()
@@ -237,7 +236,7 @@ def _run(es, n):
 def test_fused_sampling_equals_the_same_rows_through_next_batch():
     x, y = dataset(37, 3, 2, seed=4)
     torch.manual_seed(1)
-    be = BatchOracleBackend()
+    be = OracleBackend()
     a_rec, a_theta = _run(_es(agent_kwargs=dict(obs=x, target=y, batch_size=8, batch_seed=3), backend=be), 3)
     assert be.batch_calls == 3
     torch.manual_seed(1)

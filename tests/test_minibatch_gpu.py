@@ -3,6 +3,7 @@
 alignment, a captured call replays the next batches as the counter advances, ``ES.train`` with ``batch_size`` is
 bit-identical to the same rows fed through ``next_batch`` in every evaluate mode (and replays from a CUDA graph),
 resume, two GPUs where present, and the minibatch example learns."""
+import gc
 import os
 import subprocess
 import sys
@@ -14,7 +15,7 @@ import torch
 import estorch_b200 as E
 from estorch_b200 import batch_indices
 from conftest import ROOT
-from _xent_oracle import MLP
+from _mlp_oracle import MLP
 
 pytestmark = pytest.mark.gpu
 
@@ -150,6 +151,9 @@ def _streamed(obs, tgt, seed, b, base):
 
 
 def _train(policy, agent, agent_kwargs, policy_kwargs, n_steps=5, **kw):
+    # free the earlier cases' engines now (``es.log`` closes over its engine, a cycle): a collection during a
+    # later graph capture would release their pinned batches there and invalidate the capture
+    gc.collect()
     torch.manual_seed(11)
     es = E.ES(policy, agent, torch.optim.Adam, population_size=kw.pop("P", 64), sigma=0.02,
               policy_kwargs=policy_kwargs, agent_kwargs=agent_kwargs, optimizer_kwargs={"lr": 0.01},

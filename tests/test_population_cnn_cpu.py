@@ -16,8 +16,8 @@ from estorch_b200.policy_spec import CNNSpec, cnn_spec_from_module
 from conftest import ROOT, load_golden, rel_err
 from oracle import es_oracle as orc
 from _cnn_oracle import forward, pack, policy_class
-from _pop_cnn_oracle import (DIMS, ES_POLICY, NSR_POLICY, OBS_SHAPE, PixelPoint, PopCnnOracleBackend,
-                             cnn_policy)
+from _oracle_backend import OracleBackend
+from _pop_cnn_oracle import DIMS, ES_POLICY, NSR_POLICY, OBS_SHAPE, PixelPoint, cnn_policy
 
 CODE = 0 | (1 << 8) | (2 << 24)        # ReLU hidden, Tanh output, two convs (ES_POLICY)
 
@@ -26,7 +26,7 @@ def _es(cls=E.ES, optimizer=torch.optim.Adam, P=8, bc_dim=0, agent=PixelPoint, p
         backend=None, **kw):
     es = cls(cnn_policy(**policy), agent, optimizer, population_size=P, sigma=0.05, policy_kwargs={"dims": DIMS},
              agent_kwargs={"horizon": horizon, "bc_dim": bc_dim}, optimizer_kwargs={"lr": 0.01},
-             noise_table_size=1 << 14, _backend=backend or PopCnnOracleBackend(), **kw)
+             noise_table_size=1 << 14, _backend=backend or OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -69,7 +69,7 @@ def test_the_global_rng_is_untouched_and_existing_specs_unchanged():
     class ShapedWalker(LinearWalker):
         obs_shape = (1, 4, 6)
     es = E.ES(MLP, ShapedWalker, torch.optim.Adam, population_size=8, sigma=0.05, policy_kwargs={"dims": [24, 8, 4]},
-              agent_kwargs={"horizon": 2}, noise_table_size=1 << 13, _backend=PopCnnOracleBackend())
+              agent_kwargs={"horizon": 2}, noise_table_size=1 << 13, _backend=OracleBackend())
     assert type(es._spec).__name__ == "MLPSpec" and not es._is_cnn
 
 
@@ -113,7 +113,7 @@ def test_hooks_mode_serves_everything_else(case, monkeypatch):
         # would still be refused
         g = torch.Generator().manual_seed(4)
         es = E.ES(cnn_policy(**ES_POLICY), SequenceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
-                  policy_kwargs={"dims": DIMS}, noise_table_size=1 << 14, _backend=PopCnnOracleBackend(),
+                  policy_kwargs={"dims": DIMS}, noise_table_size=1 << 14, _backend=OracleBackend(),
                   agent_kwargs=dict(obs=torch.randn(3, 2, 128, generator=g), target=torch.randn(3, 2, 2, generator=g)))
         assert not es._fused and not es._is_cnn
         es._spec = CNNSpec(OBS_SHAPE, ((4, 3, 1, 1), (8, 3, 2, 0)), (16, 2), "relu", "tanh")
@@ -271,11 +271,11 @@ def check_nsr_golden(es, g):
 
 
 def test_es_population_mode_matches_reference_golden():
-    check_es_golden(*run_es_golden(PopCnnOracleBackend()))
+    check_es_golden(*run_es_golden(OracleBackend()))
 
 
 def test_nsr_population_mode_matches_reference_golden():
-    check_nsr_golden(*run_nsr_golden(PopCnnOracleBackend()))
+    check_nsr_golden(*run_nsr_golden(OracleBackend()))
 
 
 # ------------------------------------------------------------------ population mode against hooks mode

@@ -13,7 +13,8 @@ import estorch_b200.estorch as E
 from estorch_b200 import _capi
 from conftest import ROOT, load_golden, rel_err
 from oracle import es_oracle as orc
-from _pop_conv_oracle import (STATS_FLOATS, AtariPolicy, PixelWalker, PopConvOracleBackend, conv_act, conv_stats,
+from _oracle_backend import OracleBackend
+from _pop_conv_oracle import (STATS_FLOATS, AtariPolicy, PixelWalker, conv_act, conv_stats,
                               golden_table, golden_theta0, theta_subset, walker_xref)
 
 A = 4
@@ -22,7 +23,7 @@ A = 4
 def _es(cls=E.ES, optimizer=torch.optim.Adam, P=8, bc_dim=0, backend=None, horizon=3, **kw):
     es = cls(AtariPolicy, PixelWalker, optimizer, population_size=P, sigma=0.05,
              policy_kwargs={"n_actions": A, "xref": walker_xref(4)}, agent_kwargs={"horizon": horizon, "bc_dim": bc_dim},
-             optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 20, _backend=backend or PopConvOracleBackend(),
+             optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 20, _backend=backend or OracleBackend(),
              **kw)
     es.log = lambda: None
     return es
@@ -212,11 +213,11 @@ def check_nsr_golden(es, g):
 
 
 def test_es_population_mode_matches_reference_golden():
-    check_es_golden(*run_es_golden(PopConvOracleBackend()))
+    check_es_golden(*run_es_golden(OracleBackend()))
 
 
 def test_nsr_population_mode_matches_reference_golden():
-    check_nsr_golden(*run_nsr_golden(PopConvOracleBackend()))
+    check_nsr_golden(*run_nsr_golden(OracleBackend()))
 
 
 # ------------------------------------------------------------------ population mode against hooks mode

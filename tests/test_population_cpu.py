@@ -1,6 +1,6 @@
 """Population mode (estorch_b200.PopulationAgent) without a GPU: mode selection, the member order of
 ``act``, the reference goldens reproduced through ES / NSR-ES on the oracle stand-in
-(tests/_pop_oracle.py), population mode against hooks mode, checkpoint / resume, the multi-GPU fallback,
+(tests/_oracle_backend.py), population mode against hooks mode, checkpoint / resume, the multi-GPU fallback,
 and the ESTK_ACTIONS code in the header, the binding and the library's support probe."""
 import ctypes as C
 import os
@@ -14,8 +14,9 @@ import estorch_b200.estorch as E
 from estorch_b200 import PopulationAgent, _capi
 from conftest import ROOT, load_golden, rel_err
 from oracle import es_oracle as orc
-from _act_ext_oracle import MLP
-from _pop_oracle import ACTIONS, LinearWalker, PopOracleBackend, act_forward
+from _mlp_oracle import ACTIONS, MLP, act_forward
+from _oracle_backend import OracleBackend
+from _pop_oracle import LinearWalker
 
 DIMS = [24, 64, 64, 4]
 
@@ -24,7 +25,7 @@ def _es(cls=E.ES, optimizer=torch.optim.Adam, policy=MLP, P=16, bc_dim=0, backen
     es = cls(policy, LinearWalker, optimizer, population_size=P, sigma=0.05,
              policy_kwargs={"dims": DIMS, "hidden": "relu", "output": "tanh"} if policy is MLP else {},
              agent_kwargs={"horizon": 6, "bc_dim": bc_dim}, optimizer_kwargs={"lr": 0.01},
-             noise_table_size=1 << 16, _backend=backend or PopOracleBackend(), **kw)
+             noise_table_size=1 << 16, _backend=backend or OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -198,11 +199,11 @@ def check_nsr_golden(es, g):
 
 
 def test_es_population_mode_matches_reference_golden():
-    check_es_golden(*run_es_golden(PopOracleBackend()))
+    check_es_golden(*run_es_golden(OracleBackend()))
 
 
 def test_nsr_population_mode_matches_reference_golden():
-    check_nsr_golden(*run_nsr_golden(PopOracleBackend()))
+    check_nsr_golden(*run_nsr_golden(OracleBackend()))
 
 
 # ------------------------------------------------------------------ population mode against hooks mode

@@ -15,7 +15,8 @@ from estorch_b200 import DeviceAgent, _capi
 from estorch_b200.policy_spec import RNNSpec, rnn_spec_from_module
 from conftest import ROOT, load_golden, rel_err
 from oracle import es_oracle as orc
-from _rnn_oracle import (ACTIONS, CELL_GRU, CELL_LSTM, RecallAgent, RnnOracleBackend, param_count, policy_class,
+from _oracle_backend import OracleBackend
+from _rnn_oracle import (ACTIONS, CELL_GRU, CELL_LSTM, RecallAgent, param_count, policy_class,
                          state_width, step32)
 
 DIMS = (4, 16, 3)
@@ -24,7 +25,7 @@ DIMS = (4, 16, 3)
 def _es(cls=E.ES, optimizer=torch.optim.Adam, cell="gru", out_tanh=True, P=16, bc_dim=0, **kw):
     es = cls(policy_class(cell, out_tanh), RecallAgent, optimizer, population_size=P, sigma=0.05,
              policy_kwargs={"dims": DIMS}, agent_kwargs={"bc_dim": bc_dim}, optimizer_kwargs={"lr": 0.01},
-             noise_table_size=1 << 14, _backend=RnnOracleBackend(), **kw)
+             noise_table_size=1 << 14, _backend=OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -128,7 +129,7 @@ def test_hooks_mode_serves_everything_else(case, monkeypatch):
     if case == "device_agent":
         es = E.ES(policy_class("gru", True), DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
                   policy_kwargs={"dims": DIMS}, agent_kwargs={"obs": torch.zeros(2, 4), "target": torch.zeros(2, 3)},
-                  noise_table_size=1 << 14, _backend=RnnOracleBackend())
+                  noise_table_size=1 << 14, _backend=OracleBackend())
         assert es._is_rnn and not es._fused and not es._population
         return
     es = _es(**kw)
@@ -300,11 +301,11 @@ def check_nsr_golden(es, g):
 
 
 def test_es_gru_population_mode_matches_reference_golden():
-    check_es_golden(*run_es_golden(RnnOracleBackend()))
+    check_es_golden(*run_es_golden(OracleBackend()))
 
 
 def test_nsr_lstm_population_mode_matches_reference_golden():
-    check_nsr_golden(*run_nsr_golden(RnnOracleBackend()))
+    check_nsr_golden(*run_nsr_golden(OracleBackend()))
 
 
 # ------------------------------------------------------------------ population mode against hooks mode

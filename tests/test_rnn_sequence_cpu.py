@@ -16,7 +16,8 @@ import estorch_b200.estorch as E
 from estorch_b200 import DeviceAgent, SequenceAgent, _capi
 from conftest import ROOT, load_golden, rel_err
 from _rnn_oracle import CELL_GRU, CELL_LSTM, policy_class
-from _seq_oracle import SeqOracleBackend, memoryless_best, recall_dataset, seq_outputs32, seq_returns32
+from _oracle_backend import OracleBackend
+from _seq_oracle import memoryless_best, recall_dataset, seq_outputs32, seq_returns32
 from test_population_rnn_cpu import _load_theta, _Rec, check_es_golden, check_nsr_golden
 
 DIMS = (3, 8, 2)
@@ -32,7 +33,7 @@ def _es(cls=E.ES, cell="gru", out_tanh=True, optimizer=torch.optim.Adam, agent=S
     obs, tgt = _data()
     es = cls(policy_class(cell, out_tanh), agent, optimizer, population_size=P, sigma=0.05,
              policy_kwargs={"dims": dims}, agent_kwargs=agent_kwargs or dict(obs=obs, target=tgt),
-             optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, _backend=SeqOracleBackend(), **kw)
+             optimizer_kwargs={"lr": 0.02}, noise_table_size=1 << 13, _backend=OracleBackend(), **kw)
     es.log = lambda: None
     return es
 
@@ -115,7 +116,7 @@ def test_hooks_mode_serves_everything_else(case):
     elif case == "mlp_policy":
         from test_api_cpu import MLP
         es = E.ES(MLP, SequenceAgent, torch.optim.Adam, population_size=8, sigma=0.05, policy_kwargs={"dims": [3, 8, 2]},
-                  agent_kwargs=dict(obs=obs, target=tgt), noise_table_size=1 << 13, _backend=SeqOracleBackend())
+                  agent_kwargs=dict(obs=obs, target=tgt), noise_table_size=1 << 13, _backend=OracleBackend())
     elif case == "device_agent":
         es = _es(agent=DeviceAgent, agent_kwargs=dict(obs=obs[:, 0], target=tgt[:, 0]))
     elif case == "sgd":
@@ -211,11 +212,11 @@ def run_nsr_seq_golden(backend):
 
 
 def test_es_gru_sequence_matches_reference_golden():
-    check_es_golden(*run_es_seq_golden(SeqOracleBackend()))
+    check_es_golden(*run_es_seq_golden(OracleBackend()))
 
 
 def test_nsr_lstm_cross_entropy_sequence_matches_reference_golden():
-    check_nsr_golden(*run_nsr_seq_golden(SeqOracleBackend()))
+    check_nsr_golden(*run_nsr_seq_golden(OracleBackend()))
 
 
 def test_the_recall_dataset_needs_memory():

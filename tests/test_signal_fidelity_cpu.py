@@ -8,7 +8,7 @@ import torch
 
 from estorch_b200.estorch import AUTO_F16_MIN_SIGMA
 from oracle import es_oracle as orc
-import _act_ext_oracle as ext
+import _mlp_oracle as mlp
 import _fp64_signal as sig
 
 
@@ -34,7 +34,7 @@ def task(dims, B, loss, obs_scale=1.0, seed=1):
 
 
 # ------------------------------------------------------------------ the helper against torch.float64
-@pytest.mark.parametrize("hidden", sorted(ext.HIDDEN))
+@pytest.mark.parametrize("hidden", sorted(mlp.HIDDEN_CODES))
 @pytest.mark.parametrize("output,loss", [("identity", "mse"), ("tanh", "mse"), ("identity", "xent")])
 def test_reference_matches_torch_float64_sequential(hidden, output, loss):
     dims, B, pairs, sigma = [7, 33, 17, 5], 9, 4, 0.05
@@ -50,7 +50,7 @@ def test_reference_matches_torch_float64_sequential(hidden, output, loss):
     eps = (np.float32(sigma) * table[offs[1]: offs[1] + theta.size]).astype(np.float32)
     np.testing.assert_array_equal(rows[pairs + 1], (theta - eps).astype(np.float32))
     r64, tau = sig.mlp_reference(rows, dims, obs, tgt, hidden, output, loss)
-    net = ext.MLP(dims, hidden, output).double()
+    net = mlp.MLP(dims, hidden, output).double()
     t = torch.from_numpy(tgt).double()
     want = []
     for row in rows:
@@ -63,7 +63,7 @@ def test_reference_matches_torch_float64_sequential(hidden, output, loss):
             want.append(float(-((y - t) ** 2).mean()))
     np.testing.assert_allclose(r64, want, rtol=1e-12, atol=0)
     # the bound covers the fp32 forward, and is not vacuous: within 10^4 ulps of the return
-    r32, _ = ext.evaluate_population(rows, dims, obs, tgt, hidden=hidden, output=output, loss=loss)
+    r32, _ = mlp.evaluate_population(rows, dims, obs, tgt, mlp.code(hidden, output, loss))
     assert np.all(np.abs(r32 - r64) <= tau)
     assert np.all(tau < 1e4 * sig.U32 * np.abs(r64))
 
@@ -108,7 +108,7 @@ def test_fp32_restatements_keep_exact_ranks(scale):
     table, offs = noise(theta.size, pairs)
     obs, tgt = task(dims, 64, "mse")
     rows = sig.members(theta, table, offs, sigma)
-    r32, _ = ext.evaluate_population(rows, dims, obs, tgt)
+    r32, _ = mlp.evaluate_population(rows, dims, obs, tgt)
     pinned["mlp"] = _check_fp32(r32, *sig.mlp_reference(rows, dims, obs, tgt))
     gdims = (5, 32, 3)
     g = np.random.RandomState(3)
@@ -149,7 +149,7 @@ def sweep():
             r64, tau = sig.mlp_reference(rows, SWEEP_DIMS, obs, tgt)
             g64 = sig.gradient64(r64, table, offs, n)
             for mode in ("fp32", "f16", "bf16"):
-                r, _ = ext.evaluate_population(rows, SWEEP_DIMS, obs, tgt, precision=mode)
+                r, _ = mlp.evaluate_population(rows, SWEEP_DIMS, obs, tgt, precision=mode)
                 m = sig.signal_metrics(r, r64, sig.gradient64(r, table, offs, n), g64)
                 m["rank_violations"] = int(sig.rank_violations(r, r64, tau)[0].size)
                 out[mode, scale, sigma] = m
@@ -189,7 +189,8 @@ def test_auto_picks_fp32_below_the_sigma_threshold(sigma, want):
     """``eval_precision="auto"`` on a shape the f16 kernel accepts: "f16" from AUTO_F16_MIN_SIGMA up, "fp32"
     below it; an explicit "f16" is honoured at any sigma."""
     from estorch_b200 import ES, DeviceAgent
-    from _act_ext_oracle import ActExtOracleBackend, MLP
+    from _mlp_oracle import MLP
+    from _oracle_backend import OracleBackend
     dims = [64, 256, 64]
     g = torch.Generator().manual_seed(0)
     obs, tgt = torch.randn(256, 64, generator=g), torch.randn(256, 64, generator=g)
@@ -198,6 +199,6 @@ def test_auto_picks_fp32_below_the_sigma_threshold(sigma, want):
         return ES(MLP, DeviceAgent, torch.optim.Adam, population_size=8, sigma=float(sigma),
                   policy_kwargs={"dims": dims, "hidden": "relu"}, agent_kwargs={"obs": obs, "target": tgt},
                   noise_table_size=1 << 16, eval_precision=precision,
-                  _backend=ActExtOracleBackend(tensor_core=True))
+                  _backend=OracleBackend(tensor_core=True))
     assert make("auto")._precision == want
     assert make("f16")._precision == "f16"

@@ -20,9 +20,9 @@ from estorch_b200 import _capi
 from estorch_b200.backend import CudaBackend
 from estorch_b200.estorch import AUTO_F16_MIN_SIGMA
 from oracle import es_oracle as orc
-import _act_ext_oracle as ext
+import _mlp_oracle as mlp
 import _fp64_signal as sig
-from _act_oracle import ActOracleBackend
+from _oracle_backend import OracleBackend
 
 pytestmark = pytest.mark.gpu
 
@@ -230,15 +230,15 @@ def test_tensor_core_signal_vs_rounding_model_and_domain(be, config, sigma, scal
            g.standard_normal((B, dims[-1])).astype(np.float32))
     th_d = _dev(be, theta)
     ret = _tc_call(be, mode, dims, th_d, table, offs, order, sigma, _dev(be, obs), _dev(be, tgt),
-                   ext.code(hidden, "identity", loss))
+                   mlp.code(hidden, "identity", loss))
     table_h, offs_h = table.cpu().numpy(), offs.cpu().numpy()
     rows = sig.members(theta, table_h, offs_h, sigma)
     r64, _ = sig.mlp_reference(rows, dims, obs, tgt, hidden, "identity", loss)
     model_rows = rows
     if mode == "bf16s":
-        model_rows = ActOracleBackend._exact_biases(orc.sample_population_bf16s(theta, table_h, offs_h, sigma), rows,
-                                                    dims)
-    r_model, _ = ext.evaluate_population(model_rows, dims, obs, tgt, hidden=hidden, precision=mode, loss=loss)
+        model_rows = OracleBackend._exact_biases(orc.sample_population_bf16s(theta, table_h, offs_h, sigma), rows,
+                                                 dims)
+    r_model, _ = mlp.evaluate_population(model_rows, dims, obs, tgt, mlp.code(hidden, "identity", loss), mode)
     _, g64 = sig.device_gradient(be, _dev(be, r64.astype(np.float32)), table, offs, order, th_d)
     _, g = sig.device_gradient(be, ret, table, offs, order, th_d)
     _, g_model = sig.device_gradient(be, _dev(be, r_model), table, offs, order, th_d)

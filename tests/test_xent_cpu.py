@@ -1,6 +1,6 @@
 """Cross-entropy objective without a GPU: ``DeviceAgent(loss="cross_entropy")``, the loss bit of
 ``estk_mlp_desc.activation`` through the library's shape query, the fused / hooks decision, and ES /
-NSR-ES through the oracle stand-in (tests/_xent_oracle.py) against the reference-generated goldens."""
+NSR-ES through the oracle stand-in (tests/_oracle_backend.py) against the reference-generated goldens."""
 import ctypes as C
 import os
 
@@ -10,8 +10,9 @@ import torch
 import torch.nn.functional as F
 
 from conftest import load_golden, rel_err
-import _xent_oracle as xo
-from _xent_oracle import MLP, XentOracleBackend
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP
+from _oracle_backend import OracleBackend
 import estorch_b200 as E
 from estorch_b200 import _capi
 
@@ -42,7 +43,7 @@ def test_rollout_matches_torch_cross_entropy_with_probability_targets():
         want = float(F.cross_entropy(pol(obs), probs))
         logits = pol(obs).numpy()
     assert abs(r + want) <= 1e-6 * abs(want)
-    assert abs(r - float(xo.xent_return(logits, probs.numpy()))) <= 1e-6 * abs(want)
+    assert abs(r - float(mlp.xent_return(logits, probs.numpy()))) <= 1e-6 * abs(want)
 
 
 def test_rollout_with_behaviour_characteristic_returns_the_logits():
@@ -96,7 +97,7 @@ def _supported(lib, dims, act, precision, B=256):
 
 def test_supported_query_accepts_xent_under_the_shape_rule_and_refuses_other_loss_codes():
     lib = _lib()
-    assert _capi.ESTK_LOSS_XENT == xo.LOSS_XENT == 0x10000
+    assert _capi.ESTK_LOSS_XENT == mlp.LOSS_XENT == 0x10000
     north = [128, 512, 512, 512, 512, 256]
     for prec in (_capi.ESTK_PREC_F16, _capi.ESTK_PREC_BF16, _capi.ESTK_PREC_BF16S):
         for code in (0x10000, 0x10001):
@@ -138,7 +139,7 @@ def _es(hidden, output, loss, tensor_core=False, dims=None, B=None):
     rng = np.random.RandomState(3)
     obs = torch.from_numpy(rng.standard_normal((B, dims[0])).astype(np.float32))
     tgt = torch.from_numpy(rng.dirichlet(np.ones(dims[-1]), B).astype(np.float32))
-    be = XentOracleBackend(tensor_core=tensor_core)
+    be = OracleBackend(tensor_core=tensor_core)
     es = E.ES(MLP, E.DeviceAgent, torch.optim.Adam, population_size=8, sigma=0.05,
               policy_kwargs={"dims": dims, "hidden": hidden, "output": output},
               agent_kwargs=dict(obs=obs, target=tgt, loss=loss), optimizer_kwargs={"lr": 0.01},
@@ -163,7 +164,7 @@ def test_cross_entropy_conv_policy_runs_in_hooks_mode():
               optimizer_kwargs={"lr": 0.01}, noise_table_size=1 << 20)
     xent = E.ES(AtariPolicy, E.DeviceAgent, torch.optim.Adam, agent_kwargs=dict(
         obs=obs, target=F.one_hot(torch.tensor([0, 3]), 4).float(), loss="cross_entropy"),
-        _backend=XentOracleBackend(), **kw)
+        _backend=OracleBackend(), **kw)
     assert xent._is_conv and not xent._fused
     xent.agent.loss = "mse"                     # the same policy and batch with the squared error is fused
     assert xent._decide_fused(torch.optim.Adam)
@@ -173,7 +174,7 @@ def test_cross_entropy_conv_policy_runs_in_hooks_mode():
 @pytest.mark.parametrize("tensor_core", [False, True])
 def test_the_loss_bit_reaches_every_evaluate_and_auto_picks_f16(hidden, tensor_core):
     es, be, obs, tgt = _es(hidden, "identity", "cross_entropy", tensor_core)
-    code = xo.LOSS_XENT | (1 if hidden == "tanh" else 0)
+    code = mlp.LOSS_XENT | (1 if hidden == "tanh" else 0)
     assert es._fused and es._act_code() == code
     assert es._precision == ("f16" if tensor_core else "fp32")
     es.train(n_steps=3)
@@ -217,7 +218,7 @@ def test_es_cross_entropy_matches_reference_golden(mode):
         akw["loss"] = "cross_entropy"
     es = R(MLP, agent, torch.optim.Adam, population_size=64, sigma=0.1, policy_kwargs={"dims": dims},
            agent_kwargs=akw, optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]),
-           noise_seed=int(g["noise_seed"]), _backend=XentOracleBackend())
+           noise_seed=int(g["noise_seed"]), _backend=OracleBackend())
     es.rec = []
     assert es._fused == (mode == "fused")
     es._table.copy_(torch.from_numpy(g["table"]))
@@ -249,7 +250,7 @@ def test_nsr_cross_entropy_matches_reference_golden(mode):
     np.random.seed(123)
     es = R(MLP, agent, torch.optim.Adam, population_size=32, sigma=0.02, policy_kwargs={"dims": dims},
            agent_kwargs=akw, optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]),
-           noise_seed=int(g["noise_seed"]), _backend=XentOracleBackend())
+           noise_seed=int(g["noise_seed"]), _backend=OracleBackend())
     es.rec = []
     assert es._fused == (mode == "fused")
     es._table.copy_(torch.from_numpy(g["table"]))
@@ -278,6 +279,6 @@ def test_oracle_cross_entropy_reproduces_the_golden_returns():
     g = load_golden("es_xent_p64.npz")
     dims = [int(d) for d in g["dims"]]
     pop, _ = orc.sample_population(g["theta_before"][0], g["table"], g["offsets"][0], np.float32(g["sigma"]))
-    rets, _ = xo.evaluate_population(pop, dims, g["obs"], g["target"])
+    rets, _ = mlp.evaluate_population(pop, dims, g["obs"], g["target"], mlp.LOSS_XENT)
     assert rel_err(rets, g["returns"][0][:, 0]) < 2e-6
     assert np.all(g["returns"][0][:, 0] < 0)

@@ -1,5 +1,5 @@
 """Cross-entropy objective (include/estk.h ESTK_LOSS_XENT) on the H100: the fp32 and wgmma MLP evaluate
-kernels against the fp64 cross-entropy of the oracle's forwards (tests/_xent_oracle.py), run-to-run
+kernels against the fp64 cross-entropy of the oracle's forwards (tests/_mlp_oracle.py), run-to-run
 bit equality, large logits, refused codes, ES / NSR-ES against the reference-generated goldens, and the
 north-star accuracy that ``eval_precision="auto"`` rests on."""
 import json
@@ -10,8 +10,9 @@ import torch
 
 from conftest import load_golden, rel_err
 from oracle import es_oracle as orc
-import _xent_oracle as xo
-from _xent_oracle import MLP, XENT_ACTS, XentOracleBackend
+import _mlp_oracle as mlp
+from _mlp_oracle import MLP, XENT_ACTS
+from _oracle_backend import OracleBackend
 from test_eval_mlp_act_gpu import _eval, _set_theta, _tc_problem, dev
 import estorch_b200 as E
 
@@ -47,7 +48,7 @@ def _twice(be, *args, **kw):
                                               ([32, 64, 64, 64, 64, 64, 64, 64, 10], 70, 3, 0),
                                               ([24, 64, 64, 4], 256, 4, 256)])
 def test_fp32_xent_vs_oracle(be, dims, B, pairs, bc, code):
-    hidden = xo.hidden_of(code)
+    hidden = mlp.decode(code)[0]
     rng = np.random.RandomState(7)
     n = orc.mlp_param_count(dims)
     table_len = max(1 << 14, (n + 31) // 32 * 32 + 4096)
@@ -58,13 +59,13 @@ def test_fp32_xent_vs_oracle(be, dims, B, pairs, bc, code):
     offs = orc.noise_offsets(5, 0, 0, pairs, table_len, n)
     ret, bcs, _ = _twice(be, dims, theta, table, offs, 0.02, obs, tgt, code, 64 if bc else 0, bc)
     pop, _ = orc.sample_population(theta, table, offs, 0.02)
-    want, want_bc = xo.evaluate_population(pop, dims, obs, tgt, 64 if bc else 0, bc, hidden)
+    want, want_bc = mlp.evaluate_population(pop, dims, obs, tgt, code, "fp32", 64 if bc else 0, bc)
     assert rel_err(ret, want) < 2e-6
     if bc:
         assert rel_err(bcs, want_bc) < 2e-6
     one = be.zeros(1)
     be.eval_mlp_center(dims, dev(be, theta), dev(be, obs), dev(be, tgt), one, act=code)
-    w = float(xo.xent_return(xo.forward(theta, dims, obs, hidden), tgt))
+    w = float(mlp.xent_return(orc.mlp_forward(theta, dims, obs, hidden), tgt))
     assert abs(float(one) - w) < 2e-6 * abs(w)
 
 
@@ -92,7 +93,6 @@ def _tc_kw(be, mode, theta, table):
 @pytest.mark.parametrize("mode", ["f16", "bf16", "bf16s"])
 @pytest.mark.parametrize("dims", TILE_DIMS)
 def test_tensor_core_xent_vs_emulation_and_fp32(be, dims, mode, code):
-    hidden = xo.hidden_of(code)
     B, pairs, bc = 512, 3, 256
     n, table, theta, obs, _, offs = _tc_problem(dims, B, pairs)
     tgt = _soft_targets(np.random.RandomState(len(dims) + dims[-1]), B, dims[-1])
@@ -100,11 +100,11 @@ def test_tensor_core_xent_vs_emulation_and_fp32(be, dims, mode, code):
     kw = _tc_kw(be, mode, theta, table)
     got, got_bc, centre = _twice(be, dims, theta, table, offs, 0.02, obs, tgt, code, 64, bc, precision=mode,
                                  centre=True, **kw)
-    emu_be = XentOracleBackend(tensor_core=True)
+    emu_be = OracleBackend(tensor_core=True)
     rows = emu_be._rows(torch.from_numpy(theta), torch.from_numpy(table), torch.from_numpy(offs), 0.02, dims, mode)
-    emu, emu_bc = xo.evaluate_population(rows, dims, obs, tgt, 64, bc, hidden, precision=mode)
+    emu, emu_bc = mlp.evaluate_population(rows, dims, obs, tgt, code, mode, 64, bc)
     pop, _ = orc.sample_population(theta, table, offs, 0.02)
-    exact, _ = xo.evaluate_population(pop, dims, obs, tgt, 64, bc, hidden)
+    exact, _ = mlp.evaluate_population(pop, dims, obs, tgt, code, "fp32", 64, bc)
     t_emu, t_exact, t_bc = TC_TOL[mode]
     print(f"{mode} act={code:#x} {dims}: vs emulation {rel_err(got, emu):.2e}, vs fp32 {rel_err(got, exact):.2e}")
     assert rel_err(got, emu) < t_emu
@@ -131,12 +131,12 @@ def test_large_logits_stay_finite_and_match_fp64(be, mode):
     theta[w2:] *= 400.0                                          # the last layer's weights and biases
     tgt = _soft_targets(np.random.RandomState(9), B, dims[-1])
     kw = _tc_kw(be, mode, theta, table) if mode != "fp32" else {}
-    got, _, _ = _twice(be, dims, theta, table, offs, 0.001, obs, tgt, xo.LOSS_XENT, precision=mode, **kw)
-    rows = XentOracleBackend(tensor_core=True)._rows(torch.from_numpy(theta), torch.from_numpy(table),
-                                                     torch.from_numpy(offs), 0.001, dims, mode)
-    logits = xo.forward(rows[0], dims, obs, "relu", mode)
+    got, _, _ = _twice(be, dims, theta, table, offs, 0.001, obs, tgt, mlp.LOSS_XENT, precision=mode, **kw)
+    rows = OracleBackend(tensor_core=True)._rows(torch.from_numpy(theta), torch.from_numpy(table),
+                                                 torch.from_numpy(offs), 0.001, dims, mode)
+    logits = mlp.FORWARD[mode](rows[0], dims, obs)
     assert 100 < np.abs(logits).max() < 1000
-    want, _ = xo.evaluate_population(rows, dims, obs, tgt, precision=mode)
+    want, _ = mlp.evaluate_population(rows, dims, obs, tgt, mlp.LOSS_XENT, mode)
     assert np.all(np.isfinite(got))
     print(f"large logits {mode}: max |y| {np.abs(logits).max():.1f}, vs fp64 {rel_err(got, want):.2e}")
     assert rel_err(got, want) < 1e-5
@@ -157,7 +157,7 @@ def test_refused_codes_return_before_launch_and_leave_the_returns(be):
         torch.cuda.synchronize()
         assert torch.equal(ret.cpu(), torch.full((4,), 7.0))
     # a 10-class head is not a tensor-core shape: refused there, evaluated by the fp32 kernel
-    assert not be.eval_supports_f16([64, 64, 10], B, act=xo.LOSS_XENT)
+    assert not be.eval_supports_f16([64, 64, 10], B, act=mlp.LOSS_XENT)
 
 
 # ------------------------------------------------------------------ public API vs the reference goldens
@@ -174,7 +174,7 @@ def test_es_fused_xent_vs_reference_golden():
            agent_kwargs=dict(obs=torch.from_numpy(g["obs"]), target=torch.from_numpy(g["target"]),
                              loss="cross_entropy"),
            optimizer_kwargs={"lr": 0.01}, noise_table_size=len(g["table"]), noise_seed=int(g["noise_seed"]))
-    assert es._fused and es._be.name == "cuda" and es._act_code() == xo.LOSS_XENT
+    assert es._fused and es._be.name == "cuda" and es._act_code() == mlp.LOSS_XENT
     es._table.copy_(torch.from_numpy(g["table"]))
     _set_theta(es.policy, g["theta0"])
     es.train(n_steps=3)
@@ -260,14 +260,14 @@ def test_north_star_xent_accuracy_per_mode(be):
     for mode in ("fp32", "f16", "bf16", "bf16s"):
         r = be.zeros(P)
         be.eval_mlp(dims, th_d, table, offs, order, pairs, sigma, obs_d, tgt_d, r[:pairs], r[pairs:], precision=mode,
-                    act=xo.LOSS_XENT, **extra[mode])
+                    act=mlp.LOSS_XENT, **extra[mode])
         res[mode] = r.cpu().numpy()
     tab_h, offs_h, th_h = table.cpu().numpy(), offs.cpu().numpy(), theta.numpy()
     sel = np.arange(0, pairs, pairs // 256)
     want_p, want_m = [], []
     for c in range(0, sel.size, 32):
         pop, _ = orc.sample_population(th_h, tab_h, offs_h[sel[c: c + 32]], sigma)
-        w, _ = xo.evaluate_population(pop, dims, obs.numpy(), tgt.numpy())
+        w, _ = mlp.evaluate_population(pop, dims, obs.numpy(), tgt.numpy(), mlp.LOSS_XENT)
         want_p.append(w[:len(w) // 2])
         want_m.append(w[len(w) // 2:])
     want = np.concatenate(want_p + want_m)
