@@ -230,11 +230,12 @@ __global__ void __launch_bounds__(kThreadsTC, 1) eval_mlp_tc_kernel(const EvalTC
           const uint32_t h2 = pack16<F16>(x1.x, x1.y), h3 = pack16<F16>(x1.z, x1.w);
           st_shared_v4(addr, h0, h1, h2, h3);
           if constexpr (F16) {
-            // x_lo = rn_f16(x - x_hi): the observation enters layer 0 with ~22 significant bits
+            // x_lo = rn_f16(x - x_hi): the observation enters layer 0 with ~22 significant bits (an infinity, or
+            // |x| >= 131024, as a non-finite x_lo: pack_f16_lo)
             const float2 f0 = unpack_f16(h0), f1 = unpack_f16(h1), f2 = unpack_f16(h2), f3 = unpack_f16(h3);
-            st_shared_v4(addr + (K0 / kBlockK) * kHBlockBytes, pack_f16(x0.x - f0.x, x0.y - f0.y),
-                         pack_f16(x0.z - f1.x, x0.w - f1.y), pack_f16(x1.x - f2.x, x1.y - f2.y),
-                         pack_f16(x1.z - f3.x, x1.w - f3.y));
+            st_shared_v4(addr + (K0 / kBlockK) * kHBlockBytes, pack_f16_lo(x0.x - f0.x, x0.y - f0.y),
+                         pack_f16_lo(x0.z - f1.x, x0.w - f1.y), pack_f16_lo(x1.x - f2.x, x1.y - f2.y),
+                         pack_f16_lo(x1.z - f3.x, x1.w - f3.y));
           }
         }
       }

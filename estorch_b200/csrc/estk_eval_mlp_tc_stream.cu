@@ -91,7 +91,7 @@ __global__ void __launch_bounds__(256) split_obs_f16_kernel(const float* __restr
     for (int q = 0; q < 4; ++q) {
       hi[q] = pack_f16(x[2 * q], x[2 * q + 1]);
       const float2 f = unpack_f16(hi[q]);
-      lo[q] = pack_f16(x[2 * q] - f.x, x[2 * q + 1] - f.y);
+      lo[q] = pack_f16_lo(x[2 * q] - f.x, x[2 * q + 1] - f.y);   // non-finite beyond the fp16 split's range
     }
     uint8_t* tile = xin + t * 2 * kABytes + sw128_offset(r, c8);
     *reinterpret_cast<uint4*>(tile) = make_uint4(hi[0], hi[1], hi[2], hi[3]);

@@ -133,6 +133,15 @@ __device__ __forceinline__ uint32_t pack_f16_relu(float lo, float hi) {
   asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+// x_lo of layer 0's fp16 split, without satfinite: where x - x_hi is beyond the fp16 range (x = +-inf, or a finite
+// |x| >= 131024 = 65504 + 65520) it becomes +-inf, so such an observation gives non-finite outputs -- as an infinity
+// does in fp32 -- instead of entering as the finite +-131008 a saturating x_lo would make of it.  65504 + inf and
+// inf + 0 give the same products (+-inf by the sign of the weight, NaN for a zero weight).
+__device__ __forceinline__ uint32_t pack_f16_lo(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
 __device__ __forceinline__ float2 unpack_f16(uint32_t h2) {
   return __half22float2(*reinterpret_cast<const __half2*>(&h2));
 }

@@ -356,7 +356,11 @@ ESTK_API int estk_shadow_bf16(estk_ctx* ctx, const float* src, uint16_t* dst, in
  *                    evaluates exactly the members the gradient estimate (estk_rank_grad*) weights.
  *                    Hidden activations are rounded to fp16 when written back (saturating at
  *                    +-65504), the observations enter as x_hi + x_lo (two fp16 operands), biases and
- *                    the squared error are fp32.  Population: table, table16.
+ *                    the squared error are fp32.  Finite observations keep ~22 significant bits up
+ *                    to |x| = 131008 (65504 + 65504; x_hi saturates, up to 131023 rounds to it); x_lo
+ *                    does not saturate, so +-inf -- and a finite |x| >= 131024, beyond the split's
+ *                    range -- enters with x_lo = +-inf and NaN as NaN: a non-finite observation gives
+ *                    the non-finite outputs FP32 gives.  Population: table, table16.
  *   ESTK_PREC_BF16   opt-in, lower precision: wgmma with bf16 operands, fp32 accumulation; weights
  *                    are rounded to bf16 when the B-operand tile is formed, activations when they
  *                    are written back.  Returns agree with FP32 to ~1e-2 relative.  Population: table.
