@@ -16,6 +16,8 @@ LIB_PATH = os.environ.get("ESTK_LIBRARY") or os.path.join(_HERE, "lib", "libestk
 
 ESTK_MAX_LAYERS = 8
 ESTK_MAX_POPULATION = 1 << 22
+# the longest noise table (entries) every kernel reads correctly; estk_make_offsets refuses longer ones
+ESTK_MAX_TABLE_LEN = 1 << 34
 # estk_mlp_desc.activation bit fields: hidden activation in bits 0-7, output activation in bits 8-15,
 # the loss in bits 16-23 (0: squared error; ESTK_ACTIONS: no return, the outputs on each member's own observations)
 ESTK_ACT_RELU = 0

@@ -210,8 +210,8 @@ extern "C" int estk_make_offsets(estk_ctx* ctx, uint64_t seed, const estk_state*
   ESTK_CHECK_ARG(n > 0 && pair_begin >= 0, "estk_make_offsets: bad n/pair_begin");
   const int64_t n_pad = (n + 31) / 32 * 32;
   ESTK_CHECK_ARG(table_len >= n_pad, "estk_make_offsets: table_len %lld < padded row %lld", (long long)table_len, (long long)n_pad);
-  ESTK_CHECK_ARG(table_len < (1ll << 40), "estk_make_offsets: table of %lld entries is too long (< 2^40)",
-                 (long long)table_len);
+  ESTK_CHECK_ARG(table_len <= ESTK_MAX_TABLE_LEN, "estk_make_offsets: table of %lld entries is longer than %lld",
+                 (long long)table_len, (long long)ESTK_MAX_TABLE_LEN);
   const uint64_t nslots = (uint64_t)((table_len - n_pad) / 32 + 1);
   if (order_out && pairs <= kBucketSortMax) {
     int sort_len = 1;

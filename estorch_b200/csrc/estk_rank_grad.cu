@@ -311,7 +311,6 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   __shared__ __align__(16) float s_w[kPairTile];
-  __shared__ __align__(16) uint32_t s_off4[kPairTile];
   __shared__ AdamScalars s_adam;
   extern __shared__ __align__(16) unsigned long long s_key_raw[];   // [P] keys, or the sort's scratch (SORT)
   uint64_t* s_key = reinterpret_cast<uint64_t*>(s_key_raw);
@@ -390,10 +389,11 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
     // fp16 table: a 128-bit load carries 8 noise values; same 16 loads in flight per thread, half the
     // bytes per pair row.  Columns are counted in vectors of 8 elements (p.n4 holds ceil(n/8) here).
     // The loop is issue-bound once the bytes are halved (ncu: 60 % issue-active), so it is written for
-    // instruction count: one mad.wide.u32 per address (32-bit byte offset of the pair row + this thread's
-    // 64-bit column base), pair offsets / weights fetched four at a time, two fp32 FMAs per instruction
+    // instruction count: one 64-bit add per address (64-bit byte offset of the pair row + this thread's 64-bit
+    // column base: any table length), pair offsets / weights fetched four at a time, two fp32 FMAs per instruction
     // (fma.rn.f32x2: each lane an IEEE fma, so the sums are bit-identical to the fp32-table kernel), and
     // the number of live columns of a thread resolved once per pair tile instead of once per load.
+    __shared__ __align__(16) uint64_t s_off[kPairTile];   // 64-bit byte offset of each staged pair's row
     const char* tabb = reinterpret_cast<const char*>(p.table16);
     for (int64_t cbase = c0; cbase < c1; cbase += (int64_t)kThreads * NC) {
       int64_t col[NC];
@@ -418,16 +418,12 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
           const int jl = p.order ? p.order[sbase + t] : (sbase + t);
           const int jg = p.pair_begin + jl;
           s_w[t] = __fsub_rn(__ldcg(p.cvals + jg), __ldcg(p.cvals + jg + p.pairs));
-          s_off4[t] = (uint32_t)(p.offsets[jl] << 1);       // BYTE offset of the row in the fp16 table (< 2^32)
+          s_off[t] = (uint64_t)p.offsets[jl] * 2;           // byte offset of the row in the fp16 table
         }
         __syncthreads();
         constexpr int U = LOADS / NC;
         static_assert(U % 4 == 0, "pair offsets / weights are fetched four at a time");
-        auto row = [](const char* base, uint32_t off) {
-          uint64_t r;
-          asm("mad.wide.u32 %0, %1, 1, %2;" : "=l"(r) : "r"(off), "l"(base));
-          return reinterpret_cast<const uint4*>(r);
-        };
+        auto row = [](const char* base, uint64_t off) { return reinterpret_cast<const uint4*>(base + off); };
         auto fma8 = [](float2 (&a)[4], float2 w, const uint4& t) {
           a[0] = ffma2(w, __half22float2(*reinterpret_cast<const __half2*>(&t.x)), a[0]);
           a[1] = ffma2(w, __half22float2(*reinterpret_cast<const __half2*>(&t.y)), a[1]);
@@ -441,8 +437,9 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
             uint4 t[U][NA];
 #pragma unroll
             for (int q = 0; q < U / 4; ++q) {
-              const uint4 o = *reinterpret_cast<const uint4*>(s_off4 + jj + 4 * q);
-              const uint32_t ov[4] = {o.x, o.y, o.z, o.w};
+              const ulonglong2 o01 = *reinterpret_cast<const ulonglong2*>(s_off + jj + 4 * q);
+              const ulonglong2 o23 = *reinterpret_cast<const ulonglong2*>(s_off + jj + 4 * q + 2);
+              const uint64_t ov[4] = {o01.x, o01.y, o23.x, o23.y};
 #pragma unroll
               for (int e = 0; e < 4; ++e)
 #pragma unroll
@@ -463,7 +460,7 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
           for (; jj < cnt; ++jj) {
             const float w = s_w[jj];
 #pragma unroll
-            for (int c = 0; c < NA; ++c) fma8(acc[c], make_float2(w, w), ld_noise4h(row(cb[c], s_off4[jj])));
+            for (int c = 0; c < NA; ++c) fma8(acc[c], make_float2(w, w), ld_noise4h(row(cb[c], s_off[jj])));
           }
         };
         static_assert(NC <= 2, "one loop body per possible number of live columns");
@@ -485,6 +482,9 @@ __global__ void __launch_bounds__(T, T == 256 ? 3 : 1) rank_grad_kernel(const Ra
       }
     }
   } else {
+  // fp32 table: each row as its 32-bit float4 index offsets[j] / 4, exact for every table of at most
+  // ESTK_MAX_TABLE_LEN = 2^34 entries (64-bit byte offsets here cost 1.7x the time at n = 1,001,760)
+  __shared__ __align__(16) uint32_t s_off4[kPairTile];
   const float4* tab4 = reinterpret_cast<const float4*>(p.table);
   for (int64_t cbase = c0; cbase < c1; cbase += (int64_t)kThreads * NC) {
     int64_t col[NC];

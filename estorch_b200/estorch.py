@@ -46,6 +46,7 @@ import numpy as np
 import torch
 
 from ._capi import ESTK_CONV_VBN_STATS_FLOATS, ESTK_LOSS_ACCURACY, ESTK_LOSS_XENT, ESTK_MAX_POPULATION
+from ._capi import ESTK_MAX_TABLE_LEN
 from .agents import DeviceAgent, PopulationAgent, SequenceAgent
 from .backend import adam_desc, new_state, read_state, write_state
 from .policy_spec import (CNNSpec, ConvVBNSpec, RNNSpec, cnn_spec_from_module, conv_vbn_spec_from_module,
@@ -242,7 +243,9 @@ class ES:
         sigma: noise standard deviation.
         device: device of the modules handed to a *host* agent's ``rollout``.
     Engine options (keyword-only, all optional):
-        noise_table_size: length of the shared unit-normal table (default 2**28).
+        noise_table_size: length of the shared unit-normal table (default 2**28), at most
+            ``ESTK_MAX_TABLE_LEN`` (2**34) entries; longer raises ``ValueError`` here.  The
+            table takes 4 bytes per entry on every GPU, plus 2 for its fp16 copy.
         noise_seed: seed of the table and of the per-generation offsets.
         log_interval: call ``log()`` every k-th generation only (default 1 =
             reference behaviour).
@@ -314,6 +317,9 @@ class ES:
                              f"{ESTK_MAX_POPULATION} members (ESTK_MAX_POPULATION)")
         if (self.population_size // 2) % self.n_workers:
             raise ValueError("population_size/2 antithetic pairs must divide evenly over the GPUs")
+        if noise_table_size is not None and int(noise_table_size) > ESTK_MAX_TABLE_LEN:
+            raise ValueError(f"noise_table_size {int(noise_table_size)} exceeds the engine's limit of "
+                             f"{ESTK_MAX_TABLE_LEN} entries (ESTK_MAX_TABLE_LEN)")
         self.device = torch.device(device)
         self.sigma = sigma
         self._stop = False

@@ -51,6 +51,10 @@ extern "C" {
 #define ESTK_VERSION 200          /* 0.2.0 */
 #define ESTK_MAX_LAYERS 8
 #define ESTK_MAX_POPULATION (1 << 22) /* P: 4,194,304 members */
+/* Longest noise table (entries) every kernel reads correctly: 2^34 (64 GiB in fp32).  estk_make_offsets refuses
+ * longer ones.  The fp32-table loop of estk_rank_grad* holds a row as its 32-bit float4 index offsets[j] / 4;
+ * every other table reader addresses a row with 64-bit arithmetic. */
+#define ESTK_MAX_TABLE_LEN (1ll << 34)
 
 typedef enum {
   ESTK_OK = 0,
@@ -293,7 +297,7 @@ ESTK_API int estk_fill_noise_table(estk_ctx* ctx, float* table, int64_t len, uin
  * generation's estk_track_best is still folded into this one -- and never a host scalar).  order_out (nullable, int32
  * [pairs]) receives the local pair indices sorted by offset (ties by index):
  * evaluating / reducing pairs in that order lets overlapping table rows hit L2.
- * pairs <= ESTK_MAX_POPULATION/2; table_len < 2^40.  Up to 4096 pairs one CTA sorts; more
+ * pairs <= ESTK_MAX_POPULATION/2; table_len <= ESTK_MAX_TABLE_LEN.  Up to 4096 pairs one CTA sorts; more
  * take one cooperative grid-wide radix sort (workspace in the context). */
 ESTK_API int estk_make_offsets(estk_ctx* ctx, uint64_t seed, const estk_state* state, int64_t gen_host,
                       int64_t pair_begin, int32_t pairs, int64_t table_len, int64_t n,
@@ -496,6 +500,8 @@ ESTK_API int estk_track_best(estk_ctx* ctx, estk_state* state, const float* rewa
  *   estorch.py:17-19,:176.  The gradient estimate is
  *     g = (1/P) * sum_j (c_j - c_{j+pairs}) * T[off_j : off_j+n]
  *   over pair j's offset offsets[j] (order, nullable = reduction order from estk_make_offsets).
+ *   Every offsets[j] is a multiple of 32, as estk_make_offsets makes them, and offsets[j] + n is at most the
+ *   table's length (<= ESTK_MAX_TABLE_LEN).
  *   The noise table: exactly one of `table` (fp32) and `table16` (the EXACT fp16 copy made by
  *   estk_shadow_f16: 8 noise values per 128-bit load, half the bytes per pair row, the same
  *   results because every fp16 value converts exactly to the fp32 value the table holds) is
